@@ -1,7 +1,7 @@
 """bench.py -- Sycamore n53 m20 sliced-contraction throughput (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W [--dtype complex128] [--impl reference]
-                    [--config m20|peps8x8|m10|m10s|m12] [--scaling weak|strong]
+                    [--config m20|peps8x8|m10|m10s|m12] [--scaling weak|strong] [--dump-outputs DIR]
 
 Default workload (config.workload): the reference's own benchmark structure
 ``examples/benchmarks/sycamore_n53_m20_s0_e0_pABCDCDAB.json`` (381 tensors, 754
@@ -23,12 +23,17 @@ whole job has 2^36 slices, so -- exactly as ``tree.benchmark()`` (core.py:4143-4
 The same JSON line also carries, at N = 1: the complex64 run of the same workload
 (``secondary``; BASELINE config 5 "complex64 vs complex128"), the GPU-library baseline
 SURVEY 2.3 asks for -- the reference's own dispatch for torch inputs, ``torch.tensordot``
-+ ``permute`` on the same B200 (``gpu_library_baseline``) --, a parity check of one slice
++ ``permute`` on the same GPU (``gpu_library_baseline``) --, a parity check of one slice
 against the CPU oracle's golden value at this very width (``parity``) and the CPU baseline.
 
 The reference arm (``--impl reference``) times the CPU restatement of the
 reference's numpy path (``oracle/``) on the host cores, on slices of the same
 network sliced further until a step fits host memory/time.
+
+``--dump-outputs DIR`` writes, after the timed steps, the result of the last timed step (the
+array ``contract_device`` returned) as ``DIR/out_<dtype>.npy``: float64 (complex128) or float32
+(complex64) with the real and imaginary parts in a trailing axis of 2.  The operands are seeded,
+so two builds run with the same arguments can be compared output for output.
 """
 
 import argparse
@@ -119,7 +124,7 @@ def measured_bf16():
             d = json.load(f)
         if "bf16_tflops" in d:
             return float(d["bf16_tflops"]), "MEASURED_PEAKS.json dense bf16 (cuBLAS, burst)"
-    return 2250.0, "nominal 2.25 PFLOP/s dense bf16 (MEASURED_PEAKS.json absent)"
+    return 989.0, "H100 SXM data sheet: 989 TFLOP/s dense bf16 (not measured; MEASURED_PEAKS.json absent)"
 
 
 def measured_peaks():
@@ -128,7 +133,7 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "MEASURED_PEAKS.json (driver-measured copy bandwidth)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md; MEASURED_PEAKS.json absent)"
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not measured; MEASURED_PEAKS.json absent)"
 
 
 class ClockSampler(threading.Thread):
@@ -344,7 +349,7 @@ def gpu_library_baseline(spec, tensors, flops_slice, reps=2, first_slice=0):
         return {
             "value": flops_slice / (ms * 1e-3) / 1e12, "unit": UNIT, "ms_per_slice": ms, "reps": reps,
             "impl": ("the reference's own dispatch for torch inputs (cotengra/contract.py:752-773): torch.tensordot + "
-                     "permute per node on the same B200 (cuBLAS GEMM behind permute/reshape copies); no kernel of "
+                     "permute per node on the same GPU (cuBLAS GEMM behind permute/reshape copies); no kernel of "
                      f"this repo involved (torch {torch.__version__})"),
             "peak_gib": peak,
             "_slice_value": complex(val.reshape(-1)[0].item()) if val.numel() == 1 else None,
@@ -419,6 +424,24 @@ def timed_run(ex, tensors, args, world, rank, dev, S, slice_ids=None):
     return {"ms": ms, "launches": launches, "node_ms": node_ms, "clocks": clocks, "out": out, "barrier": barrier}
 
 
+# at most 64 MB in all: a larger result is written as a fixed sample of its elements
+DUMP_MAX_ELEMS = 2**21
+
+
+def dump_output(args, out, rank):
+    """--dump-outputs: the result of the last timed step as DIR/out_<dtype>.npy (real view)."""
+    if not args.dump_outputs or rank != 0:
+        return
+    a = out.detach().cpu().numpy()
+    a = np.stack([a.real, a.imag], axis=-1) if np.iscomplexobj(a) else a
+    a = a.astype(np.float64 if a.dtype.itemsize >= 8 else np.float32)
+    if a.size > DUMP_MAX_ELEMS:
+        idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+        a = a.reshape(-1)[idx]
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    np.save(os.path.join(args.dump_outputs, f"out_{str(out.dtype).replace('torch.', '')}.npy"), a)
+
+
 def roofline_of(plan, node_ms, dtype, peaks):
     """Binding roofline of the dominant node of the last timed slice."""
     hbm_peak, hbm_src = measured_peaks()
@@ -428,18 +451,7 @@ def roofline_of(plan, node_ms, dtype, peaks):
     el = sum(int(np.prod(x.shape)) for x in (nd["a"], nd["b"], nd["c"]))
     node_flops = 8.0 * Bn * M * N * K
     node_bytes = el * plan.esize
-    traffic, traffic_src = None, None
-    for name in ("r02_top_kernel.json", "r01_top_kernel.json"):
-        tp = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tp):
-            with open(tp) as f:
-                rec = json.load(f).get(dtype, {})
-            # (only for the node the capture was taken on: other configurations have no capture)
-            if rec.get("dram_bytes_per_launch") and abs(rec.get("algorithmic_bytes", 0) - node_bytes) <= 1e-3 * node_bytes:
-                traffic = rec["dram_bytes_per_launch"]
-                traffic_src = (f"static: dram__bytes_read.sum + dram__bytes_write.sum of this node from the "
-                               f"ncu --set full capture recorded in profiles/{name} (not measured in this run)")
-                break
+    traffic, traffic_src = None, "not measured"
     fp64 = dtype in ("complex128", "float64")
     achieved_tf = node_flops / (t_ms * 1e-3) / 1e12
     achieved_gbs = node_bytes / (t_ms * 1e-3) / 1e9
@@ -448,7 +460,7 @@ def roofline_of(plan, node_ms, dtype, peaks):
         tensor_src = ("fp64 DMMA microbenchmark run in this process (ctgb_probe_fp64_peaks); "
                       "MEASURED_PEAKS.json holds no fp64 figure")
     else:
-        # complex64 runs as three kind::tf32 passes over the real embedding (8C real flops each):
+        # complex64 runs as three tf32 wgmma passes over the real embedding (8C real flops each):
         # effective peak = dense TF32 peak / 3, dense TF32 = half the measured dense bf16 figure
         bf16, bf16_src = measured_bf16()
         tensor_peak = bf16 / 2.0 / 3.0
@@ -510,6 +522,7 @@ def run_gpu(args):
     ex.workspace(host_staging=True)  # allocate once, outside the timed region
 
     r = timed_run(ex, tensors, args, world, rank, dev, S)
+    dump_output(args, r["out"], rank)
     ms, launches, node_ms, clocks, out, barrier = (r[k] for k in ("ms", "launches", "node_ms", "clocks", "out", "barrier"))
     macs_ref, _macs_inv, elems_ref = ex.reference_work
     flops_slice = 8 * macs_ref
@@ -552,6 +565,7 @@ def run_gpu(args):
         ex64 = cb.TreeExecutor(spec, dtype="complex64", device=local, fuse=not args.no_fuse)
         t64 = [t.to(torch.complex64) for t in tensors]
         r64 = timed_run(ex64, t64, args, world, rank, dev, S)
+        dump_output(args, r64["out"], rank)
         m64, _i64, _e64 = ex64.reference_work
         v64 = 8 * m64 * total_slices / (r64["ms"] * 1e-3) / 1e12
         if rank == 0:
@@ -633,7 +647,7 @@ def run_gpu(args):
             if tv is not None:
                 parity["vs_torch_rel_err"] = abs(got - tv) / abs(tv)
             if "value" in gpu_lib:
-                gpu_lib["b200_speedup"] = value / gpu_lib["value"]
+                gpu_lib["speedup"] = value / gpu_lib["value"]
 
     cpu = None
     if world == 1 and not args.no_cpu and args.config == "m20":
@@ -688,6 +702,8 @@ def main():
     ap.add_argument("--no-secondary", action="store_true", help="skip the complex64 leg")
     ap.add_argument("--no-gpu-lib", action="store_true", help="skip the torch.tensordot GPU-library baseline")
     ap.add_argument("--no-fuse", action="store_true", help="execute the reference's node sequence one to one")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's result as DIR/out_<dtype>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-"""cotengra_b200 -- B200-native executor for cotengra's sliced contraction trees.
+"""cotengra_b200 -- H100-native executor for cotengra's sliced contraction trees.
 
 The drop-in for ONE path of jcmgray/cotengra: ``ContractionTree.contract()`` ->
 per-slice ``Contractor`` node loop -> pairwise tensordot/einsum

@@ -96,7 +96,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -c 'import "
-            "__graft_entry__ as g; g.build()'` (nvcc, sm_100a). cotengra_b200 "
+            "__graft_entry__ as g; g.build()'` (nvcc, sm_90a). cotengra_b200 "
             "has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
@@ -166,5 +166,5 @@ def launch_count() -> int:
 
 
 def tensor_map_launches() -> int:
-    """tcgen05 launches so far whose A tiles were fetched by tensor-map TMA."""
+    """wgmma launches so far whose A tiles were fetched by tensor-map TMA."""
     return int(load().ctgb_tensor_map_launches())

@@ -1,5 +1,5 @@
 """Reference-facing host API: the same names, argument meaning and error
-behaviour as cotengra's execution path, backed by the sm_100a kernels.
+behaviour as cotengra's execution path, backed by the sm_90a kernels.
 
     einsum(eq, a, b=None) ............ cotengra/contract.py:414
     tensordot(a, b, axes) ............ cotengra/contract.py:521
@@ -47,7 +47,7 @@ def _torch():
 
     if not torch.cuda.is_available():
         raise RuntimeError(
-            "cotengra_b200 needs a CUDA device (sm_100a); there is no CPU fallback"
+            "cotengra_b200 needs a CUDA device (sm_90a); there is no CPU fallback"
         )
     return torch
 
@@ -657,7 +657,7 @@ def make_contractor(tree, strip_exponent=False, check_zero=False, **_ignored):
 
 def install(tree, strip_exponent=False, check_zero=False):
     """Route ``tree.contract(...)`` / ``tree.contract_slice(...)`` of a live
-    cotengra tree through the B200 contractor by seeding its contractor cache
+    cotengra tree through this package's contractor by seeding its contractor cache
     (core.py:3699-3711).  Key order: ``(autojit, order, prefer_einsum,
     strip_exponent, check_zero, implementation, progbar)``.  Call after the tree
     is final: slicing/reconfiguration clears the cache (core.py:2040, 2087)."""

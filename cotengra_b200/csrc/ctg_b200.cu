@@ -64,7 +64,7 @@ DevInfo& devinfo() {
       d.minor = p.minor;
       d.smem_optin = p.sharedMemPerBlockOptin;
       cached_dev = dev;
-      // the tcgen05 launches take their B' scratch from the stream-ordered pool: keep freed
+      // the wgmma launches take their B' scratch from the stream-ordered pool: keep freed
       // blocks cached across synchronisation points instead of returning them to the driver
       cudaMemPool_t pool;
       if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
@@ -270,7 +270,7 @@ int launch_dmmastream(const int64_t* h, const int64_t* d, const void* A, const v
 
 std::atomic<int64_t> g_tmap_launches{0};
 
-// Tensor map for the A tile of the tcgen05 kernel.  The tile is described in A's memory order by
+// Tensor map for the A tile of the wgmma kernel.  The tile is described in A's memory order by
 // the descriptor's load list (ext, stride), smallest stride first; adjacent entries that continue
 // each other coalesce into box dims.  If at most four box dims remain, the innermost is contiguous
 // and everything is 16-byte granular, ONE cp.async.bulk.tensor fetches the tile: dims 0..n-1 are
@@ -359,7 +359,7 @@ int tc05_make_tensor_map(const int64_t* h, const void* A, CUtensorMap* tm) {
   return rc == CUDA_SUCCESS ? nb + 1 : 0;
 }
 
-// complex64 on tcgen05: prepare B' (hi/lo, tile order) once, then the warp-specialised kernel
+// complex64 on wgmma: prepare B' (hi/lo, tile order) once, then the warp-specialised kernel
 template <int NT>
 int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
   using Cfg = Tc05Cfg<NT>;
@@ -373,7 +373,7 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
       !exact(W_PGM, W_MFULL, W_MTEXT) || !exact(W_PGN, W_NFULL, W_NTEXT) || !exact(W_PGK, W_KFULL, W_KTEXT) ||
       h[W_STEPS_K] > TC05_KTAB || h[W_LBOPAD] < 0 || h[W_LBOPAD] > 4 ||
       ((h[W_FLAGS] & 64) && (h[W_RUNA] < 16 || (h[W_MTA] * h[W_KTA]) % h[W_RUNA] != 0)))
-    return fail(CTGB_E_VALUE, "descriptor does not fit the tcgen05 kernel");
+    return fail(CTGB_E_VALUE, "descriptor does not fit the wgmma kernel");
   const uint64_t work = (uint64_t)h[W_TILES_M] * (uint64_t)h[W_TILES_N] * (uint64_t)h[W_TILES_B] * (uint64_t)h[W_SPLITK];
   if (work == 0) return CTGB_OK;
   if (work >= (1ull << 31)) return fail(CTGB_E_VALUE, "too many tiles for one launch");
@@ -381,9 +381,7 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   int dev;
   cudaGetDevice(&dev);
   if (attr_dev != dev) {
-    CUDA_TRY(cudaFuncSetAttribute(tc05_kernel<NT, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)di.smem_optin - 1024));
-    CUDA_TRY(cudaFuncSetAttribute(tc05_kernel<NT, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CUDA_TRY(cudaFuncSetAttribute(tc05_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)di.smem_optin - 1024));
     attr_dev = dev;
   }
@@ -402,14 +400,14 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   }
   long long sa = (pool - nb * Cfg::PAIR_BYTES) / ((long long)Cfg::A_TILE * 8);
   if (sa > Cfg::SA_MAX) sa = Cfg::SA_MAX;
-  if (sa < 2) return fail(CTGB_E_CUDA, "tcgen05 kernel needs more shared memory than the device offers");
+  if (sa < 2) return fail(CTGB_E_CUDA, "wgmma kernel needs more shared memory than the device offers");
   if (grid > work) {
     grid = work;
     if (b_stat && grid % (uint64_t)tiles_n != 0) b_stat = 0, nb = nb < 3 ? 3 : nb;  // tiny launch: plain ring
   }
   const size_t smem = Cfg::smem_bytes((int)sa, (int)nb);
   if (smem + 1024 > di.smem_optin)
-    return fail(CTGB_E_CUDA, "tcgen05 kernel needs more shared memory than the device offers");
+    return fail(CTGB_E_CUDA, "wgmma kernel needs more shared memory than the device offers");
 
   const unsigned long long tiles = (unsigned long long)h[W_TILES_B] * h[W_TILES_N] * h[W_STEPS_K];
   const size_t bytes = (size_t)tiles * Cfg::PAIR_BYTES;
@@ -433,15 +431,8 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   static const bool tm_off = getenv("CTGB_NO_TENSOR_MAP") != nullptr;
   const int tm_rank = tm_off ? 0 : tc05_make_tensor_map(h, A, &tm);
   if (tm_rank) g_tmap_launches.fetch_add(1, std::memory_order_relaxed);
-  // the lean epilogue: 32-byte quads of a dense, aligned C, no accumulation (see tc05_kernel.cuh)
-  const bool lean = (h[W_FLAGS] & 16) && !(h[W_FLAGS] & 1) && h[W_SPLITK] == 1 &&
-                    (reinterpret_cast<unsigned long long>(C) & 31ull) == 0;
-  if (lean)
-    tc05_kernel<NT, 0><<<(unsigned)grid, Cfg::THREADS, smem, st>>>(d, (const float2*)A, Bp, (float2*)C, (unsigned)sa,
-                                                                    (unsigned)nb, b_stat, tm, tm_rank);
-  else
-    tc05_kernel<NT, 1><<<(unsigned)grid, Cfg::THREADS, smem, st>>>(d, (const float2*)A, Bp, (float2*)C, (unsigned)sa,
-                                                                    (unsigned)nb, b_stat, tm, tm_rank);
+  tc05_kernel<NT><<<(unsigned)grid, Cfg::THREADS, smem, st>>>(d, (const float2*)A, Bp, (float2*)C, (unsigned)sa,
+                                                              (unsigned)nb, b_stat, tm, tm_rank);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
   cudaFreeAsync(Bp, st);
@@ -515,9 +506,10 @@ template <typename T>
 int launch_single_typed(const int64_t* h, const int64_t* d, const void* X, void* out, cudaStream_t st) {
   long long n = h[S_OUT_ELEMS];
   if (n <= 0) return CTGB_OK;
+  const long long cap = (long long)(devinfo().ok ? devinfo().sms : 132) * 16;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
-  if (h[S_SUM_ELEMS] >= 1024 && n <= 148 * 16) {
+  if (blocks > cap) blocks = cap;
+  if (h[S_SUM_ELEMS] >= 1024 && n <= cap) {
     // few outputs over a long summed range: one block per output element
     single_reduce_kernel<T><<<(unsigned)n, 256, 0, st>>>(d, (const T*)X, (T*)out);
   } else {
@@ -539,8 +531,9 @@ int launch_single(const int64_t* h, const int64_t* d, const void* X, void* out, 
 }
 
 unsigned flat_grid(long long n) {
+  const long long cap = (long long)(devinfo().ok ? devinfo().sms : 132) * 8;
   long long b = (n + 255) / 256;
-  if (b > 148 * 8) b = 148 * 8;
+  if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (unsigned)b;
 }
@@ -783,7 +776,7 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
       const int64_t* w = n.desc;
       q.measure_after = w[W_SPLITK] > 1 || w[W_VARIANT] == VAR_DOTSTREAM || w[W_VARIANT] == VAR_DOTSTREAM4;
       // (the block-reduction epilogue of KRED runs once: its result is measured afterwards as well;
-      // so is a tcgen05 node whose contracted range is folded into C chunk by chunk)
+      // so is a wgmma node whose contracted range is folded into C chunk by chunk)
       q.measure_after |= w[W_VARIANT] == VAR_KRED;
       q.measure_after |= (w[W_VARIANT] == VAR_TC05_128x64 || w[W_VARIANT] == VAR_TC05_128x32 ||
                           w[W_VARIANT] == VAR_TC05_128x16) &&

@@ -4,11 +4,11 @@
 // Every warp owns blocks of 32 output rows and runs them start to finish on its own:
 // A fragments straight from global memory into registers (a lane of the m8k4 A fragment
 // holds one complex element: one LDG.128, 16 of them in flight per lane), B fragments from
-// a zero-padded shared-memory copy made once per CTA, 4 real DMMAs per fragment pair, 256-bit
+// a zero-padded shared-memory copy made once per CTA, 4 real DMMAs per fragment pair, 128-bit
 // stores.  No operand staging, no producer warps, no CTA barriers in the loop: the warps of
 // an SM drift apart, so loads, DMMAs and stores of different row blocks overlap by themselves
 // -- which the staged 256x16 policy could not do (all consumer warps share one phase: ncu
-// showed its N=16 K=16 node at 3.3 TB/s, compute and HBM time adding up instead of overlapping).
+// showed its N=16 K=16 node with compute and HBM time adding up instead of overlapping).
 // (included inside namespace ctgb)
 #pragma once
 

@@ -2,7 +2,7 @@
 // out = sum_k A[k] * B[k] over two operands of up to 2^30 elements whose index orders differ.
 //
 // The staged KRED policy moves every element with its own cp.async; for 8-byte types that
-// is one LSU wavefront per lane (3.5 TB/s for complex64, ncu: LSU bound).  Here a thread
+// is one LSU wavefront per lane (LSU bound for complex64).  Here a thread
 // owns the same DS_U tile-local elements of every 2048-element tile: their offsets in A and
 // in B (the tile dims' digits times the strides) are launch-invariant and live in registers,
 // the tile base (grid dims) is computed once per tile by each warp (one lane per grid dim +
@@ -18,7 +18,7 @@ constexpr int DOT_KT = 2048, DOT_THREADS = 256, DOT_U = DOT_KT / DOT_THREADS;
 // of a stem peeled over the final inner product (cotengra_b200/fusion.py),
 //   R[m, n] = sum_k A[k, m] * B[k, n],
 // 16 accumulators per thread, 4 k per thread and tile (16 + 16 loads in flight: 128 KB per SM,
-// what the 1x1 kernel needs for 6.9 TB/s; with 2 k it stopped at 5.6 TB/s)
+// what the 1x1 kernel needs to stream at HBM rate; 2 k per thread were measurably slower)
 constexpr int DOT4_MN = 4;
 // k per thread and tile: 4 for 16-byte elements, 8 for narrower ones (the same 128 KB in flight)
 template <typename T> constexpr int dot4_u() { return sizeof(T) >= 16 ? 4 : 8; }

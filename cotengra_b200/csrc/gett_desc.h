@@ -40,8 +40,8 @@ enum : int {
                        // bit2: tile-grid extents are powers of two; bit3: all m dims are powers of two
   W_VARIANT = 32,      // kernel variant chosen by the host
   W_CELEMS = 33,       // elements of a dense C (memset before split-K atomics); 0: strided C
-  W_RUNA = 34,         // tcgen05: elements of the contiguous runs the A tile is made of (flags bit6)
-  W_LBOPAD = 35,       // tcgen05: chunk-stride padding of the A' images, x16 bytes (bank spreading)
+  W_RUNA = 34,         // wgmma: elements of the contiguous runs the A tile is made of (flags bit6)
+  W_LBOPAD = 35,       // wgmma: chunk-stride padding of the A' images, x16 bytes (bank spreading)
   // fused strip_exponent (contract.py:816-829), patched into the plan's device copy of the
   // descriptor by ctgb_plan_create; 0 = off.  Device addresses of doubles:
   W_SCALE_A = 36,      //   max|A| of operand A as stored (A is a lazily-normalised intermediate) or 1.0
@@ -74,7 +74,7 @@ enum : int {
   VAR_ROW_128x8 = 6,   // one output row per thread (HBM-bound skinny nodes), N <= 8
   VAR_ROW_256x4 = 7,   // same, N <= 4 (fewer registers -> more resident CTAs)
   VAR_ROWSTREAM = 8,   // N, K <= 8, exact tiles, no batch: thread-per-row straight from global memory
-  VAR_TC05_128x64 = 9, // complex64, exact 128 x 64 x 16 tiles: tcgen05.mma kind::tf32 (3 passes), TMEM accumulators
+  VAR_TC05_128x64 = 9, // complex64, exact 128 x 64 x 16 tiles: wgmma tf32 (3 passes), register accumulators
   VAR_TC05_128x32 = 10,
   VAR_TC05_128x16 = 11,
   VAR_DMMA3M_128x32 = 12,  // complex128, 3M complex product (three DMMAs per fragment pair)

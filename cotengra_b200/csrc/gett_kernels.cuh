@@ -1,4 +1,4 @@
-// gett_kernels.cuh -- permutation-fused pairwise tensor contraction for sm_100a.
+// gett_kernels.cuh -- permutation-fused pairwise tensor contraction for sm_90a.
 //
 // Replaces cotengra/contract.py:364-411 (`_do_contraction_via_bmm`: transpose ->
 // reshape(copy) -> matmul -> reshape/transpose) by ONE kernel:
@@ -60,15 +60,16 @@ __device__ __forceinline__ void atomic_add_of(double2* p, double2 v) {
   atomicAdd(&p->y, v.y);
 }
 
-// two adjacent elements with one store; 256-bit (STG.E.ENL2.256) for complex128
+// two adjacent elements (sm_90 has no 256-bit global store: complex128 takes two 128-bit ones)
 template <typename T>
 __device__ __forceinline__ void store_pair_of(T* p, T v0, T v1) {
   p[0] = v0;
   p[1] = v1;
 }
-template <>
-__device__ __forceinline__ void store_pair_of<double2>(double2* p, double2 v0, double2 v1) {
-  asm volatile("st.global.v4.f64 [%0], {%1,%2,%3,%4};" ::"l"(p), "d"(v0.x), "d"(v0.y), "d"(v1.x), "d"(v1.y)
+// four adjacent 8-byte elements (32-byte aligned) as two 128-bit stores
+__device__ __forceinline__ void st_quad8(void* p, const unsigned long long* q) {
+  asm volatile("st.global.v2.b64 [%0], {%1,%2};\n\tst.global.v2.b64 [%0+16], {%3,%4};" ::"l"(p), "l"(q[0]), "l"(q[1]),
+               "l"(q[2]), "l"(q[3])
                : "memory");
 }
 
@@ -133,7 +134,7 @@ __device__ __forceinline__ StripCtx strip_begin(const int64_t* __restrict__ D) {
 // their bit patterns, so an element whose larger component lies below (current maximum)/sqrt(2) is
 // dismissed with four ALU instructions and touches neither the fp64 pipe the DMMAs run on nor the
 // instruction cache (with the arithmetic inlined at each of the 32-64 store sites of an unrolled
-// epilogue the DMMA nodes lost 18 %, the tcgen05 nodes 60 %: instruction fetch).  The rare candidates
+// epilogue the DMMA and tensor-core nodes lost to instruction fetch).  The rare candidates
 // call ONE out-of-line routine: re^2 + im^2 against the running maximum of squares (square root taken
 // once at the end); squares that would leave the double range, and NaNs, take a hypot path with its own
 // maximum, so that magnitudes down to the denormals survive.
@@ -444,7 +445,7 @@ struct RowPolicy {
     for (int h = 0; h < 2; ++h) {
       const int r = (int)threadIdx.x + h * THREADS;
       if (pair_ok) {
-        // the row's columns are adjacent in C: 32-byte (256-bit) stores, full sectors
+        // the row's columns are adjacent in C: 32-byte runs as two 128-bit stores, full sectors
 #pragma unroll
         for (int j = 0; j < NT; j += 2) {
           if (j >= ncols) break;
@@ -461,9 +462,9 @@ struct RowPolicy {
   }
 };
 
-// fp64 tensor-core policy: mma.sync.aligned.m8n8k4 (DMMA).  tcgen05 has no f64
-// kind (cute/arch/mma_sm100_umma.hpp exposes f16/tf32/f8f6f4/i8/mx* only), so
-// the double-precision tensor path on sm_100a is the warp-level DMMA.
+// fp64 tensor-core policy: mma.sync.aligned.m8n8k4 (DMMA).  wgmma has no f64
+// kind (f16/bf16/tf32/fp8/int8 only), so the double-precision tensor path on
+// sm_90a is the warp-level DMMA.
 // Complex products are four real DMMAs per (A-frag, B-frag) pair:
 //   Cr += Ar*Br;  Cr += (-Ai)*Bi;  Ci += Ar*Bi;  Ci += Ai*Br
 // or, with M3 ("3M", the ZGEMM3M identity), three:
@@ -604,7 +605,7 @@ struct DmmaPolicy {
         const int r = (wm * FM + i) * 8 + frow;
         const int c = (wn * FN + j) * 8 + fc;
         if constexpr (CPLX) {
-          // a lane owns two adjacent columns of the fragment: one 256-bit store
+          // a lane owns two adjacent columns of the fragment: one 128-bit store
           if (pair_ok) {
             store_pair(r, c, make_double2(acc.re[i][j][0], acc.im[i][j][0]),
                        make_double2(acc.re[i][j][1], acc.im[i][j][1]));

@@ -2,10 +2,10 @@
 // one output row per thread, operands read straight from global memory
 // (coalesced 128-bit loads when consecutive rows are adjacent in A, which the
 // host's dim ordering arranges), the small operand held in registers or
-// broadcast from shared memory, 256-bit stores.  No shared-memory staging and
+// broadcast from shared memory, 128-bit stores.  No shared-memory staging and
 // no producer warps: HBM-bound nodes want LSU wavefronts and instructions per
 // row at the minimum and many resident warps to cover latency (ncu showed the
-// staged row policy at 61-69 % LSU data-pipe utilisation, 4.4 TB/s).
+// staged row policy bound by the LSU data pipe).
 // (included inside namespace ctgb)
 #pragma once
 
@@ -27,7 +27,7 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
   const bool accumulate = (D[W_FLAGS] & 1) != 0;
   const bool pair_ok = (D[W_FLAGS] & 2) != 0 && !accumulate && sizeof(T) == 16;
   // 8-byte elements: bit4 = groups of four columns are adjacent and 32-byte aligned,
-  // bit5 = pairs of columns adjacent and 16-byte aligned -> 256-/128-bit row stores
+  // bit5 = pairs of columns adjacent and 16-byte aligned -> 2 x 128-bit / 128-bit row stores
   [[maybe_unused]] const bool quad8 = (D[W_FLAGS] & 16) != 0 && !accumulate && sizeof(T) == 8;
   [[maybe_unused]] const bool pair8 = (D[W_FLAGS] & 32) != 0 && !accumulate && sizeof(T) == 8;
   const bool pow2 = (D[W_FLAGS] & 8) != 0;  // every m dim (tile and grid) is a power of two
@@ -187,9 +187,7 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
             for (int c = 0; c + 3 < CH; c += 4)
               if (c0 + c < N) {
                 const unsigned long long* q = reinterpret_cast<const unsigned long long*>(&acc[c]);
-                asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(pc + s_cnoff[c0 + c]), "l"(q[0]), "l"(q[1]),
-                             "l"(q[2]), "l"(q[3])
-                             : "memory");
+                st_quad8(pc + s_cnoff[c0 + c], q);
               }
             done = true;
           } else if (pair8) {
@@ -373,9 +371,7 @@ rowstream_longk_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, c
           for (int c = 0; c + 3 < RSK_NMAX; c += 4)
             if (c < N) {
               const unsigned long long* q = reinterpret_cast<const unsigned long long*>(&acc[i][c]);
-              asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(pc + s_cnoff[c]), "l"(q[0]), "l"(q[1]), "l"(q[2]),
-                           "l"(q[3])
-                           : "memory");
+              st_quad8(pc + s_cnoff[c], q);
             }
           done = true;
         }

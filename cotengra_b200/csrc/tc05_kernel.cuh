@@ -1,50 +1,46 @@
-// tc05_kernel.cuh -- complex64 dense nodes on the 5th-generation tensor cores
-// (tcgen05.mma kind::tf32, accumulators in TMEM).  Included inside namespace ctgb,
-// after gett_ws.cuh (mbarrier helpers) and tc05_policy.cuh (bprime_kernel, descriptors).
+// tc05_kernel.cuh -- complex64 dense nodes on the Hopper tensor cores (wgmma kind tf32,
+// accumulators in registers).  Included inside namespace ctgb, after gett_ws.cuh (mbarrier
+// helpers) and tc05_policy.cuh (bprime_kernel, descriptors).
 //
 // A complex tile product C[128 x NT] += A[128 x 16] * B[16 x NT] runs as the real
 // product C'[128 x 2NT] += A'[128 x 32] * B'[2NT x 32]^T (tc05_policy.cuh); the 3xTF32 split
-// (hi*hi + lo*hi + hi*lo) takes two UMMAs per k8 because B'hi and B'lo are stacked along N.  The CTA is specialised into four roles that only meet at
-// mbarriers:
+// (hi*hi + lo*hi + hi*lo) takes two wgmmas per k8 because B'hi and B'lo are stacked along N.
+// The CTA is three warpgroups that only meet at mbarriers:
 //
-//   warps  8-11  A producers   the A tile of a k-step is fetched in A's MEMORY order
-//                              into a staging ring (SA deep, 16 KB each): ONE tensor-map TMA
-//                              copy (cp.async.bulk.tensor, a <= 4-D box of A's coalesced dims +
-//                              an offset dim) when the tile is such a box; else TMA bulk copies
-//                              of whole contiguous runs (cp.async.bulk + complete_tx) when
-//                              the tile is made of runs >= 128 B, an 8-byte cp.async
-//                              gather otherwise.  The ring only holds raw data, so it is
-//                              deep enough to cover HBM latency.
-//   warp   12    B' producer   one TMA bulk copy per k-step of the prepared B'hi|B'lo
-//                              pair (ring of NB slots fed from L2; when all the B' tiles a
-//                              CTA ever needs fit the ring they are loaded once and stay).
-//   warps  0-3   scatter       staging -> A'hi / A'lo in UMMA's K-major core-matrix
-//                              layout (double buffered A' images).
-//   warp   13    MMA issuer    a whole warp runs the issue loop with warp-uniform control
-//                              flow (descriptors stay in uniform registers); one elected
-//                              lane issues the 8 UMMAs of a k-step and commits them to the
-//                              "operand free", "B' slot free" and (last step) "accumulator
-//                              full" barriers.  Kept apart from the scatter warps: the
-//                              issue sequence costs ~1300 clk per step when it runs
-//                              divergently inside them (ncu, profiles/).
-//   warps  4-7   epilogue      TMEM -> registers -> C (32-byte row sectors) for tile j-1
-//                              while the MMAs of tile j run (two TMEM accumulators).
+//   warps  8-11  producer      fetches the A tile of a k-step in A's MEMORY order into a
+//                              staging ring (SA deep, 16 KB each): ONE tensor-map TMA copy
+//                              (cp.async.bulk.tensor, a <= 4-D box of A's coalesced dims + an
+//                              offset dim) when the tile is such a box; else TMA bulk copies of
+//                              whole contiguous runs (cp.async.bulk + complete_tx) when the tile
+//                              is made of runs >= 128 B, an 8-byte cp.async gather otherwise.
+//                              The loads run SA steps ahead of the scatter: staging -> A'hi /
+//                              A'lo in wgmma's K-major core-matrix layout (double-buffered A'
+//                              images).  One thread also streams the prepared B'hi|B'lo pair
+//                              of every k-step into a ring of NB slots with one TMA bulk copy
+//                              (when all the B' tiles a CTA ever needs fit the ring they are
+//                              loaded once and stay).
+//   warps  0-3   consumer 0    rows 0-63 of the tile, warps 4-7 (consumer 1) rows 64-127: each
+//                              warpgroup issues the wgmmas of a k-step into its register
+//                              accumulator (2NT floats a thread: [A'hi B'hi | A'hi B'lo +
+//                              A'lo B'hi]), commits a k-step and waits for the one before it, and
+//                              stores the finished accumulation into C.  (ptxas serialises the
+//                              wgmmas of this kernel (C7511); a setmaxnreg split that removes that
+//                              spills and halved complex64 throughput on H100, so it is not used.)
 //
-// The scatter map (element of the staging tile -> UMMA position) is the same for every
-// stage and lives in registers.  The chunk stride (LBO) of the A' images is padded by
+// The scatter map (element of the staging tile -> position in the A' image) is the same for
+// every stage and lives in registers.  The chunk stride (LBO) of the A' images is padded by
 // D[W_LBOPAD] x 16 B, chosen by the host so that the 16 lanes of a half warp -- 16
 // consecutive elements of A's memory order -- hit 16 different 8-byte bank pairs.
 #pragma once
 
-// k-steps (of 16) accumulated in ONE TMEM accumulation: a contracted range of up to 16 steps (K <= 256,
-// every dense Sycamore node) is a single accumulation.  Longer ranges are folded into C by the epilogue
-// chunk by chunk with round-to-nearest adds; the read-modify-write of a chunk hits the C tile the same
-// CTA wrote a moment ago, i.e. L2.  (4-step chunks were measured too: 42.5 instead of 18.6 ms on the
-// bond-6 PEPS tree for no gain in accuracy -- its error came from the truncating operand split.)
+// k-steps (of 16) accumulated in ONE register accumulation: a contracted range of up to 16 steps
+// (K <= 256, every dense Sycamore node) is a single accumulation.  Longer ranges are folded into C
+// chunk by chunk with round-to-nearest adds; the read-modify-write of a chunk hits the C tile the
+// same thread wrote a moment ago, i.e. L2.
 constexpr int TC05_CHUNK = 16;
 // ... balanced (17 full steps are 9 + 8), and shorter in k8 accumulations for tiles with a shorter k (12 on
-// 6^n extents: 12 steps = 36 accumulations): those trees are deep chains of dependent nodes, and with 54
-// accumulations per chunk the bond-6 PEPS amplitude came out at 1.09e-5 instead of 8.8e-6
+// 6^n extents: 12 steps = 36 accumulations): those trees are deep chains of dependent nodes, where the
+// truncating accumulation of long chunks shows in the amplitude's error
 __host__ __device__ inline unsigned tc05_chunk_steps(unsigned steps, unsigned nq) {
   const unsigned cap = nq >= 4u ? (unsigned)TC05_CHUNK : 36u / (nq ? nq : 1u);
   const unsigned n = (steps + cap - 1) / cap;
@@ -62,30 +58,16 @@ struct Tc05Cfg {
   static constexpr int A_TILE = MT * KT;                   // float2 elements of one staged A tile
   static constexpr int LBO_BASE = MT * 16;                 // bytes between k chunks of A' (unpadded)
   static constexpr int OP_BYTES = 8 * (LBO_BASE + 64);     // one A' image with the largest padding
-  static constexpr int TMEM_COLS = 4 * NT;                 // fp32 columns of one accumulator: [A'hi B'hi | A'hi B'lo + A'lo B'hi]
-  // tile-info ring.  With one k-step per tile the A producer runs ahead of the epilogue by the staging
-  // ring (SA) + the scatter of 2 tiles (operand double buffer) + 2 accumulations in TMEM, and it writes
-  // the NEXT tile's entry before it blocks: SA + 5 entries are live.  (SA + 4 was a race on store-bound
-  // single-step nodes, M = 2^25 x 32 x 16: a tile now and then went to another tile's C address.)
-  static constexpr int TI = SA_MAX + 8;
-  static constexpr int NBARS = 2 * SA_MAX + 2 * NB_MAX + 2 + 2 + 4;
-  static constexpr int THREADS = 14 * 32;
-  static_assert(TMEM_COLS == 64 || TMEM_COLS == 128 || TMEM_COLS == 256,
-                "two accumulators: a power of two >= 32 columns each, <= 512 together");
+  static constexpr int NBARS = SA_MAX + 2 * NB_MAX + 2 + 2;
+  static constexpr int THREADS = 3 * 128;
+  static_assert(NT == 16 || NT == 32 || NT == 64, "wgmma N = 4NT must be 64, 128 or 256");
   static constexpr size_t fixed_bytes() {  // everything but the two rings
-    return 4 * (size_t)OP_BYTES + 8 * (size_t)(MT + NT + TC05_KTAB + 4 * TI + NBARS) + 128;
+    return 4 * (size_t)OP_BYTES + 8 * (size_t)(MT + NT + TC05_KTAB + NBARS) + 128;
   }
   static constexpr size_t smem_bytes(int sa, int nb) {
     return fixed_bytes() + (size_t)sa * A_TILE * 8 + (size_t)nb * PAIR_BYTES;
   }
 };
-
-// one lane of a converged warp (the compiler keeps the surrounding code warp-uniform)
-__device__ __forceinline__ bool elect_one() {
-  unsigned pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}\n" : "=r"(pred));
-  return pred != 0;
-}
 
 // ring position + phase bit of an mbarrier ring
 struct RingPos {
@@ -98,17 +80,62 @@ struct RingPos {
   }
 };
 
+// ---- wgmma (sm_90a): D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 operands K-major in shared memory
+__device__ __forceinline__ void wgmma_tf32_n32(float* d, uint64_t da, uint64_t db, unsigned acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float* d, uint64_t da, uint64_t db, unsigned acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float* d, uint64_t da, uint64_t db, unsigned acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n256(float* d, uint64_t da, uint64_t db, unsigned acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(acc));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db, unsigned acc) {
+  if constexpr (N == 32) wgmma_tf32_n32(d, da, db, acc);
+  else if constexpr (N == 64) wgmma_tf32_n64(d, da, db, acc);
+  else if constexpr (N == 128) wgmma_tf32_n128(d, da, db, acc);
+  else wgmma_tf32_n256(d, da, db, acc);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accesses of an accumulator across the asynchronous wgmmas
+__device__ __forceinline__ void reg_fence(float& x) { asm volatile("" : "+f"(x)::"memory"); }
+
 // SA: depth of the A staging ring.  NB: slots of the B' ring.  b_stat: the B' tiles of this
 // CTA never change (one batch, grid a multiple of tiles_n, steps_k <= NB): they are
 // loaded once into slot = k-step and stay resident.
-template <int NT, int EPI>
-__global__ void __launch_bounds__(448, 1)
+template <int NT>
+__global__ void __launch_bounds__(384, 1)
 tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const float* __restrict__ Bp,
             float2* __restrict__ C, const unsigned SA, const unsigned NB, const int b_stat,
             const __grid_constant__ CUtensorMap tmA, const int tm_rank) {
   using Cfg = Tc05Cfg<NT>;
-  constexpr int MT = Cfg::MT, TI = Cfg::TI, A_TILE = Cfg::A_TILE;
-  constexpr int GROUP = 128;  // threads of the scatter group / of the A producers
+  constexpr int MT = Cfg::MT, A_TILE = Cfg::A_TILE;
+  constexpr int GROUP = 128;  // threads of the producer warpgroup
   extern __shared__ __align__(128) unsigned char tc05_smem[];
   unsigned char* smem_raw = tc05_smem;
   float2* stg = reinterpret_cast<float2*>(smem_raw);                  // [SA][A_TILE], memory order
@@ -117,16 +144,11 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
   long long* offMC = reinterpret_cast<long long*>(sB + (size_t)NB * Cfg::PAIR_BYTES);
   long long* offNC = offMC + MT;
   long long* kbA = offNC + NT;
-  long long* ti_base = kbA + TC05_KTAB;  // [TI][4]: A base, -, C base, -
-  unsigned long long* stg_full = reinterpret_cast<unsigned long long*>(ti_base + 4 * TI);
-  unsigned long long* stg_empty = stg_full + Cfg::SA_MAX;
-  unsigned long long* b_full = stg_empty + Cfg::SA_MAX;
+  unsigned long long* stg_full = reinterpret_cast<unsigned long long*>(kbA + TC05_KTAB);
+  unsigned long long* b_full = stg_full + Cfg::SA_MAX;
   unsigned long long* b_empty = b_full + Cfg::NB_MAX;
-  unsigned long long* op_empty = b_empty + Cfg::NB_MAX;  // [2] one tcgen05.commit
-  unsigned long long* op_full = op_empty + 2;    // [2] four scatter warps
-  unsigned long long* tmem_full = op_full + 2;   // [2] one tcgen05.commit
-  unsigned long long* tmem_empty = tmem_full + 2;  // [2] four epilogue warps
-  __shared__ unsigned tmem_slot;
+  unsigned long long* op_full = b_empty + Cfg::NB_MAX;  // [2] four producer warps
+  unsigned long long* op_empty = op_full + 2;           // [2] eight consumer warps
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
@@ -143,10 +165,10 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
   // actual tile extents: full 128 x NT x 16 on power-of-two networks; on others (PEPS bond 6) the
   // host picks exact divisors of the index extents, so every tile has the SAME smaller shape --
   // rows >= MTa and columns >= NTa of the operand images are padding that the epilogue ignores
-  // (B' is zero there), k >= KTa costs nothing: the UMMAs of the missing k8 groups are not issued
+  // (B' is zero there), k >= KTa costs nothing: the wgmmas of the missing k8 groups are not issued
   const unsigned MTa = (unsigned)D[W_MTA], NTa = (unsigned)D[W_NTA], KTa = (unsigned)D[W_KTA];
   const unsigned a_elems = MTa * KTa;       // elements of one staged A tile
-  const unsigned nq = KTa >> 2;             // UMMA k8 groups per k-step (KTa is a multiple of 4)
+  const unsigned nq = KTa >> 2;             // k8 groups per k-step (KTa is a multiple of 4)
   // flags bit6: the A tile is made of contiguous runs of run_a elements (>= 128 B, even offsets)
   const bool bulk_a = (D[W_FLAGS] & 64) != 0 && (reinterpret_cast<unsigned long long>(A) & 15ull) == 0;
   const unsigned lbo_a = (unsigned)Cfg::LBO_BASE + 16u * (unsigned)D[W_LBOPAD];
@@ -178,22 +200,15 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
 
   // ---- one-time tables ----
   if (tid == 0) {
-    for (unsigned s = 0; s < SA; ++s) {
-      mbar_init(&stg_full[s], GROUP);
-      mbar_init(&stg_empty[s], 4);
-    }
+    for (unsigned s = 0; s < SA; ++s) mbar_init(&stg_full[s], GROUP);
     for (unsigned s = 0; s < NB; ++s) {
       mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
+      mbar_init(&b_empty[s], 8);
     }
-    mbar_init(&op_empty[0], 1);
-    mbar_init(&op_empty[1], 1);
     mbar_init(&op_full[0], 4);
     mbar_init(&op_full[1], 4);
-    mbar_init(&tmem_full[0], 1);
-    mbar_init(&tmem_full[1], 1);
-    mbar_init(&tmem_empty[0], 4);
-    mbar_init(&tmem_empty[1], 4);
+    mbar_init(&op_empty[0], 8);
+    mbar_init(&op_empty[1], 8);
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   if (tid < 256) {
@@ -219,7 +234,7 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
       }
       offNC[c] = o;
     }
-  } else if (tid < 384) {
+  } else {
     // A base offset of every k-step (the host guarantees steps_k <= TC05_KTAB)
     for (unsigned s = tid - 256; s < steps_k; s += GROUP) {
       long long a = 0;
@@ -230,16 +245,7 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
       kbA[s] = a;
     }
   }
-  if (warp == 0) {
-    const unsigned a = (unsigned)__cvta_generic_to_shared(&tmem_slot);
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(a), "r"(2 * Cfg::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const unsigned taddr = tmem_slot;
 
   // the host guarantees total_work < 2^31
   const unsigned tiles_all = tiles_m * tiles_n * tiles_b;
@@ -268,9 +274,34 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
       ib_ = t / tiles_m;
     }
   };
+  // base offsets of work item j's tile in A and C (every lane of a converged warp)
+  auto tile_bases = [&](unsigned j, long long& a, long long& c) {
+    unsigned in_, im_, ib_;
+    work_tile(j, in_, im_, ib_);
+    a = 0;
+    c = 0;
+    for (int q = lane; q < n_gm; q += 32) {
+      const int64_t* G = D + OFF_GM + q * 4;
+      const unsigned dig = digit_of(im_, (unsigned)G[1], (unsigned)G[0]);
+      a += (long long)dig * G[2];
+      c += (long long)dig * G[3];
+    }
+    for (int q = lane; q < n_gn; q += 32) {
+      const int64_t* G = D + OFF_GN + q * 4;
+      c += (long long)digit_of(in_, (unsigned)G[1], (unsigned)G[0]) * G[3];
+    }
+    for (int q = lane; q < n_gb; q += 32) {
+      const int64_t* G = D + OFF_GB + q * 5;
+      const unsigned dig = digit_of(ib_, (unsigned)G[1], (unsigned)G[0]);
+      a += (long long)dig * G[2];
+      c += (long long)dig * G[4];
+    }
+    a = warp_sum_ll(a);
+    c = warp_sum_ll(c);
+  };
 
-  if (warp >= 8 && warp < 12) {
-    // ===================================================== A PRODUCERS
+  if (warp >= 8) {
+    // ===================================================== PRODUCER WARPGROUP
     const int ptid = tid - 256;
     const unsigned nruns = bulk_a ? a_elems / run_a : 0u;  // <= 128: run_a >= 16
     constexpr int NG = A_TILE / GROUP;
@@ -279,51 +310,48 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
     for (int i = 0; i < NG; ++i)
       goff[i] = (bulk_a || (unsigned)(ptid + i * GROUP) >= a_elems) ? 0ll : a_off((unsigned)(ptid + i * GROUP));
     if (bulk_a && (unsigned)ptid < nruns) goff[0] = a_off((unsigned)ptid * run_a);
-    RingPos ra;
-    for (unsigned j = 0; j < nw; ++j) {
-      unsigned k0, k1;
-      work_krange(j, k0, k1);
-      const int slot = (int)(j % TI);
-      if (ptid < 32) {
-        unsigned in_, im_, ib_;
-        work_tile(j, in_, im_, ib_);
-        long long a = 0, c = 0;
-        for (int q = lane; q < n_gm; q += 32) {
-          const int64_t* G = D + OFF_GM + q * 4;
-          const unsigned dig = digit_of(im_, (unsigned)G[1], (unsigned)G[0]);
-          a += (long long)dig * G[2];
-          c += (long long)dig * G[3];
+    unsigned upos[NG];
+#pragma unroll
+    for (int i = 0; i < NG; ++i)
+      upos[i] = (unsigned)(ptid + i * GROUP) < a_elems ? a_pos((unsigned)(ptid + i * GROUP)) : 0xFFFFFFFFu;
+
+    // load cursor (A): work item lj, k-step ls of [ls, le); tile base ltA
+    unsigned lj = 0, ls = 0, le = 0, issued = 0;
+    bool lstart = true;
+    long long ltA = 0;
+    RingPos rl;
+    // B' cursor: work item bj, k-step bs of [bs, be)
+    unsigned bj = 0, bs = 0, be = 0, b_issued = 0;
+    bool bstart = true;
+    unsigned long long btile = 0;
+    RingPos rbp;
+    const unsigned nwb = b_stat ? min(nw, 1u) : nw;  // resident B': loaded with the first work item only
+    // the pair is chunk-major (k'/4 outermost): a tile with fewer than 16 k uses a PREFIX of it, and only
+    // that is fetched (12 k on 6^n extents: 24 of 32 KB)
+    const unsigned pair_bytes = 2u * nq * (4u * NT) * 16u;
+
+    RingPos rs;
+    for (unsigned g = 0;; ++g) {
+      // A loads run SA steps ahead: the slot of step g + SA - 1 was scattered (and released by the
+      // barrier below) in iteration g - 1
+      while (issued < g + SA) {
+        while (ls >= le) {
+          if (!lstart) ++lj;
+          lstart = false;
+          if (lj >= nw) break;
+          work_krange(lj, ls, le);
+          long long c;
+          tile_bases(lj, ltA, c);
         }
-        for (int q = lane; q < n_gn; q += 32) {
-          const int64_t* G = D + OFF_GN + q * 4;
-          c += (long long)digit_of(in_, (unsigned)G[1], (unsigned)G[0]) * G[3];
-        }
-        for (int q = lane; q < n_gb; q += 32) {
-          const int64_t* G = D + OFF_GB + q * 5;
-          const unsigned dig = digit_of(ib_, (unsigned)G[1], (unsigned)G[0]);
-          a += (long long)dig * G[2];
-          c += (long long)dig * G[4];
-        }
-        a = warp_sum_ll(a);
-        c = warp_sum_ll(c);
-        if (lane == 0) {
-          ti_base[slot * 4 + 0] = a;
-          ti_base[slot * 4 + 2] = c;
-          __threadfence_block();
-        }
-      }
-      named_sync<1, GROUP>();
-      const long long tA = ti_base[slot * 4 + 0];
-      for (unsigned step = k0; step < k1; ++step, ra.next(SA)) {
-        const unsigned sa = ra.idx;
-        mbar_wait(&stg_empty[sa], ra.ph ^ 1);
-        const float2* src = A + tA + kbA[step];
+        if (lj >= nw) break;
+        const unsigned sa = rl.idx, step = ls;
+        const float2* src = A + ltA + kbA[step];
         float2* dst = stg + (size_t)sa * A_TILE;
         const unsigned bar = (unsigned)__cvta_generic_to_shared(&stg_full[sa]);
         if (tm_rank) {
-          // ONE tensor-map TMA copy per k-step (cp.async.bulk.tensor, SASS UTMALDG): the tile is a
-          // box of up to four coalesced dims of A in memory order, its position the coordinate of a
-          // fifth "offset" dim of stride 16 bytes (tc05_make_tensor_map)
+          // ONE tensor-map TMA copy per k-step: the tile is a box of up to four coalesced dims of A in
+          // memory order, its position the coordinate of a fifth "offset" dim of stride 16 bytes
+          // (tc05_make_tensor_map)
           const unsigned bytes = ptid == 0 ? a_elems * 8u : 0u;
           asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}\n" ::"r"(bar),
                        "r"(bytes)
@@ -331,7 +359,7 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
           if (ptid == 0) {
             const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
             const unsigned long long tm = reinterpret_cast<unsigned long long>(&tmA);
-            const int c = (int)((unsigned long long)(tA + kbA[step]) >> 1);  // 16-byte units
+            const int c = (int)((unsigned long long)(ltA + kbA[step]) >> 1);  // 16-byte units
             if (tm_rank == 2)
               asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(d), "l"(tm), "r"(0), "r"(c), "r"(bar) : "memory");
             else if (tm_rank == 3)
@@ -360,30 +388,31 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
             if ((unsigned)(ptid + i * GROUP) < a_elems) cp_async_zfill<8>(dst + ptid + i * GROUP, src + goff[i], true);
           mbar_arrive_cp_async(&stg_full[sa]);
         }
+        ++ls;
+        ++issued;
+        rl.next(SA);
       }
-    }
-    cp_async_commit();
-    cp_async_wait<0>();  // do not exit with copies in flight
-  } else if (warp == 12) {
-    // ===================================================== B' PRODUCER
-    if (lane == 0) {
-      RingPos rb;
-      const unsigned nwb = b_stat ? min(nw, 1u) : nw;  // resident B': loaded with the first work item only
-      // the pair is chunk-major (k'/4 outermost): a tile with fewer than 16 k uses a PREFIX of it, and only
-      // that is fetched (12 k on 6^n extents: 24 of 32 KB -- B' is 3/4 of what the TMA unit moves on the
-      // 46656 x 1296 x 1296 PEPS node, whose 108 k-steps cannot stay resident)
-      const unsigned pair_bytes = 2u * nq * (4u * NT) * 16u;
-      for (unsigned j = 0; j < nwb; ++j) {
-        unsigned k0, k1, in_, im_, ib_;
-        work_krange(j, k0, k1);
-        work_tile(j, in_, im_, ib_);
-        const unsigned long long tile = (unsigned long long)ib_ * tiles_n + in_;
-        for (unsigned step = k0; step < k1; ++step, rb.next(NB)) {
-          const unsigned sb = rb.idx;
-          mbar_wait(&b_empty[sb], rb.ph ^ 1);
+      if (g >= issued) break;  // every k-step of every work item is scattered
+
+      // B' pairs: up to step g + NB - 2 (its slot was freed with step g - 2, which the scatter below
+      // waits for anyway); resident B' is loaded in the first iteration
+      if (ptid == 0) {
+        while (b_stat ? b_issued < NB : b_issued + 1 < g + NB) {
+          while (bs >= be) {
+            if (!bstart) ++bj;
+            bstart = false;
+            if (bj >= nwb) break;
+            work_krange(bj, bs, be);
+            unsigned in_, im_, ib_;
+            work_tile(bj, in_, im_, ib_);
+            btile = (unsigned long long)ib_ * tiles_n + in_;
+          }
+          if (bj >= nwb) break;
+          const unsigned sb = rbp.idx;
+          if (!b_stat) mbar_wait(&b_empty[sb], rbp.ph ^ 1);
           const unsigned bar = (unsigned)__cvta_generic_to_shared(&b_full[sb]);
           const unsigned dst = (unsigned)__cvta_generic_to_shared(sB + (size_t)sb * Cfg::PAIR_BYTES);
-          const char* src = reinterpret_cast<const char*>(Bp) + (tile * steps_k + step) * (unsigned long long)Cfg::PAIR_BYTES;
+          const char* src = reinterpret_cast<const char*>(Bp) + (btile * steps_k + bs) * (unsigned long long)Cfg::PAIR_BYTES;
           asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}\n" ::"r"(bar),
                        "r"(pair_bytes)
                        : "memory");
@@ -391,380 +420,157 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
               "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(dst),
               "l"(src), "r"(pair_bytes), "r"(bar)
               : "memory");
+          ++bs;
+          ++b_issued;
+          rbp.next(NB);
         }
       }
-    }
-  } else if (warp < 4) {
-    // ===================================================== SCATTER GROUP
-    constexpr int NSCAT = A_TILE / GROUP;
-    unsigned upos[NSCAT];
+
+      // scatter step g: staging -> A'hi / A'lo
+      const unsigned sa = rs.idx, ob = g & 1;
+      float2* hi2 = reinterpret_cast<float2*>(op + (size_t)(ob * 2) * Cfg::OP_BYTES);
+      float2* lo2 = reinterpret_cast<float2*>(op + (size_t)(ob * 2 + 1) * Cfg::OP_BYTES);
+      const float2* src = stg + (size_t)sa * A_TILE;
+      mbar_wait(&op_empty[ob], ((g >> 1) & 1) ^ 1);  // the wgmmas of step g-2 have read these images
+      mbar_wait(&stg_full[sa], rs.ph);
+      // all loads first: the compiler cannot prove the A' images do not alias the staging
+      // tile and would otherwise serialise LDS -> STS -> LDS ...
+      float2 v[NG];
 #pragma unroll
-    for (int i = 0; i < NSCAT; ++i)
-      upos[i] = (unsigned)(tid + i * GROUP) < a_elems ? a_pos((unsigned)(tid + i * GROUP)) : 0xFFFFFFFFu;
-    unsigned g = 0;
-    RingPos ra;
-    for (unsigned j = 0; j < nw; ++j) {
-      unsigned k0, k1;
-      work_krange(j, k0, k1);
-      for (unsigned step = k0; step < k1; ++step, ++g, ra.next(SA)) {
-        const unsigned sa = ra.idx, ob = g & 1;
-        float2* hi2 = reinterpret_cast<float2*>(op + (size_t)(ob * 2) * Cfg::OP_BYTES);
-        float2* lo2 = reinterpret_cast<float2*>(op + (size_t)(ob * 2 + 1) * Cfg::OP_BYTES);
-        const float2* src = stg + (size_t)sa * A_TILE;
-        mbar_wait(&op_empty[ob], ((g >> 1) & 1) ^ 1);  // the UMMAs of step g-2 have read these images
-        mbar_wait(&stg_full[sa], ra.ph);
-        // all loads first: the compiler cannot prove the A' images do not alias the staging
-        // tile and would otherwise serialise LDS -> STS -> LDS ...
-        float2 v[NSCAT];
+      for (int i = 0; i < NG; ++i) v[i] = upos[i] != 0xFFFFFFFFu ? src[ptid + i * GROUP] : make_float2(0.f, 0.f);
 #pragma unroll
-        for (int i = 0; i < NSCAT; ++i) v[i] = upos[i] != 0xFFFFFFFFu ? src[tid + i * GROUP] : make_float2(0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < NSCAT; ++i) {
-          if (upos[i] != 0xFFFFFFFFu) {
+      for (int i = 0; i < NG; ++i) {
+        if (upos[i] != 0xFFFFFFFFu) {
 #ifdef CTGB_TC05_TRUNC_SPLIT  // A/B knob: the cheaper truncating split (biased, see tc05_policy.cuh)
-            hi2[upos[i]] = v[i];
-            lo2[upos[i]] = make_float2(v[i].x - trunc_tf32(v[i].x), v[i].y - trunc_tf32(v[i].y));
+          hi2[upos[i]] = v[i];
+          lo2[upos[i]] = make_float2(v[i].x - trunc_tf32(v[i].x), v[i].y - trunc_tf32(v[i].y));
 #else
-            const float2 h = make_float2(round_tf32(v[i].x), round_tf32(v[i].y));
-            hi2[upos[i]] = h;
-            lo2[upos[i]] = make_float2(half_up_tf32(v[i].x - h.x), half_up_tf32(v[i].y - h.y));
+          const float2 h = make_float2(round_tf32(v[i].x), round_tf32(v[i].y));
+          hi2[upos[i]] = h;
+          lo2[upos[i]] = make_float2(half_up_tf32(v[i].x - h.x), half_up_tf32(v[i].y - h.y));
 #endif
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // generic-proxy writes -> tensor core
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&stg_empty[sa]);  // this warp's reads of the staging tile are done
-          mbar_arrive(&op_full[ob]);    // ... and its part of the A' images is written
         }
       }
+      // generic-proxy writes (and reads of the staging slot) -> tensor core / TMA
+      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&op_full[ob]);
+      named_sync<1, GROUP>();  // the staging slot is refilled in the next iteration
+      rs.next(SA);
     }
-  } else if (warp == 13) {
-    // ===================================================== MMA ISSUER (warp-uniform loop)
-    // InstrDescriptor: D=f32 [4,6)=1, A=tf32 [7,10)=2, B=tf32 [10,13)=2, K-major A/B, N>>3 [17,23), M>>4 [24,29)
-    // Two instructions per k8 instead of three passes: B'hi and B'lo are stacked along N, so
-    //   [P | Q] (4NT columns)  = A'hi x [B'hi ; B'lo]^T      (A'hi is read from shared memory once)
-    //        Q  (2NT columns) += A'lo x  B'hi^T
-    // and the epilogue adds the small terms Q to P.  Both corrections go to Q because the tensor
-    // core truncates its accumulator after every instruction: P, the one that carries the magnitude,
-    // then sees ONE truncation per k8 (measured shrink of a K = 36 node: 6.7e-7 with two).
-    constexpr unsigned idesc_wide =
-        (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)((4 * NT) >> 3) << 17) | ((unsigned)(MT >> 4) << 24);
-    constexpr unsigned idesc_half =
-        (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)((2 * NT) >> 3) << 17) | ((unsigned)(MT >> 4) << 24);
-    const unsigned op_base = (unsigned)__cvta_generic_to_shared(op);
+    cp_async_commit();
+    cp_async_wait<0>();  // do not exit with copies in flight
+  } else {
+    // ===================================================== CONSUMER WARPGROUPS
+    const int wg = warp >> 2;
+    // accumulator: [P | Q], P = A'hi B'hi (NT floats), Q = A'hi B'lo + A'lo B'hi (NT floats).  Thread
+    // (warp w of the group, lane l) holds rows 64wg + 16(w%4) + l/4 (+8) and complex columns 4i + l%4
+    float acc[2 * NT];
+#pragma unroll
+    for (int i = 0; i < 2 * NT; ++i) acc[i] = 0.f;
+    const unsigned op_base = (unsigned)__cvta_generic_to_shared(op) + (unsigned)wg * 1024u;  // 8 row groups x 128 B
     const unsigned b_base = (unsigned)__cvta_generic_to_shared(sB);
-    unsigned g = 0, acq = 0;  // acq: accumulations started (TMEM buffer = acq & 1)
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cl = lane & 3;
+    const bool row_ok0 = (unsigned)r0 < MTa, row_ok1 = (unsigned)(r0 + 8) < MTa;
+    const long long row_off0 = row_ok0 ? offMC[r0] : 0ll, row_off1 = row_ok1 ? offMC[r0 + 8] : 0ll;
+    StripCtx sctx = strip_begin(D);  // fused strip_exponent
+    unsigned g = 0;
     RingPos rb;
+    auto release = [&](unsigned ob, unsigned sb) {
+      if (lane == 0) {
+        mbar_arrive(&op_empty[ob]);
+        if (!b_stat) mbar_arrive(&b_empty[sb]);
+      }
+    };
     for (unsigned j = 0; j < nw; ++j) {
       unsigned kb, ke;
       work_krange(j, kb, ke);
+      long long a_unused, cbase;
+      tile_bases(j, a_unused, cbase);
       // a contracted range longer than TC05_CHUNK k-steps (K > 256) is accumulated chunk by chunk:
-      // every chunk starts a fresh TMEM accumulation, the epilogue folds it into C with
-      // round-to-nearest adds (the tensor core's own accumulation truncates)
-      for (unsigned k0 = kb; k0 < ke; k0 += chunk, ++acq) {
-      const unsigned k1 = min(ke, k0 + chunk);
-      const unsigned buf = acq & 1;
-      mbar_wait(&tmem_empty[buf], ((acq >> 1) & 1) ^ 1);  // the epilogue two accumulations back has drained it
-      for (unsigned step = k0; step < k1; ++step, ++g, rb.next(NB)) {
-        const unsigned ob = g & 1, sb = b_stat ? step : rb.idx;
-        mbar_wait(&op_full[ob], (g >> 1) & 1);
-        if (!b_stat) {
-          mbar_wait(&b_full[sb], rb.ph);
-        } else if (j == 0) {
-          mbar_wait(&b_full[sb], 0);  // resident B': filled once
-        }
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const unsigned a_hi = op_base + (ob * 2) * (unsigned)Cfg::OP_BYTES, a_lo = a_hi + (unsigned)Cfg::OP_BYTES;
-        const unsigned b_all = b_base + sb * (unsigned)Cfg::PAIR_BYTES;
-        const unsigned dcol = taddr + buf * Cfg::TMEM_COLS;
-        if (elect_one()) {
+      // every chunk starts a fresh accumulation, the epilogue folds it into C with round-to-nearest
+      // adds (the tensor core's own accumulation truncates)
+      for (unsigned k0 = kb; k0 < ke; k0 += chunk) {
+        const unsigned k1 = min(ke, k0 + chunk);
+        unsigned prev_ob = 0, prev_sb = 0;
+        for (unsigned step = k0; step < k1; ++step, ++g, rb.next(NB)) {
+          const unsigned ob = g & 1, sb = b_stat ? step : rb.idx;
+          mbar_wait(&op_full[ob], (g >> 1) & 1);
+          if (!b_stat) {
+            mbar_wait(&b_full[sb], rb.ph);
+          } else if (j == 0) {
+            mbar_wait(&b_full[sb], 0);  // resident B': filled once
+          }
+          const unsigned a_hi = op_base + (ob * 2) * (unsigned)Cfg::OP_BYTES, a_lo = a_hi + (unsigned)Cfg::OP_BYTES;
+          const unsigned b_all = b_base + sb * (unsigned)Cfg::PAIR_BYTES;
+#pragma unroll
+          for (int i = 0; i < 2 * NT; ++i) reg_fence(acc[i]);
+          wgmma_fence();
+          // Two instructions per k8 instead of three passes: B'hi and B'lo are stacked along N, so
+          //   [P | Q] (4NT columns)  = A'hi x [B'hi ; B'lo]^T      (A'hi is read from shared memory once)
+          //        Q  (2NT columns) += A'lo x  B'hi^T
+          // and the epilogue adds the small terms Q to P.  Both corrections go to Q because the tensor
+          // core truncates its accumulator after every instruction: P, the one that carries the
+          // magnitude, then sees ONE truncation per k8.
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             if ((unsigned)q >= nq) break;  // (uniform) a tile with fewer than 16 k
-            // one UMMA eats K = 8 floats = 2 chunks; chunk stride = LBO, 8-row group stride (SBO) = 128 B
-            const uint64_t d_hi = umma_desc_kmajor(a_hi + q * 2 * lbo_a, lbo_a, 128);
-            const uint64_t d_lo = umma_desc_kmajor(a_lo + q * 2 * lbo_a, lbo_a, 128);
-            const uint64_t d_b = umma_desc_kmajor(b_all + q * 2 * (4 * NT) * 16, (4 * NT) * 16, 128);
-            const unsigned acc = (step != k0 || q != 0) ? 1u : 0u;
-            asm volatile(
-                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(dcol),
-                "l"(d_hi), "l"(d_b), "r"(idesc_wide), "r"(acc)
-                : "memory");
-            asm volatile(
-                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(dcol + 2 * NT),
-                "l"(d_lo), "l"(d_b), "r"(idesc_half), "r"(1u)
-                : "memory");
+            // one wgmma eats K = 8 floats = 2 chunks; chunk stride = LBO, 8-row group stride (SBO) = 128 B
+            const uint64_t d_hi = gmma_desc_kmajor(a_hi + q * 2 * lbo_a, lbo_a, 128);
+            const uint64_t d_lo = gmma_desc_kmajor(a_lo + q * 2 * lbo_a, lbo_a, 128);
+            const uint64_t d_b = gmma_desc_kmajor(b_all + q * 2 * (4 * NT) * 16, (4 * NT) * 16, 128);
+            wgmma_tf32<4 * NT>(acc, d_hi, d_b, (step != k0 || q != 0) ? 1u : 0u);
+            wgmma_tf32<2 * NT>(acc + NT, d_lo, d_b, 1u);
           }
-          const unsigned m_op = (unsigned)__cvta_generic_to_shared(&op_empty[ob]);
-          asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(m_op)
-                       : "memory");
-          if (!b_stat) {
-            const unsigned m_b = (unsigned)__cvta_generic_to_shared(&b_empty[sb]);
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(m_b)
-                         : "memory");
-          }
-          if (step + 1 == k1) {
-            const unsigned mf = (unsigned)__cvta_generic_to_shared(&tmem_full[buf]);
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(mf)
-                         : "memory");
-          }
+          wgmma_commit();
+#pragma unroll
+          for (int i = 0; i < 2 * NT; ++i) reg_fence(acc[i]);
+          // the operands of the previous k-step are free once it is done
+          wgmma_wait<1>();
+          if (step != k0) release(prev_ob, prev_sb);
+          prev_ob = ob;
+          prev_sb = sb;
         }
-        __syncwarp();
-      }
-      }
-    }
-  } else if (warp < 8) {
-    // ===================================================== EPILOGUE GROUP (warps 4-7)
-    const bool quad_ok = (D[W_FLAGS] & 16) != 0 && !accumulate && !atomic &&
-                         (reinterpret_cast<unsigned long long>(C) & 31ull) == 0;
-    // (an even but not fourfold tile width, 54 columns on 6^n extents: 16-byte pairs)
-    const bool pair_ok = (D[W_FLAGS] & 32) != 0 && !accumulate && !atomic &&
-                         (reinterpret_cast<unsigned long long>(C) & 15ull) == 0;
-    const int quad = warp & 3;  // TMEM lane quadrant of this warp
-    const int r = quad * 32 + lane;
-    const bool row_ok = (unsigned)r < MTa;  // padding rows hold whatever the A' images held
-    const long long row_off = row_ok ? offMC[r] : 0ll;
-    StripCtx sctx = strip_begin(D);  // fused strip_exponent
-    unsigned acq = 0;
-    for (unsigned j = 0; j < nw; ++j) {
-      unsigned kb, ke;
-      work_krange(j, kb, ke);
-      for (unsigned k0 = kb; k0 < ke; k0 += chunk, ++acq) {
-      const unsigned buf = acq & 1;
-      // a later chunk of the same tile adds to what the first one stored (accumulating and split-K
-      // launches add every chunk to C anyway)
-      const bool fold = k0 != kb && !accumulate && !atomic;
-      mbar_wait(&tmem_full[buf], (acq >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-      float2* crow = C + ti_base[(j % TI) * 4 + 2] + row_off;
-      // Two epilogues, chosen by the launcher (template parameter EPI): the lean one -- 32-byte quads of a
-      // dense, aligned, non-accumulating C, every dense Sycamore node -- and the general one (16-byte
-      // pairs or single elements, accumulating / split-K launches, and the folds of long contracted
-      // ranges prefetched per column group).  In ONE kernel the general paths cost the single-step
-      // nodes 14 % (instruction fetch: 99 -> 85 TFLOP/s on M = 2^15, N = 1024, K = 64).
-      if constexpr (EPI == 0) {
-        const bool rmw = fold;
-        // 32 fp32 columns (16 complex) per tcgen05.ld: one TMEM round trip per 128 bytes of a row
-#pragma unroll 1
-        for (int col = 0; col < 2 * NT; col += 32) {
-          unsigned v[32];
-          const unsigned ta = taddr + buf * Cfg::TMEM_COLS + ((unsigned)(quad * 32) << 16) + (unsigned)col;
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-              "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-              : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-              : "r"(ta));
-          // the small terms A'hi B'lo + A'lo B'hi sit 2NT columns further
-          unsigned u[32];
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-              "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-              : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]), "=r"(u[8]),
-                "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]), "=r"(u[16]),
-                "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]), "=r"(u[24]),
-                "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-              : "r"(ta + 2u * NT));
-          asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+        wgmma_wait<0>();
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(u[i]));
-          if (sctx.on && row_ok) {
-            if (sctx.scale) {
+        for (int i = 0; i < 2 * NT; ++i) reg_fence(acc[i]);
+        release(prev_ob, prev_sb);
+
+        // ---- epilogue: registers -> C ----
+        // a later chunk of the same tile adds to what the first one stored (accumulating and split-K
+        // launches add every chunk to C anyway)
+        const bool fold = k0 != kb && !accumulate && !atomic;
+        float2* crow0 = C + cbase + row_off0;
+        float2* crow1 = C + cbase + row_off1;
 #pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                const float2 z = strip_apply(sctx, make_float2(__uint_as_float(v[i]), __uint_as_float(v[i + 1])));
-                v[i] = __float_as_uint(z.x);
-                v[i + 1] = __float_as_uint(z.y);
-              }
-            } else {
-              // max|C|: integer scan over the 32 words, then (rarely) the values (see gett_ws.cuh)
-              int hmax = 0;
+        for (int i = 0; i < NT / 4; ++i) {
+          const unsigned n = (unsigned)(4 * i + cl);
 #pragma unroll
-              for (int i = 0; i < 32; ++i) hmax = max(hmax, (int)(v[i] & 0x7fffffffu));
-              if (strip_hot<float2>(sctx, hmax)) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) strip_track_f(sctx, __uint_as_float(v[i]), __uint_as_float(v[i + 1]));
+          for (int h = 0; h < 2; ++h) {
+            const bool ok = (h ? row_ok1 : row_ok0) && n < NTa;
+            float2 val = make_float2(acc[4 * i + 2 * h] + acc[NT + 4 * i + 2 * h],
+                                     acc[4 * i + 2 * h + 1] + acc[NT + 4 * i + 2 * h + 1]);
+            if (!ok) continue;
+            if (sctx.on) {
+              if (sctx.scale) {
+                val = strip_apply(sctx, val);
+              } else if (strip_hot<float2>(sctx, strip_hi(val))) {
+                strip_track_f(sctx, val.x, val.y);
               }
             }
-          }
-#pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4) {  // groups of 4 complex columns
-            const int c0 = (col >> 1) + s4 * 4;
-            const unsigned* w = v + s4 * 8;
-            if (!row_ok || (unsigned)c0 >= NTa) continue;
-            if (quad_ok && (unsigned)c0 + 3 < NTa) {
-              unsigned x[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) x[e] = w[e];
-              if (rmw) {
-                // same thread, same addresses as the chunk before: program order makes the sum visible
-                unsigned long long p0, p1, p2, p3;
-                asm volatile("ld.global.v4.b64 {%0,%1,%2,%3}, [%4];\n" : "=l"(p0), "=l"(p1), "=l"(p2), "=l"(p3) : "l"(crow + offNC[c0]) : "memory");
-                const unsigned long long pp[4] = {p0, p1, p2, p3};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  x[2 * e] = __float_as_uint(__uint_as_float(x[2 * e]) + __uint_as_float((unsigned)pp[e]));
-                  x[2 * e + 1] = __float_as_uint(__uint_as_float(x[2 * e + 1]) + __uint_as_float((unsigned)(pp[e] >> 32)));
-                }
-              }
-              const unsigned long long q0 = ((unsigned long long)x[1] << 32) | x[0], q1 = ((unsigned long long)x[3] << 32) | x[2];
-              const unsigned long long q2 = ((unsigned long long)x[5] << 32) | x[4], q3 = ((unsigned long long)x[7] << 32) | x[6];
-              asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};\n" ::"l"(crow + offNC[c0]), "l"(q0), "l"(q1), "l"(q2),
-                           "l"(q3)
-                           : "memory");
+            float2* p = (h ? crow1 : crow0) + offNC[n];
+            if (atomic) {
+              atomic_add_of(p, val);
+            } else if (accumulate || fold) {  // (after the strip scaling: what was stored is scaled already)
+              *p = add_of(*p, val);
             } else {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                if ((unsigned)(c0 + e) >= NTa) break;
-                float2* p = crow + offNC[c0 + e];
-                const float2 val = make_float2(__uint_as_float(w[2 * e]), __uint_as_float(w[2 * e + 1]));
-                if (atomic) {
-                  atomic_add_of(p, val);
-                } else if (accumulate || rmw) {
-                  *p = add_of(*p, val);
-                } else {
-                  *p = val;
-                }
-              }
+              *p = val;
             }
           }
         }
-      } else {
-        // 32 fp32 columns (16 complex) per tcgen05.ld: one TMEM round trip per 128 bytes of a row
-#pragma unroll 1
-        for (int col = 0; col < 2 * NT; col += 32) {
-          // a later chunk adds to what the previous one stored: fetch those 16 complex values FIRST, so
-          // that their L2 latency overlaps the TMEM loads instead of being paid once per vector
-          // (same thread, same addresses as the chunk before: program order makes its stores visible)
-          unsigned long long old[16];
-          if (fold && row_ok) {
-#pragma unroll
-            for (int s4 = 0; s4 < 4; ++s4) {
-              const int c0 = (col >> 1) + s4 * 4;
-              unsigned long long* o = old + s4 * 4;
-              if ((unsigned)c0 >= NTa) continue;
-              if (quad_ok && (unsigned)c0 + 3 < NTa) {
-                asm volatile("ld.global.v4.b64 {%0,%1,%2,%3}, [%4];\n" : "=l"(o[0]), "=l"(o[1]), "=l"(o[2]), "=l"(o[3]) : "l"(crow + offNC[c0]) : "memory");
-              } else if (pair_ok) {
-#pragma unroll
-                for (int e = 0; e < 4; e += 2)
-                  if ((unsigned)(c0 + e) < NTa)
-                    asm volatile("ld.global.v2.b64 {%0,%1}, [%2];\n" : "=l"(o[e]), "=l"(o[e + 1]) : "l"(crow + offNC[c0 + e]) : "memory");
-              } else {
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                  if ((unsigned)(c0 + e) < NTa)
-                    asm volatile("ld.global.b64 %0, [%1];\n" : "=l"(o[e]) : "l"(crow + offNC[c0 + e]) : "memory");
-              }
-            }
-          }
-          unsigned v[32];
-          const unsigned ta = taddr + buf * Cfg::TMEM_COLS + ((unsigned)(quad * 32) << 16) + (unsigned)col;
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-              "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-              : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-              : "r"(ta));
-          // the small terms A'hi B'lo + A'lo B'hi sit 2NT columns further
-          unsigned u[32];
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-              "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-              : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]), "=r"(u[8]),
-                "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]), "=r"(u[16]),
-                "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]), "=r"(u[24]),
-                "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-              : "r"(ta + 2u * NT));
-          asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(u[i]));
-          if (sctx.on && row_ok) {
-            if (sctx.scale) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                const float2 z = strip_apply(sctx, make_float2(__uint_as_float(v[i]), __uint_as_float(v[i + 1])));
-                v[i] = __float_as_uint(z.x);
-                v[i + 1] = __float_as_uint(z.y);
-              }
-            } else {
-              // max|C|: integer scan over the 32 words, then (rarely) the values (see gett_ws.cuh)
-              int hmax = 0;
-#pragma unroll
-              for (int i = 0; i < 32; ++i) hmax = max(hmax, (int)(v[i] & 0x7fffffffu));
-              if (strip_hot<float2>(sctx, hmax)) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) strip_track_f(sctx, __uint_as_float(v[i]), __uint_as_float(v[i + 1]));
-              }
-            }
-          }
-          if (fold && row_ok) {  // (after the strip scaling: what was stored is scaled already)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              if ((unsigned)((col >> 1) + i) >= NTa) break;
-              v[2 * i] = __float_as_uint(__uint_as_float(v[2 * i]) + __uint_as_float((unsigned)old[i]));
-              v[2 * i + 1] = __float_as_uint(__uint_as_float(v[2 * i + 1]) + __uint_as_float((unsigned)(old[i] >> 32)));
-            }
-          }
-#pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4) {  // groups of 4 complex columns
-            const int c0 = (col >> 1) + s4 * 4;
-            const unsigned* w = v + s4 * 8;
-            if (!row_ok || (unsigned)c0 >= NTa) continue;
-            if (quad_ok && (unsigned)c0 + 3 < NTa) {
-              unsigned x[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) x[e] = w[e];
-              const unsigned long long q0 = ((unsigned long long)x[1] << 32) | x[0], q1 = ((unsigned long long)x[3] << 32) | x[2];
-              const unsigned long long q2 = ((unsigned long long)x[5] << 32) | x[4], q3 = ((unsigned long long)x[7] << 32) | x[6];
-              asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};\n" ::"l"(crow + offNC[c0]), "l"(q0), "l"(q1), "l"(q2),
-                           "l"(q3)
-                           : "memory");
-            } else if (pair_ok) {
-#pragma unroll
-              for (int e = 0; e < 4; e += 2) {
-                if ((unsigned)(c0 + e) >= NTa) break;  // NTa is even here
-                float2* p = crow + offNC[c0 + e];
-                unsigned x[4] = {w[2 * e], w[2 * e + 1], w[2 * e + 2], w[2 * e + 3]};
-                const unsigned long long q0 = ((unsigned long long)x[1] << 32) | x[0], q1 = ((unsigned long long)x[3] << 32) | x[2];
-                asm volatile("st.global.v2.b64 [%0], {%1,%2};\n" ::"l"(p), "l"(q0), "l"(q1) : "memory");
-              }
-            } else {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                if ((unsigned)(c0 + e) >= NTa) break;
-                float2* p = crow + offNC[c0 + e];
-                const float2 val = make_float2(__uint_as_float(w[2 * e]), __uint_as_float(w[2 * e + 1]));
-                if (atomic) {
-                  atomic_add_of(p, val);
-                } else if (accumulate) {
-                  *p = add_of(*p, val);
-                } else {
-                  *p = val;
-                }
-              }
-            }
-          }
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
       }
     }
     strip_end(sctx);
-  }
-  if (warp < 8) {
-    named_sync<2, 256>();
-    if (warp == 0)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(2 * Cfg::TMEM_COLS)
-                   : "memory");
   }
 }

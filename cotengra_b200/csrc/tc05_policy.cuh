@@ -1,4 +1,4 @@
-// tc05_policy.cuh -- operand preparation for the tcgen05 (kind::tf32) complex64 kernel.
+// tc05_policy.cuh -- operand preparation for the wgmma (tf32) complex64 kernel.
 // Included inside namespace ctgb.  The kernel itself is tc05_kernel.cuh.
 //
 // A complex tile product C[128 x NT] += A[128 x 16] * B[16 x NT] is run as the real
@@ -7,27 +7,26 @@
 //   B'[2n][2k] = Br   B'[2n][2k+1] = -Bi   B'[2n+1][2k] = Bi   B'[2n+1][2k+1] = Br
 // so that C' is C's own interleaved image.  fp32 accuracy comes from the 3xTF32
 // split  D = A'hi*B'hi + (A'lo*B'hi + A'hi*B'lo)  (hi = rn_tf32(x), lo = rn_tf32(x - hi); the tensor
-// core itself would only truncate, which biases a deep tree):
-// 1.3e-6 relative on a K = 64 tile (scripts/ubench/umma_c64.cu).
+// core itself would only truncate, which biases a deep tree).
 //
-// B' (hi and lo, already in shared-memory tile order: UMMA's K-major no-swizzle
+// B' (hi and lo, already in shared-memory tile order: wgmma's K-major no-swizzle
 // core-matrix layout [chunk = k'/4][row][k'%4]) is prepared once per launch by
 // bprime_kernel -- B is the small operand, <= a few MB -- so that each k-step's pair
 // of tiles is ONE contiguous TMA bulk copy.
 #pragma once
 
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // SmemDescriptor (cute/arch/mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
-  // version=1 [46,48), layout_type [61,64) = 0 (no swizzle / interleave)
+__device__ __forceinline__ uint64_t gmma_desc_kmajor(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  // wgmma matrix descriptor (PTX ISA, "Matrix Descriptor Format"): start>>4 [0,14), LBO>>4 [16,30),
+  // SBO>>4 [32,46), base offset [49,52) = 0, layout [62,64) = 0 (no swizzle).  K-major, no swizzle:
+  // LBO = stride between the two core matrices along K, SBO = stride between 8-row groups
   return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
 }
 // Round to nearest (ties away) onto the tf32 grid with integer ALU ops.  The tensor core only truncates,
 // and a truncating split (hi = trunc(x), lo = x - hi, lo truncated again by the MMA) biases every product
-// towards zero by ~2^-22: over the dependent nodes of a deep tree that bias adds up linearly (1.7e-5
-// instead of 2.3e-5 on the bond-6 PEPS tree, 2.2e-5 instead of 3.8e-5 on one Sycamore m20 slice once
-// rounded).  cvt.rna.tf32.f32 does the same but costs the scatter pass 13 % (63 instead of 72.6 TFLOP/s on
-// the m20 tree); add + mask are full-rate.  (x within 2^-11 of FLT_MAX would round to inf: not handled.)
+// towards zero by ~2^-22: over the dependent nodes of a deep tree that bias adds up linearly.
+// cvt.rna.tf32.f32 does the same with a slower instruction; add + mask are full-rate.  (x within 2^-11
+// of FLT_MAX would round to inf: not handled.)
 __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 __device__ __forceinline__ float round_tf32(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
@@ -83,7 +82,7 @@ __global__ void __launch_bounds__(256) bprime_kernel(const int64_t* __restrict__
     const float2 b = B[off];
     const float v = (q == p) ? b.x : (q == 0 ? -b.y : b.y);
     // stacked along N: chunk c holds 4NT rows -- rows [0, 2NT) are B'hi, rows [2NT, 4NT) are B'lo --
-    // so that one UMMA of N = 4NT multiplies A'hi with both and one of N = 2NT takes B'hi alone
+    // so that one wgmma of N = 4NT multiplies A'hi with both and one of N = 2NT takes B'hi alone
     const unsigned long long base = (idx / TILE) * (2ull * TILE) + ((unsigned long long)chunk * (4 * NT)) * 4 + j;
 #ifdef CTGB_TC05_TRUNC_SPLIT  // A/B knob: the truncating split
     Bp[base + row * 4] = v;

@@ -160,7 +160,7 @@ class ExecPlan:
             try:
                 sm_count = _lib.device_info()["sm_count"]
             except Exception:
-                sm_count = 148
+                sm_count = 132  # H100 SXM
         self.sm_count = sm_count
         self._keep = []
         self._build(hoist, allow_dmma, variant)

@@ -39,8 +39,8 @@ import math
 
 from .tree import TreeSpec
 
-# ---- per-node time model (seconds).  Rates are what the round-1/2 kernels reach on B200
-# (profiles/r0*_nodes_*.csv); they only have to rank alternatives, not predict times.
+# ---- per-node time model (seconds).  Relative kernel rates (not re-measured on H100); they only
+# have to rank alternatives, not predict times.
 _LAUNCH = 4e-6
 _RATES = {
     # dtype-class: (stream_bw, staged_bw, tensor rates by K, tiny-MN-huge-K bandwidth)
@@ -91,7 +91,7 @@ def node_time(dtype, B, M, N, K, elems):
     if N < 24:
         tf *= 0.8
         if dtype == "complex64":
-            staged_bw = 3.2e12  # tcgen05 128 x 16 tiles: measured on the M = 2^26, N = K = 16 node
+            staged_bw = 3.2e12  # wgmma 128 x 16 tiles
     # tile occupancy of the staged tensor-core variants (lowering.choose_variant)
     MT, NT = (64, 128) if N >= 96 else (128, 64) if N >= 48 else (256, 32) if N >= 24 else (256, 16)
     util = (M / (-(-M // MT) * MT)) * (N / (-(-N // NT) * NT))

@@ -64,7 +64,7 @@ VAR_DMMA_32x32, VAR_ROWSTREAM_K = 18, 19
 DMMASTREAM_MAX_N = 16  # the kernel takes N <= 32, but at N = 32 the staged 256x32 policy is faster (31.8 vs 26 TFLOP/s)
 TC05_VARIANTS = (VAR_TC05_128x64, VAR_TC05_128x32, VAR_TC05_128x16)
 TC05_MAX_K = 16384       # 1024 k-steps (the kernel's k table); beyond 256 in chunks of 256
-TC05_CHUNK_STEPS = 16    # full k-steps accumulated in TMEM before a round-to-nearest fold (tc05_chunk_steps in
+TC05_CHUNK_STEPS = 16    # full k-steps accumulated in one register accumulation before a round-to-nearest fold (tc05_chunk_steps in
                          # csrc/tc05_kernel.cuh balances the chunks and shortens them for tiles with fewer than 16 k)
 # (MT, NT, KT) of every kernel variant -- must match ctg_b200.cu's dispatch
 VARIANT_TILES = {
@@ -282,7 +282,7 @@ def split_tile(dims, cols, limit, order_col, exact=False, multiple=1):
     ``exact``: the blocked dim is cut into equal blocks (the largest divisor of its extent
     that fits), so that every tile has the same shape -- for kernels without ragged tiles;
     ``multiple``: ... among the divisors that make the tile's extent a multiple of this (the k of a
-    tcgen05 tile is whole UMMA k8 groups of complex numbers: 4).
+    wgmma tile is whole wgmma k8 groups of complex numbers: 4).
     """
     cand = sorted(range(len(dims)), key=lambda i: (_min_stride(dims[i], cols), i))
     tile, used, prod, partial_src = [], set(), 1, None
@@ -373,10 +373,10 @@ def choose_variant(dtype, B, M, N, K, allow_dmma=True, allow_stream=True, allow_
         return VAR_ROWSTREAM_K
     if N <= 8 and M >= 64:
         return VAR_ROW_256x4 if N <= 4 else VAR_ROW_128x8
-    # complex64 dense nodes with exact power-of-two tiles: tcgen05 (kind::tf32 x3, TMEM)
-    # (K > 256 runs in chunks of 256 inside the kernel: every chunk accumulates in TMEM from zero
+    # complex64 dense nodes with exact power-of-two tiles: wgmma (tf32 x3, register accumulators)
+    # (K > 256 runs in chunks of 256 inside the kernel: every chunk accumulates from zero
     # and the epilogue folds it into C with round-to-nearest adds -- the tensor core's own
-    # accumulation truncates, which is why a single TMEM accumulation stops at K = 256)
+    # accumulation truncates, which is why a single accumulation stops at K = 256)
     if (allow_dmma and allow_tc05 and dtype == "complex64" and M >= 128 and K >= 4 and N >= 12
             and K <= TC05_MAX_K and M * N * K >= 1 << 20):
         # (extents need not be powers of two: build_pair_desc cuts every class into EQUAL tiles by
@@ -391,9 +391,8 @@ def choose_variant(dtype, B, M, N, K, allow_dmma=True, allow_stream=True, allow_
     if allow_dmma and M * N * K >= 1 << 15 and M * N >= 1024:
         if dtype == "complex128" and allow_3m and N >= 64 and K >= 64:
             # 3M complex product (opt-in): 25 % fewer DMMAs but narrower tiles (accumulator
-            # registers).  Measured on B200: 36.6-37.8 vs 33.6 TFLOP/s at N=128 K=64, but 14 vs
-            # 24 at N=128 K=16 (per-tile epilogue dominates) and no gain on the whole Sycamore
-            # slice (160.5 vs 159 ms), so the default stays the 4-DMMA product.
+            # registers): faster on long k, slower on short k (per-tile epilogue dominates) and no
+            # gain on the whole Sycamore slice, so the default stays the 4-DMMA product.
             return VAR_DMMA3M_128x32
         if N >= 96:
             return VAR_DMMA_64x128
@@ -405,7 +404,7 @@ def choose_variant(dtype, B, M, N, K, allow_dmma=True, allow_stream=True, allow_
     return VAR_SIMT_64x64
 
 
-def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=148,
+def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
                     variant=None, allow_dmma=True, c_dense_elems=0,
                     force_splitk=None) -> PairPlan:
     """Pack a classified node into descriptor words."""
@@ -441,7 +440,7 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=148,
         KT = 2048  # 8 k per thread for the narrower element types (csrc/dotstream.cuh dot4_u)
 
     if variant in TC05_VARIANTS:
-        # tcgen05: every thread of the epilogue owns a whole row, so the rows of a tile need
+        # wgmma: the epilogue addresses every row through its own offset, so the rows of a tile need
         # not be neighbours in C -- pick them for the longest contiguous runs of A instead
         # (and B is re-packed by bprime_kernel anyway: only A's strides matter for k too)
         tm, gm, pm = split_tile(m, (1,), MT, order_col=1, exact=True)
@@ -536,10 +535,10 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=148,
     grid_pow2 = all(is_p2(g[0]) for g in gm + gn + gb)
     m_pow2 = all(is_p2(d[0]) for d in tm) and all(is_p2(g[0]) for g in gm)
     if variant in TC05_VARIANTS:
-        # the tcgen05 kernel takes tiles of ONE shape: its native 128 x NT x 16, or smaller with
-        # the rest of the tensor-core tile as padding (KTa in steps of 4: whole UMMA k8 groups);
+        # the wgmma kernel takes tiles of ONE shape: its native 128 x NT x 16, or smaller with
+        # the rest of the tensor-core tile as padding (KTa in steps of 4: whole wgmma k8 groups);
         # below 40 % occupancy the mma.sync policy is the better choice
-        # (k padding is free -- the UMMAs of missing k8 groups are not issued -- so only rows and columns count)
+        # (k padding is free -- the wgmmas of missing k8 groups are not issued -- so only rows and columns count)
         occupancy = (MTa * NTa) / float(MT * NT)
         exact = (MTa <= MT and NTa <= NT and KTa <= KT and KTa % 4 == 0 and dtype == "complex64"
                  and occupancy >= 0.4 and steps_k <= 1024
@@ -604,7 +603,7 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=148,
             and all(x[4] % g == 0 for x in gb)
         )
 
-    # tcgen05 variants: if the A tile is made of long contiguous runs (dense prefix of
+    # wgmma variants: if the A tile is made of long contiguous runs (dense prefix of
     # the load order), the producers fetch whole runs with TMA bulk copies (bit6)
     run_a, bulk_a = 1, False
     if variant in TC05_VARIANTS:

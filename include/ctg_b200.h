@@ -189,7 +189,7 @@ int ctgb_probe_fp64_peaks(double* dmma_tflops, double* dfma_tflops, void* stream
 /* Number of kernels this library has launched since load (bench.py's
  * `gpu_launches`). */
 int64_t ctgb_launch_count(void);
-/* ... of which tcgen05 launches whose A tiles are fetched by tensor-map TMA (cp.async.bulk.tensor). */
+/* ... of which wgmma launches whose A tiles are fetched by tensor-map TMA (cp.async.bulk.tensor). */
 int64_t ctgb_tensor_map_launches(void);
 
 #ifdef __cplusplus

@@ -481,8 +481,55 @@ def gen_sycamore():
     print("sycamore:", stats, tree.nslices, small.nslices, med.nslices)
 
 
+def gen_live_trees():
+    """40 random greedy trees (sliced, index-removed, sorted variants) with the reference's IR and
+    slice keys: the data tests/test_tree_ir.py compares TreeSpec against."""
+    rng = random.Random(5)
+    recs = []
+    for trial in range(40):
+        c = ctg.utils.rand_equation(
+            n=rng.randint(4, 12), reg=rng.randint(2, 4), n_out=rng.randint(0, 3),
+            n_hyper_in=rng.randint(0, 2), n_hyper_out=rng.randint(0, 2),
+            d_min=1, d_max=4, seed=trial,
+        )
+        tree = ctg.array_contract_tree(
+            c.inputs, c.output, c.size_dict, optimize="greedy",
+            sort_contraction_indices=rng.choice([None, "root", "flops"]),
+        )
+        if tree.max_size() > 16 and rng.random() < 0.7:
+            tree.slice_(target_size=max(tree.max_size() // 4, 1))
+        rem = [ix for ix in tree.get_legs(tree.root)]
+        if rem and rng.random() < 0.5:
+            tree.remove_ind_(rng.choice(rem))
+        recs.append(tree_record(f"live{trial}", tree, "complex128", seed=trial))
+    with open(os.path.join(GOLDEN_DIR, "live_trees.json"), "w") as f:
+        json.dump(recs, f)
+
+
+def gen_circuits():
+    """The Sycamore m10 / m20 circuit files (data) and the tensor-rank sequence of the
+    reference's simplified m20 benchmark network."""
+    import gzip
+    import shutil
+
+    for m in (10, 20):
+        name = f"circuit_n53_m{m}_s0_e0_pABCDCDAB.qsim"
+        with open(os.path.join("/root/reference/examples", name), "rb") as f, \
+                gzip.GzipFile(os.path.join(GOLDEN_DIR, name + ".gz"), "wb", mtime=0) as g:
+            shutil.copyfileobj(f, g)
+    with open("/root/reference/examples/benchmarks/sycamore_n53_m20_s0_e0_pABCDCDAB.json") as f:
+        ref = json.load(f)
+    ref_inputs = ref["inputs"] if isinstance(ref, dict) else ref[0]
+    with open(os.path.join(GOLDEN_DIR, "sycamore_m20_ranks.json"), "w") as f:
+        json.dump(sorted(len(t) for t in ref_inputs), f)
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["parsers", "equations", "trees", "sycamore"]
+    which = sys.argv[1:] or ["parsers", "equations", "trees", "sycamore", "live", "circuits"]
+    if "live" in which:
+        gen_live_trees()
+    if "circuits" in which:
+        gen_circuits()
     if "parsers" in which:
         gen_parsers()
     if "equations" in which:

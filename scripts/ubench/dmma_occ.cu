@@ -48,7 +48,8 @@ void run(const char* name, F launch, double flop) {
 }
 int main() {
   double* sink; cudaMalloc(&sink, 64);
-  int sms = 148, iters = 8192;
+  int sms = 0, iters = 8192;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   for (int warps : {4, 8, 16, 32}) {
     for (int blocks : {1, 2}) {
       char nm[64];

@@ -149,7 +149,7 @@ def install(monkeypatch):
     monkeypatch.setattr(contract, "_stream_ptr", lambda: 0)
     monkeypatch.setattr(_lib, "load", lambda: fake_lib)
     monkeypatch.setattr(_lib, "check", lambda rc: None if not rc else (_ for _ in ()).throw(RuntimeError(rc)))
-    monkeypatch.setattr(_lib, "device_info", lambda: {"sm_count": 148, "cc": (10, 0), "smem_optin": 232448})
+    monkeypatch.setattr(_lib, "device_info", lambda: {"sm_count": 132, "cc": (9, 0), "smem_optin": 232448})
 
     def create(self):
         self.handle = "emulated"

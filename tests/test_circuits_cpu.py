@@ -1,12 +1,24 @@
-"""Host-side .qsim reader: gate set sanity (no GPU, no reference needed) and, in the
-build container, the structure of the reference's Sycamore circuit files."""
+"""Host-side .qsim reader: gate set sanity and the structure of the Sycamore circuit files
+(stored under tests/golden/)."""
 
+import gzip
+import json
 import os
 
 import numpy as np
 import pytest
 
 from cotengra_b200.circuits import amplitude_network, gate_matrix, read_qsim
+from tests.helpers import GOLDEN_DIR
+
+
+def _qsim(m, tmp_path):
+    """The stored (gzip-compressed) Sycamore circuit file, unpacked to a temporary path."""
+    name = f"circuit_n53_m{m}_s0_e0_pABCDCDAB.qsim"
+    path = tmp_path / name
+    with gzip.open(os.path.join(GOLDEN_DIR, name + ".gz"), "rb") as f:
+        path.write_bytes(f.read())
+    return str(path)
 
 
 def test_gates_are_unitary_and_square_roots():
@@ -28,9 +40,8 @@ def test_gates_are_unitary_and_square_roots():
         gate_matrix("cz", ())
 
 
-@pytest.mark.reference
-def test_sycamore_m10_network_structure():
-    path = "/root/reference/examples/circuit_n53_m10_s0_e0_pABCDCDAB.qsim"
+def test_sycamore_m10_network_structure(tmp_path):
+    path = _qsim(10, tmp_path)
     n, gates = read_qsim(path)
     assert n == 53 and len(gates) == 1658  # SURVEY.md Appendix C
     inputs, output, size_dict, arrays = amplitude_network(path)
@@ -83,15 +94,14 @@ def test_rank_simplify_small_circuit_keeps_the_amplitude(tmp_path):
     assert abs(a0 - a1) < 1e-12 * max(1.0, abs(a0))
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize("m,tensors,indices", [(10, 164, 319), (20, 381, 754)])
-def test_rank_simplify_reaches_the_notebook_sizes(m, tensors, indices):
+def test_rank_simplify_reaches_the_notebook_sizes(m, tensors, indices, tmp_path):
     """The reference notebooks contract networks simplified by quimb: m10 has 164 tensors / 319
     indices (`Quantum Circuit Example Old.ipynb:143`), m20 381 / 754 -- the shipped benchmark JSON
     (`ex_benchmarking.ipynb` cell 4).  rank_simplify reproduces both counts from the .qsim files."""
     from cotengra_b200.circuits import rank_simplify
 
-    path = f"/root/reference/examples/circuit_n53_m{m}_s0_e0_pABCDCDAB.qsim"
+    path = _qsim(m, tmp_path)
     inputs, output, size_dict, arrays = amplitude_network(path)
     s_in, _o, s_sizes, s_arr = rank_simplify(inputs, output, size_dict, arrays)
     assert len(s_in) == tensors and len(s_sizes) == indices
@@ -103,9 +113,5 @@ def test_rank_simplify_reaches_the_notebook_sizes(m, tensors, indices):
     assert set(counts.values()) == {2}
     if m == 20:
         # same degree sequence as the reference's benchmark structure file
-        import json
-
-        with open("/root/reference/examples/benchmarks/sycamore_n53_m20_s0_e0_pABCDCDAB.json") as f:
-            ref = json.load(f)
-        ref_inputs = ref["inputs"] if isinstance(ref, dict) else ref[0]
-        assert sorted(len(t) for t in ref_inputs) == sorted(len(t) for t in s_in)
+        with open(os.path.join(GOLDEN_DIR, "sycamore_m20_ranks.json")) as f:
+            assert json.load(f) == sorted(len(t) for t in s_in)

@@ -1,5 +1,5 @@
-"""The drop-in boundary exercised through the reference's REAL control flow (build container
-only: needs /root/reference; the GPU launch is emulated by tests/emu_device.py).
+"""The drop-in boundary exercised through cotengra's REAL control flow (the unmodified package,
+installed into oracle/_ref/ by build(); the GPU launch is emulated by tests/emu_device.py).
 
     ctg.einsum(eq, *arrays, implementation=cb.implementation())   interface.py -> Contractor
     cb.install(tree); tree.contract(arrays)                       core.py:3943 -> contraction_cores
@@ -25,7 +25,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 @pytest.fixture()
 def ctg(monkeypatch):
-    sys.path[:0] = [os.path.join(ROOT, "oracle", "refshim"), "/root/reference"]
+    # the reference as build() installed it (oracle/build_ref.py) and its numpy-only autoray
+    sys.path[:0] = [os.path.join(ROOT, "oracle", "refshim"), os.path.join(ROOT, "oracle", "_ref")]
     try:
         import cotengra
 

@@ -1,4 +1,4 @@
-"""GPU parity tests proper: the sm_100a kernels, called through the C-ABI,
+"""GPU parity tests proper: the sm_90a kernels, called through the C-ABI,
 against (a) the golden vectors of the unmodified reference, (b) the numpy oracle
 on the same seeded inputs, and (c) size-independent properties at large sizes.
 

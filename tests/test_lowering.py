@@ -16,7 +16,7 @@ VARIANTS = [L.VAR_SIMT_64x64, L.VAR_DMMA_128x64, L.VAR_DMMA_64x128, L.VAR_DMMA_2
             L.VAR_DMMA3M_128x32, L.VAR_DMMA3M_256x16, L.VAR_DMMASTREAM, L.VAR_DOTSTREAM]
 
 
-def run_pair(eq, a, b, variant=None, splitk=None, sm_count=148):
+def run_pair(eq, a, b, variant=None, splitk=None, sm_count=132):
     terms, out = L.split_equation(eq)
     dims = L.classify_pair(terms[0], a.shape, terms[1], b.shape, out)
     n_out = int(np.prod(dims.out_shape)) if dims.out_shape else 1
@@ -190,7 +190,7 @@ def test_tcgen05_descriptor_properties():
         sizes["z"] = 3
         sa, sb = tuple(sizes[c] for c in ta), tuple(sizes[c] for c in tb)
         dims = L.classify_pair("".join(ta), sa, "".join(tb), sb, "".join(out))
-        plan = L.build_pair_desc(dims, "complex64", sm_count=148, c_dense_elems=1, force_splitk=1)
+        plan = L.build_pair_desc(dims, "complex64", sm_count=132, c_dense_elems=1, force_splitk=1)
         W = plan.words
         if plan.variant not in L.TC05_VARIANTS:
             continue
@@ -273,7 +273,7 @@ def test_tcgen05_tiles_on_extents_that_are_not_powers_of_two(eq, sa, sb):
     terms, out = L.split_equation(eq)
     dims = L.classify_pair(terms[0], sa, terms[1], sb, out)
     n_out = int(np.prod(dims.out_shape))
-    plan = L.build_pair_desc(dims, "complex64", sm_count=148, c_dense_elems=n_out)
+    plan = L.build_pair_desc(dims, "complex64", sm_count=132, c_dense_elems=n_out)
     assert plan.variant in L.TC05_VARIANTS, plan.variant
     W = plan.words
     MT, NT, KT = L.VARIANT_TILES[plan.variant]
@@ -297,7 +297,7 @@ def test_tcgen05_refuses_what_it_cannot_tile():
                        ("mk,kn->mn", (256, 32768), (32768, 64))]:     # K > 16384
         terms, out = L.split_equation(eq)
         dims = L.classify_pair(terms[0], sa, terms[1], sb, out)
-        plan = L.build_pair_desc(dims, "complex64", sm_count=148, c_dense_elems=int(np.prod(dims.out_shape)))
+        plan = L.build_pair_desc(dims, "complex64", sm_count=132, c_dense_elems=int(np.prod(dims.out_shape)))
         if plan.variant in L.TC05_VARIANTS:
             # whatever it accepted must still be an exact, sufficiently full tiling
             W = plan.words
@@ -331,7 +331,7 @@ def test_tcgen05_random_layouts_on_mixed_radix_extents():
         eq = "".join(ta) + "," + "".join(tb) + "->" + "".join(out)
         dims = L.classify_pair("".join(ta), sa, "".join(tb), sb, "".join(out))
         n_out = int(np.prod(dims.out_shape))
-        plan = L.build_pair_desc(dims, "complex64", sm_count=148, c_dense_elems=n_out)
+        plan = L.build_pair_desc(dims, "complex64", sm_count=132, c_dense_elems=n_out)
         if plan.variant not in L.TC05_VARIANTS:
             continue
         taken += 1
