@@ -30,6 +30,7 @@ EXPORTS = (
     "ctgb_plan_destroy",
     "ctgb_plan_workspace_bytes",
     "ctgb_plan_launches_per_slice",
+    "ctgb_plan_strip_modes",
     "ctgb_plan_execute",
     "ctgb_plan_execute_host",
     "ctgb_launch_count",
@@ -110,6 +111,7 @@ def load():
     lib.ctgb_plan_workspace_bytes.argtypes = [C.c_void_p]
     lib.ctgb_plan_launches_per_slice.restype = C.c_int64
     lib.ctgb_plan_launches_per_slice.argtypes = [C.c_void_p]
+    lib.ctgb_plan_strip_modes.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]
     lib.ctgb_device_info.argtypes = [
         C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_size_t)
     ]

@@ -459,7 +459,8 @@ def _combine_stripped(m1, e1, m2, e2):
         return m2, e2
     if e2 == -math.inf:
         return m1, e1
-    e = max(e1, e2)
+    # a NaN exponent stays NaN whichever side it is on (Python's max would keep it on one side only)
+    e = math.nan if math.isnan(e1) or math.isnan(e2) else max(e1, e2)
     return m1 * 10.0 ** (e1 - e) + m2 * 10.0 ** (e2 - e), e
 
 

@@ -893,6 +893,15 @@ size_t ctgb_plan_workspace_bytes(const ctgb_plan* p) {
   return p ? (size_t)(p->workspace_bytes + p->persistent_bytes) : 0;
 }
 int64_t ctgb_plan_launches_per_slice(const ctgb_plan* p) { return p ? p->launches_per_slice : 0; }
+int ctgb_plan_strip_modes(const ctgb_plan* p, int32_t* prescale_b, int32_t* measure_after, int n) {
+  if (!p || n < (int)p->nodes.size() || !prescale_b || !measure_after) return fail(CTGB_E_VALUE, "bad arguments");
+  for (size_t i = 0; i < p->nodes.size(); ++i) {
+    const auto& q = p->nodes[i];
+    prescale_b[i] = q.kind == 0 ? q.prescale_b : -1;
+    measure_after[i] = q.measure_after;
+  }
+  return CTGB_OK;
+}
 
 // Install the (single-operand style) descriptor that maps the dense root result
 // of one slice onto its chunk of the full output; only used with strip_exponent.

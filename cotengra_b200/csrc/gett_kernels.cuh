@@ -739,10 +739,16 @@ __device__ __forceinline__ double2 mulr_of(double2 v, double s) { return make_do
 //   e = max(E, es);  out = out * 10^(E - e) (+ chunk: m * 10^(es - e));  E = e
 // Phase 0 rescales the whole output (early-out when the scale is exactly 1),
 // phase 1 adds the slice mantissa into its chunk, phase 2 commits E.
+// A NaN slice exponent (a slice whose value is NaN somewhere) makes E NaN for good, and with it every
+// element of the sum: fmax would drop the NaN and leave a finite exponent beside a NaN mantissa, and
+// the reference's Python max keeps or drops it depending on the order of the slices.
+__device__ __forceinline__ double exponent_max(double a, double b) {
+  return (a != a || b != b) ? __longlong_as_double(0x7ff8000000000000LL) : fmax(a, b);
+}
 template <typename T>
 __global__ void rescale_out_kernel(T* __restrict__ out, long long n, const double* __restrict__ E,
                                    const double* __restrict__ es) {
-  const double e = fmax(*E, *es);
+  const double e = exponent_max(*E, *es);
   const double so = (*E == e) ? 1.0 : pow(10.0, *E - e);
   if (so == 1.0) return;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
@@ -754,7 +760,7 @@ __global__ void add_chunk_kernel(const int64_t* __restrict__ D, T* __restrict__ 
                                  const double* __restrict__ froot) {
   // D: single-operand descriptor mapping the dense slice result onto the chunk
   // froot: the root's own factor max|m| -- the stored root is not normalised yet (lazy scaling)
-  const double e = fmax(*E, *es);
+  const double e = exponent_max(*E, *es);
   double sn = (*es == e) ? 1.0 : pow(10.0, *es - e);
   if (froot != nullptr) sn = (*froot != 0.0) ? sn / *froot : 0.0;
   const int n_o = (int)D[S_NO];
@@ -772,7 +778,7 @@ __global__ void add_chunk_kernel(const int64_t* __restrict__ D, T* __restrict__ 
   }
 }
 __global__ void commit_exponent_kernel(double* __restrict__ E, const double* __restrict__ es) {
-  *E = fmax(*E, *es);
+  *E = exponent_max(*E, *es);
 }
 // strip_exponent, small operand pre-scaled: dst = src / (fA fB) over the whole underlying buffer of
 // the node's small operand (a few KB on a contraction stem), so that the big kernel's epilogue

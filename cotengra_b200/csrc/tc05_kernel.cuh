@@ -165,7 +165,9 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
   // actual tile extents: full 128 x NT x 16 on power-of-two networks; on others (PEPS bond 6) the
   // host picks exact divisors of the index extents, so every tile has the SAME smaller shape --
   // rows >= MTa and columns >= NTa of the operand images are padding that the epilogue ignores
-  // (B' is zero there), k >= KTa costs nothing: the wgmmas of the missing k8 groups are not issued
+  // (A' rows >= MTa hold whatever an earlier step left there, and bprime_kernel fills B' columns >= NTa
+  // with wrapped copies of real columns: both only reach accumulator rows / columns that are never
+  // stored), k >= KTa costs nothing: the wgmmas of the missing k8 groups are not issued
   const unsigned MTa = (unsigned)D[W_MTA], NTa = (unsigned)D[W_NTA], KTa = (unsigned)D[W_KTA];
   const unsigned a_elems = MTa * KTa;       // elements of one staged A tile
   const unsigned nq = KTa >> 2;             // k8 groups per k-step (KTa is a multiple of 4)
@@ -438,19 +440,44 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
       float2 v[NG];
 #pragma unroll
       for (int i = 0; i < NG; ++i) v[i] = upos[i] != 0xFFFFFFFFu ? src[ptid + i * GROUP] : make_float2(0.f, 0.f);
+#ifdef CTGB_TC05_TRUNC_SPLIT  // A/B knob: the cheaper truncating split (biased, see tc05_policy.cuh; inf gives
+                              // lo = inf - inf = NaN, so an inf operand yields NaN; not run by the test suite)
 #pragma unroll
       for (int i = 0; i < NG; ++i) {
         if (upos[i] != 0xFFFFFFFFu) {
-#ifdef CTGB_TC05_TRUNC_SPLIT  // A/B knob: the cheaper truncating split (biased, see tc05_policy.cuh)
           hi2[upos[i]] = v[i];
           lo2[upos[i]] = make_float2(v[i].x - trunc_tf32(v[i].x), v[i].y - trunc_tf32(v[i].y));
-#else
-          const float2 h = make_float2(round_tf32(v[i].x), round_tf32(v[i].y));
-          hi2[upos[i]] = h;
-          lo2[upos[i]] = make_float2(half_up_tf32(v[i].x - h.x), half_up_tf32(v[i].y - h.y));
-#endif
         }
       }
+#else
+      // fast split; one FMA per element collects whether any x - hi is inf or NaN (its product with the
+      // other component's is then inf or NaN, and so is the sum; a finite sum that overflows only sends
+      // this thread's elements down the exact path needlessly)
+      float bad = 0.f;
+#pragma unroll
+      for (int i = 0; i < NG; ++i) {
+        if (upos[i] != 0xFFFFFFFFu) {
+          const float2 h = make_float2(round_tf32(v[i].x), round_tf32(v[i].y));
+          const float dx = v[i].x - h.x, dy = v[i].y - h.y;
+          hi2[upos[i]] = h;
+          lo2[upos[i]] = make_float2(half_up_tf32(dx), half_up_tf32(dy));
+          bad = fmaf(dx, dy, bad);
+        }
+      }
+      if (!(fabsf(bad) <= 3.402823466e38f)) {  // inf, NaN or |x| near FLT_MAX in this thread's elements (rare)
+#pragma unroll
+        for (int i = 0; i < NG; ++i) {
+          if (upos[i] != 0xFFFFFFFFu) {
+            const float2 w = src[ptid + i * GROUP];  // (re-read: v[] need not stay live past the fast loop)
+            float2 h, l;
+            tc05_split(w.x, h.x, l.x);
+            tc05_split(w.y, h.y, l.y);
+            hi2[upos[i]] = h;
+            lo2[upos[i]] = l;
+          }
+        }
+      }
+#endif
       // generic-proxy writes (and reads of the staging slot) -> tensor core / TMA
       asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
       __syncwarp();

@@ -25,14 +25,30 @@ __device__ __forceinline__ uint64_t gmma_desc_kmajor(uint32_t saddr, uint32_t lb
 // Round to nearest (ties away) onto the tf32 grid with integer ALU ops.  The tensor core only truncates,
 // and a truncating split (hi = trunc(x), lo = x - hi, lo truncated again by the MMA) biases every product
 // towards zero by ~2^-22: over the dependent nodes of a deep tree that bias adds up linearly.
-// cvt.rna.tf32.f32 does the same with a slower instruction; add + mask are full-rate.  (x within 2^-11
-// of FLT_MAX would round to inf: not handled.)
+// cvt.rna.tf32.f32 does the same with a slower instruction; add + mask are full-rate.
 __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
+// the low half: the MMA drops the 13 low bits itself, adding half a tf32 ulp first makes that a rounding
+__device__ __forceinline__ float half_up_tf32(float x) { return __uint_as_float(__float_as_uint(x) + 0x1000u); }
+// The fast 3xTF32 split: hi = round_tf32(x), lo = half_up_tf32(x - hi) (x - hi is exact).  Its integer add
+// must not reach the exponent field, and for three kinds of input it does: a NaN whose top mantissa bits
+// are set (0x7FFFFFFF, the NaN GPU arithmetic makes) carries into the sign bit and becomes +-0, a finite x
+// within half a tf32 ulp of FLT_MAX becomes inf, and a NaN with its payload in the low 13 bits (0x7F800001)
+// becomes inf.  Exactly for those (and for +-inf) x - hi is not finite, which is how the producer's scatter
+// (tc05_kernel.cuh) finds them and sends them to tc05_split; bprime_kernel calls tc05_split directly.
 __device__ __forceinline__ float round_tf32(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-// the low half: the MMA drops the 13 low bits itself, adding half a tf32 ulp first makes that a rounding
-__device__ __forceinline__ float half_up_tf32(float x) { return __uint_as_float(__float_as_uint(x) + 0x1000u); }
+// The split for every input: a finite x whose rounding would carry into the exponent is truncated (lo stays
+// finite and exact), inf stays inf, a NaN gets its quiet bit set (the MMA reads only the top 10 mantissa
+// bits, so 0x7F800001 would otherwise be read as inf).  lo of an inf or NaN is whatever the add makes of
+// x - hi: the product is non-finite either way.
+__device__ __forceinline__ void tc05_split(float x, float& hi, float& lo) {
+  const unsigned u = __float_as_uint(x), a = u & 0x7FFFFFFFu;
+  unsigned h = (u + 0x1000u) & 0xFFFFE000u;
+  if (a >= 0x7F7FF000u) h = a > 0x7F800000u ? (u | 0x00400000u) : a == 0x7F800000u ? u : (u & 0xFFFFE000u);
+  hi = __uint_as_float(h);
+  lo = half_up_tf32(x - hi);
+}
 
 // B -> B'hi / B'lo in shared-memory tile order:
 //   Bp[((ib*tiles_n + in)*steps_k + step)][chunk 0..7][row 0..4NT-1: hi rows, then lo rows][4 floats]
@@ -84,13 +100,15 @@ __global__ void __launch_bounds__(256) bprime_kernel(const int64_t* __restrict__
     // stacked along N: chunk c holds 4NT rows -- rows [0, 2NT) are B'hi, rows [2NT, 4NT) are B'lo --
     // so that one wgmma of N = 4NT multiplies A'hi with both and one of N = 2NT takes B'hi alone
     const unsigned long long base = (idx / TILE) * (2ull * TILE) + ((unsigned long long)chunk * (4 * NT)) * 4 + j;
-#ifdef CTGB_TC05_TRUNC_SPLIT  // A/B knob: the truncating split
+#ifdef CTGB_TC05_TRUNC_SPLIT  // A/B knob: the truncating split (inf gives lo = inf - inf = NaN: a product
+                              // with an inf operand comes out NaN, not inf; not run by the test suite)
     Bp[base + row * 4] = v;
     Bp[base + (row + 2 * NT) * 4] = v - trunc_tf32(v);
 #else
-    const float vh = round_tf32(v);
-    Bp[base + row * 4] = vh;                                // hi
-    Bp[base + (row + 2 * NT) * 4] = half_up_tf32(v - vh);   // lo (v - vh is exact)
+    float vh, vl;
+    tc05_split(v, vh, vl);
+    Bp[base + row * 4] = vh;                   // hi
+    Bp[base + (row + 2 * NT) * 4] = vl;        // lo
 #endif
   }
 }

@@ -18,6 +18,10 @@ __device__ __forceinline__ unsigned to_tf32(float x) {
 }
 __device__ __forceinline__ void split_tf32(float x, unsigned& hi, unsigned& lo) {
   hi = to_tf32(x);
+  // a finite x within half a tf32 ulp of FLT_MAX rounds to inf (and hi + lo = inf - inf): truncate it
+  // instead; inf and NaN inputs pass through
+  if ((hi & 0x7FFFFFFFu) == 0x7F800000u && (__float_as_uint(x) & 0x7FFFFFFFu) != 0x7F800000u)
+    hi = __float_as_uint(x) & 0xFFFFE000u;
   lo = to_tf32(x - __uint_as_float(hi));
 }
 __device__ __forceinline__ void mma_tf32(float (&c)[4], const unsigned (&a)[4], const unsigned (&b)[2]) {

@@ -441,6 +441,14 @@ class ExecPlan:
     def launches_per_slice(self):
         return int(_lib.load().ctgb_plan_launches_per_slice(self.handle))
 
+    def strip_modes(self):
+        """strip_exponent plans: ``(prescale_b, measure_after)`` of every node of ``self.nodes``
+        (ctgb_plan_strip_modes; prescale_b is -1 for single-operand nodes)."""
+        n = len(self.nodes)
+        pre, after = (C.c_int32 * n)(), (C.c_int32 * n)()
+        _lib.check(_lib.load().ctgb_plan_strip_modes(self.handle, pre, after, n))
+        return [(int(a), int(b)) for a, b in zip(pre, after)]
+
     def destroy(self):
         if self.handle is not None:
             _lib.load().ctgb_plan_destroy(self.handle)

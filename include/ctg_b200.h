@@ -148,6 +148,12 @@ int ctgb_plan_set_chunk_desc(ctgb_plan* plan, const int64_t* desc);
 void ctgb_plan_destroy(ctgb_plan* plan);
 size_t ctgb_plan_workspace_bytes(const ctgb_plan* plan);
 int64_t ctgb_plan_launches_per_slice(const ctgb_plan* plan);
+/* strip_exponent plans: how each node (in desc->nodes order, n entries) applies the 1/(fA fB) of its
+ * operands' factors.  prescale_b[i] = 1: a scaled copy of the B operand is made first (operands of at
+ * most 16 MiB); 0: the kernel's epilogue multiplies (and may take the float, double or two-factor
+ * route); -1: a single-operand node.  measure_after[i] = 1: max|C| is measured by a pass after the
+ * launch (split-K, dot-type, KRED and chunked wgmma nodes). */
+int ctgb_plan_strip_modes(const ctgb_plan* plan, int32_t* prescale_b, int32_t* measure_after, int n);
 
 /* Contract slices slice_begin, slice_begin + slice_step, ... (slice_count of
  * them) and ACCUMULATE their contributions into `out` (device, out_elements of

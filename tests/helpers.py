@@ -52,6 +52,16 @@ def decode_sliced(sliced):
             for ind, size, project in sliced]
 
 
+def tree_spec(rec):
+    """The ``cotengra_b200.TreeSpec`` of a golden tree record (``trees.json``)."""
+    import cotengra_b200 as cb
+
+    n_in = len(rec["inputs"])
+    node_inds = {int(k): v for k, v in rec["inds"].items() if int(k) >= n_in}
+    return cb.TreeSpec(rec["inputs"], rec["output"], rec["size_dict"], rec["path"],
+                       decode_sliced(rec["sliced"]), node_inds)
+
+
 def rel_err(x, ref):
     x = np.asarray(x)
     ref = np.asarray(ref)
