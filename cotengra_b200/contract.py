@@ -24,6 +24,7 @@ from __future__ import annotations
 import ctypes as C
 import functools
 import math
+import warnings
 
 import numpy as np
 
@@ -206,6 +207,8 @@ class TreeExecutor:
         self.strip_exponent = bool(strip_exponent)
         self._ws = None
         self._ref_work = None
+        self._ir, self._plan_opts = ir, plan_opts
+        self._vjp_plans, self._vjp_ws = {}, None
 
     @property
     def reference_work(self):
@@ -258,20 +261,69 @@ class TreeExecutor:
             if self.strip_exponent and exponent is None:
                 exponent = torch.full((1,), -math.inf, dtype=torch.float64, device=self.device)
             ws = self.workspace()
-            ptrs, keep = [], []
-            for i, t in enumerate(tensors):
-                if dtype_name(t.dtype) != self.dtype:
-                    raise TypeError(f"plan was built for {self.dtype}, got {t.dtype}")
-                if t.device != self.device:
-                    raise ValueError(f"array {i} lives on {t.device}, the plan on {self.device}")
-                if not t.is_contiguous():
-                    # the kernels address row-major storage by the plan's own strides
-                    t = t.contiguous()
-                    keep.append(t)
-                ptrs.append(t.data_ptr())
+            ptrs, _keep = self._input_ptrs(tensors)
             self.plan.execute(ptrs, out.data_ptr(), exponent.data_ptr() if exponent is not None else None,
                               ws.data_ptr(), ws.numel(), begin, step, count, _stream_ptr())
         return (out, exponent) if self.strip_exponent else out
+
+    def _input_ptrs(self, tensors):
+        """Device pointers of the inputs (plus the contiguous copies that must outlive the call)."""
+        ptrs, keep = [], []
+        for i, t in enumerate(tensors):
+            if dtype_name(t.dtype) != self.dtype:
+                raise TypeError(f"plan was built for {self.dtype}, got {t.dtype}")
+            if t.device != self.device:
+                raise ValueError(f"array {i} lives on {t.device}, the plan on {self.device}")
+            if not t.is_contiguous():
+                # the kernels address row-major storage by the plan's own strides
+                t = t.contiguous()
+                keep.append(t)
+            ptrs.append(t.data_ptr())
+        return ptrs, keep
+
+    # ------------------------------------------------------------------ gradients
+    def vjp_plan(self, wrt=None):
+        """The (cached) ``VjpPlan`` of the executed program for the inputs ``wrt`` (default all)."""
+        from .vjp import VjpPlan
+
+        n = len(self.spec.inputs)
+        key = tuple(range(n)) if wrt is None else tuple(sorted({int(i) for i in wrt}))
+        plan = self._vjp_plans.get(key)
+        if plan is None:
+            torch = _torch()
+            with torch.cuda.device(self.device):
+                plan = VjpPlan(self._ir, self.spec.inputs, self.spec.output, self.spec.size_dict,
+                               self.spec.sliced, dtype=self.dtype, wrt=key,
+                               strip_exponent=self.strip_exponent, **self._plan_opts).create()
+            self._vjp_plans[key] = plan
+        return plan
+
+    def vjp(self, tensors, cotangent, begin=0, step=1, count=None, wrt=None):
+        """Gradients of the sum of slices ``begin, begin+step, ...`` (``count`` of them) for the
+        output cotangent ``cotangent`` (the full output's shape): a list with one tensor per input,
+        ``None`` for inputs outside ``wrt`` (default: all).  Complex gradients follow torch's
+        convention.  Asynchronous on the current stream.  Gradients are linear in the cotangent and
+        additive over slices, so one call per rank over ``rank_slices(...)`` followed by an
+        all-reduce gives the gradient of the whole tree."""
+        torch = _torch()
+        self._check_inputs(tensors)
+        begin, step, count = self._check_slice_range(begin, step, count)
+        plan = self.vjp_plan(wrt)
+        tdt = getattr(torch, _NP2T[self.dtype])
+        with torch.cuda.device(self.device):
+            ptrs, _keep = self._input_ptrs(tensors)
+            if tuple(cotangent.shape) != tuple(plan.out_shape):
+                raise ValueError(f"cotangent has shape {tuple(cotangent.shape)}, the output {tuple(plan.out_shape)}")
+            cot = cotangent.to(device=self.device, dtype=tdt).contiguous()
+            grads = [torch.zeros(tuple(t.shape), dtype=tdt, device=self.device) if i in plan.wrt else None
+                     for i, t in enumerate(tensors)]
+            if self._vjp_ws is None or self._vjp_ws.numel() < plan.total_bytes:
+                self._vjp_ws = None
+                self._vjp_ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
+            ws = self._vjp_ws
+            plan.execute(ptrs, cot.data_ptr(), [g.data_ptr() if g is not None else None for g in grads],
+                         ws.data_ptr(), ws.numel(), begin, step, count, _stream_ptr())
+        return grads
 
     def _check_slice_range(self, begin, step, count):
         """Slice ids ``begin, begin+step, ...`` must all lie in ``[0, nslices)``: the device
@@ -380,11 +432,56 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
             return _finish_stripped(m, e, check_zero)
         return res
     tensors = [_to_device(a, ex.device)[0] for a in arrays]
+    if _records_grad(torch, arrays, ex.strip_exponent):
+        return _differentiable(torch, lambda ts: ex.contract_device(ts, begin, step, count),
+                               lambda ts, g, wrt: ex.vjp(ts, g, begin, step, count, wrt=wrt), tensors)
     res = ex.contract_device(tensors, begin, step, count)
     if ex.strip_exponent:
         m, e = res
         return _finish_stripped(m, float(e.item()), check_zero)
     return res
+
+
+def _records_grad(torch, arrays, strip_exponent):
+    """Whether a call records a torch autograd node: torch tensor inputs, at least one requiring
+    grad, grad mode on.  ``strip_exponent`` results get no gradient (a warning says so)."""
+    if not torch.is_grad_enabled() or not arrays:
+        return False
+    if not all(isinstance(a, torch.Tensor) for a in arrays) or not any(a.requires_grad for a in arrays):
+        return False
+    if strip_exponent:
+        warnings.warn("strip_exponent=True: no gradient is recorded for the (mantissa, exponent) result",
+                      UserWarning, stacklevel=3)
+        return False
+    return True
+
+
+_GRAD_FN = None
+
+
+def _differentiable(torch, run, vjp, tensors):
+    """``run(tensors)`` as one torch autograd node whose backward is ``vjp(tensors, grad, wrt)``
+    (a ``VjpPlan`` on the device; ``wrt`` from ``ctx.needs_input_grad``)."""
+    global _GRAD_FN
+    if _GRAD_FN is None:
+        from torch.autograd.function import once_differentiable
+
+        class _Contract(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, run, vjp, *tensors):
+                ctx.vjp = vjp
+                ctx.save_for_backward(*tensors)
+                return run(list(tensors))
+
+            @staticmethod
+            @once_differentiable
+            def backward(ctx, grad):
+                wrt = [i for i, need in enumerate(ctx.needs_input_grad[2:]) if need]
+                grads = ctx.vjp(list(ctx.saved_tensors), grad, wrt)
+                return (None, None, *grads)
+
+        _GRAD_FN = _Contract
+    return _GRAD_FN.apply(run, vjp, *tensors)
 
 
 def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=None, **plan_opts):
@@ -585,7 +682,10 @@ class B200Contractor:
         dtype = _common_dtype(*tensors)
         with torch.cuda.device(tensors[0].device if tensors else torch.cuda.current_device()):
             ex = self._executor(tuple(tuple(t.shape) for t in tensors), dtype, strip)
-            res = ex.run([t.to(ex.device) for t in tensors])
+            on_dev = [t.to(ex.device) for t in tensors]
+            if _records_grad(torch, arrays, strip):
+                return _differentiable(torch, ex.run, ex.vjp, on_dev)
+            res = ex.run(on_dev)
         if strip:
             m, e = res
             e = float(e.item())
@@ -611,6 +711,8 @@ class _FlatExecutor:
         self.strip = strip
         self.ws = torch.empty(max(self.plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
         self.tdt = getattr(torch, _NP2T[self.plan.dtype])
+        self._program = (contractions, inputs, output, sd)
+        self._vjp_plans = {}
 
     def run(self, tensors):
         torch = _torch()
@@ -621,6 +723,26 @@ class _FlatExecutor:
                               exp.data_ptr() if exp is not None else None, self.ws.data_ptr(),
                               self.ws.numel(), 0, 1, 1, _stream_ptr())
         return (out, exp) if self.strip else out
+
+    def vjp(self, tensors, cotangent, wrt):
+        """Input gradients for ``cotangent`` (``None`` outside ``wrt``) through a ``VjpPlan``."""
+        from .vjp import VjpPlan
+
+        torch = _torch()
+        key = tuple(sorted(wrt))
+        with torch.cuda.device(self.device):
+            plan = self._vjp_plans.get(key)
+            if plan is None:
+                plan = self._vjp_plans[key] = VjpPlan(*self._program, (), dtype=self.plan.dtype, wrt=key).create()
+            cot = cotangent.to(device=self.device, dtype=self.tdt).contiguous()
+            grads = [torch.zeros(tuple(t.shape), dtype=self.tdt, device=self.device) if i in plan.wrt else None
+                     for i, t in enumerate(tensors)]
+            ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
+            srcs = [t.contiguous() for t in tensors]
+            plan.execute([t.data_ptr() for t in srcs], cot.data_ptr(),
+                         [g.data_ptr() if g is not None else None for g in grads], ws.data_ptr(), ws.numel(),
+                         0, 1, 1, _stream_ptr())
+        return grads
 
 
 def _program_output_shape(contractions, shapes):

@@ -14,6 +14,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <type_traits>
 #include <string>
@@ -485,6 +486,8 @@ int launch_gett_typed(const int64_t* h, const int64_t* d, const void* A, const v
       case VAR_DMMA_64x128: return launch_gett_policy<T, Tf32Policy<T, 2, 4, 2, 4, 16, 3>>(h, d, A, B, C, st);
       case VAR_DMMA_256x32: return launch_gett_policy<T, Tf32Policy<T, 8, 1, 2, 4, 8, 3>>(h, d, A, B, C, st);
       case VAR_DMMA_256x16: return launch_gett_policy<T, Tf32Policy<T, 8, 1, 2, 2, 8, 3>>(h, d, A, B, C, st);
+      // DMMA_32x32's geometry: one 32 x 32 tile, four warps, the contracted range split over the SMs
+      case VAR_TF32_32x32: return launch_gett_policy<T, Tf32Policy<T, 2, 2, 1, 2, 16, 4>>(h, d, A, B, C, st);
       default: break;
     }
   }
@@ -595,18 +598,113 @@ int accum_stripped(int dtype, const int64_t* dchunk, const int64_t* hchunk, void
   return fail(CTGB_E_VALUE, "bad dtype");
 }
 
+template <typename T>
+int conj_typed(void* p, long long n, cudaStream_t st) {
+  conj_kernel<T><<<flat_grid(n), 256, 0, st>>>((T*)p, n);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  CUDA_TRY(cudaGetLastError());
+  return CTGB_OK;
+}
+// in-place conjugate of n elements (nothing to do for real dtypes)
+int conj_inplace(int dtype, void* p, long long n, cudaStream_t st) {
+  if (n <= 0) return CTGB_OK;
+  if (dtype == CTGB_C64) return conj_typed<float2>(p, n, st);
+  if (dtype == CTGB_C128) return conj_typed<double2>(p, n, st);
+  return CTGB_OK;
+}
+
+int launch_node(int kind, const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
+  return kind == 0 ? launch_gett(h, d, A, B, C, st) : launch_single(h, d, A, C, st);
+}
+
 }  // namespace
+
+// ================================================================== shared by plans and VJP plans
+// A tensor slot (ctgb_tensor) as the library keeps it.
+struct ctgb_tensor_rec {
+  int kind, input_index;
+  int64_t offset, nbytes;
+  std::vector<int32_t> slice_pos;
+  std::vector<int64_t> slice_stride;
+};
+
+// The memory tensor slots resolve to while one slice runs.
+struct ctgb_slice_mem {
+  const void* const* inputs = nullptr;  // kind 0
+  void* const* grads = nullptr;         // kind 5
+  char* persistent = nullptr;           // kinds 2, 6
+  char* scratch = nullptr;              // kind 1
+  char* out = nullptr;                  // kind 3
+  const char* cot = nullptr;            // kind 4
+  size_t es = 0;
+  const int64_t* digits = nullptr;
+};
+
+static char* resolve_tensor(const ctgb_tensor_rec& q, const ctgb_slice_mem& m, int64_t out_off) {
+  auto sliced = [&](const void* base) {
+    int64_t off = 0;
+    for (size_t j = 0; j < q.slice_pos.size(); ++j) off += m.digits[q.slice_pos[j]] * q.slice_stride[j];
+    return (char*)base + off * (int64_t)m.es;
+  };
+  switch (q.kind) {
+    case 0: return sliced(m.inputs[q.input_index]);
+    case 1: return m.scratch + q.offset;
+    case 2:
+    case 6: return m.persistent + q.offset;
+    case 4: return (char*)m.cot + out_off * (int64_t)m.es;
+    case 5: return sliced(m.grads[q.input_index]);
+    default: return m.out + out_off * (int64_t)m.es;
+  }
+}
+
+// slice id -> digits, most significant first (core.py:3775-3800); returns the element offset of the
+// slice's output view (sum of digit * out_stride)
+static int64_t decode_slice(int64_t id, const std::vector<int64_t>& radix, const std::vector<int64_t>& project,
+                            const std::vector<int64_t>& out_stride, std::vector<int64_t>& digits) {
+  // least-significant digit first: the same digits as i // stride_j % radix_j,
+  // without forming the strides (their product overflows 64 bits for trees
+  // with more than 63 binary sliced indices; ids themselves are < 2^63)
+  const int ns = (int)radix.size();
+  int64_t rem = id;
+  for (int j = ns - 1; j >= 0; --j) {
+    if (project[j] >= 0) {
+      digits[j] = project[j];
+    } else {
+      digits[j] = rem % radix[j];
+      rem /= radix[j];
+    }
+  }
+  int64_t out_off = 0;
+  for (int j = 0; j < ns; ++j) out_off += digits[j] * out_stride[j];
+  return out_off;
+}
+
+// copies a ctgb_tensor array into records, checking input and slice references
+static int copy_tensors(const ctgb_tensor* ts, int n, int n_inputs, int n_sliced, std::vector<ctgb_tensor_rec>& out) {
+  out.resize(n);
+  for (int i = 0; i < n; ++i) {
+    const ctgb_tensor& t = ts[i];
+    auto& q = out[i];
+    q.kind = t.kind;
+    q.input_index = t.input_index;
+    q.offset = t.offset;
+    q.nbytes = t.nbytes;
+    if ((t.kind == 0 || t.kind == 5) && (t.input_index < 0 || t.input_index >= n_inputs))
+      return fail(CTGB_E_VALUE, "tensor refers to a missing input");
+    for (int j = 0; j < t.n_sliced; ++j) {
+      if (t.slice_pos[j] < 0 || t.slice_pos[j] >= n_sliced) return fail(CTGB_E_VALUE, "slice position out of range");
+      q.slice_pos.push_back(t.slice_pos[j]);
+      q.slice_stride.push_back(t.slice_stride[j]);
+    }
+  }
+  return CTGB_OK;
+}
 
 // ================================================================== plans
 struct ctgb_plan {
   int dtype = 0;
   int n_inputs = 0;
-  struct Tensor {
-    int kind, input_index;
-    int64_t offset, nbytes;
-    std::vector<int32_t> slice_pos;
-    std::vector<int64_t> slice_stride;
-  };
+  using Tensor = ctgb_tensor_rec;
   struct Node {
     int kind, a, b, c, invariant, is_root;
     size_t desc_off;  // word offset into descs
@@ -726,26 +824,9 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
   ctgb_plan* p = new ctgb_plan();
   p->dtype = pd->dtype;
   p->n_inputs = pd->n_inputs;
-  p->tensors.resize(pd->n_tensors);
-  for (int i = 0; i < pd->n_tensors; ++i) {
-    const ctgb_tensor& t = pd->tensors[i];
-    auto& q = p->tensors[i];
-    q.kind = t.kind;
-    q.input_index = t.input_index;
-    q.offset = t.offset;
-    q.nbytes = t.nbytes;
-    if (t.kind == 0 && (t.input_index < 0 || t.input_index >= pd->n_inputs)) {
-      delete p;
-      return fail(CTGB_E_VALUE, "tensor refers to a missing input");
-    }
-    for (int j = 0; j < t.n_sliced; ++j) {
-      if (t.slice_pos[j] < 0 || t.slice_pos[j] >= pd->n_sliced) {
-        delete p;
-        return fail(CTGB_E_VALUE, "slice position out of range");
-      }
-      q.slice_pos.push_back(t.slice_pos[j]);
-      q.slice_stride.push_back(t.slice_stride[j]);
-    }
+  if (int rc = copy_tensors(pd->tensors, pd->n_tensors, pd->n_inputs, pd->n_sliced, p->tensors)) {
+    delete p;
+    return rc;
   }
   p->nodes.resize(pd->n_nodes);
   int64_t per_slice = 0;
@@ -931,19 +1012,14 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   double* d_slice_exp = p->d_scalars + 1;
   double* d_inv_exp = p->d_scalars + 2;
 
-  auto resolve = [&](int t, int64_t out_off) -> char* {
-    const ctgb_plan::Tensor& q = p->tensors[t];
-    switch (q.kind) {
-      case 0: {
-        int64_t off = 0;
-        for (size_t j = 0; j < q.slice_pos.size(); ++j) off += digits[q.slice_pos[j]] * q.slice_stride[j];
-        return (char*)inputs[q.input_index] + off * (int64_t)es;
-      }
-      case 1: return scratch + q.offset;
-      case 2: return persistent + q.offset;
-      default: return (char*)out + out_off * (int64_t)es;
-    }
-  };
+  ctgb_slice_mem mem;
+  mem.inputs = inputs;
+  mem.persistent = persistent;
+  mem.scratch = scratch;
+  mem.out = (char*)out;
+  mem.es = es;
+  mem.digits = digits.data();
+  auto resolve = [&](int t, int64_t out_off) -> char* { return resolve_tensor(p->tensors[t], mem, out_off); };
 
   auto run_nodes = [&](bool invariant_pass, int64_t out_off) -> int {
     for (size_t ni = 0; ni < p->nodes.size(); ++ni) {
@@ -967,9 +1043,9 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
           if (rc) return rc;
           B = p->d_bscale + (B - under);
         }
-        rc = launch_gett(h, d, A, B, C, st);
+        rc = launch_node(0, h, d, A, B, C, st);
       } else {
-        rc = launch_single(h, d, A, C, st);
+        rc = launch_node(1, h, d, A, nullptr, C, st);
       }
       if (rc) return rc;
       // contract.py:816-829 strips after every *pairwise* node (single-operand preprocessing
@@ -1004,24 +1080,7 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   }
 
   for (int64_t k = 0; k < slice_count; ++k) {
-    // slice id -> digits, most significant first (core.py:3775-3800)
-    int64_t i = slice_begin + k * slice_step;
-    {
-      // least-significant digit first: the same digits as i // stride_j % radix_j,
-      // without forming the strides (their product overflows 64 bits for trees
-      // with more than 63 binary sliced indices; ids themselves are < 2^63)
-      int64_t rem = i;
-      for (int j = ns - 1; j >= 0; --j) {
-        if (p->project[j] >= 0) {
-          digits[j] = p->project[j];
-        } else {
-          digits[j] = rem % p->radix[j];
-          rem /= p->radix[j];
-        }
-      }
-    }
-    int64_t out_off = 0;
-    for (int j = 0; j < ns; ++j) out_off += digits[j] * p->out_stride[j];
+    const int64_t out_off = decode_slice(slice_begin + k * slice_step, p->radix, p->project, p->out_stride, digits);
     if (p->strip_exponent && p->n_var_slots > 0) {
       reset_slots_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists, p->n_var_slots);
       g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -1110,6 +1169,161 @@ int ctgb_plan_execute_host(ctgb_plan* p, const void* const* host_inputs, const i
   if (p->strip_exponent && host_exponent)
     CUDA_TRY(cudaMemcpyAsync(host_exponent, d_exp, sizeof(double), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
+  return CTGB_OK;
+}
+
+}  // extern "C"
+
+// ================================================================== VJP plans
+// Reverse mode through a tree (cotengra_b200/vjp.py plans it).  Every backward node is an ordinary
+// pairwise or single-operand descriptor: the plan propagates H = conj(cotangent), for which the
+// adjoint of a contraction needs no conjugation, so only the cotangent's copy and the finished input
+// gradients are conjugated (complex dtypes).
+struct ctgb_vjp {
+  int dtype = 0;
+  int n_inputs = 0;
+  std::vector<ctgb_tensor_rec> tensors;
+  struct Node {
+    int kind, a, b, c, phase, zero_fill;
+    size_t desc_off;
+  };
+  std::vector<Node> nodes;
+  std::vector<int64_t> descs;
+  int64_t* d_descs = nullptr;
+  std::vector<int64_t> radix, project, out_stride;
+  int64_t out_elements = 0, workspace_bytes = 0, persistent_bytes = 0, cot_offset = -1;
+  std::vector<int64_t> grad_elems;  // per input: elements of its gradient (0: not differentiated)
+};
+
+extern "C" {
+
+int ctgb_vjp_create(const ctgb_vjp_desc* vd, ctgb_vjp** out) {
+  if (!vd || !out) return fail(CTGB_E_VALUE, "null argument");
+  const size_t es = elem_size(vd->dtype);
+  if (es == 0) return fail(CTGB_E_VALUE, "bad dtype");
+  const bool cplx = vd->dtype == CTGB_C64 || vd->dtype == CTGB_C128;
+  if (cplx && (vd->cotangent_offset < 0 ||
+               vd->cotangent_offset + vd->out_elements * (int64_t)es > vd->persistent_bytes))
+    return fail(CTGB_E_VALUE, "a complex VJP plan needs room for the conjugated cotangent");
+  ctgb_vjp* v = new ctgb_vjp();
+  v->dtype = vd->dtype;
+  v->n_inputs = vd->n_inputs;
+  if (int rc = copy_tensors(vd->tensors, vd->n_tensors, vd->n_inputs, vd->n_sliced, v->tensors)) {
+    delete v;
+    return rc;
+  }
+  v->grad_elems.assign(vd->n_inputs, 0);
+  for (const auto& q : v->tensors) {
+    if (q.kind < 0 || q.kind > 6 || q.kind == 3) {
+      delete v;
+      return fail(CTGB_E_VALUE, "bad tensor kind for a VJP plan");
+    }
+    if (q.kind == 5) v->grad_elems[q.input_index] = q.nbytes / (int64_t)es;
+  }
+  v->nodes.resize(vd->n_nodes);
+  for (int i = 0; i < vd->n_nodes; ++i) {
+    const ctgb_vjp_node& n = vd->nodes[i];
+    auto& q = v->nodes[i];
+    q.kind = n.kind;
+    q.a = n.a;
+    q.b = n.b;
+    q.c = n.c;
+    q.phase = n.phase;
+    q.zero_fill = n.zero_fill;
+    const int words = n.kind == 0 ? (int)DESC_WORDS : (int)SDESC_WORDS;
+    const int64_t magic = n.kind == 0 ? DESC_MAGIC : SDESC_MAGIC;
+    auto bad = [&](int t) { return t < 0 || t >= vd->n_tensors; };
+    if (n.kind < 0 || n.kind > 1 || !n.desc || n.desc[0] != magic || n.phase < 0 || n.phase > 3 || bad(n.a) ||
+        bad(n.c) || (n.kind == 0 && bad(n.b))) {
+      delete v;
+      return fail(CTGB_E_VALUE, "bad VJP node");
+    }
+    q.desc_off = v->descs.size();
+    v->descs.insert(v->descs.end(), n.desc, n.desc + words);
+  }
+  v->radix.assign(vd->slice_radix, vd->slice_radix + vd->n_sliced);
+  v->project.assign(vd->slice_project, vd->slice_project + vd->n_sliced);
+  v->out_stride.assign(vd->slice_out_stride, vd->slice_out_stride + vd->n_sliced);
+  v->out_elements = vd->out_elements;
+  v->workspace_bytes = vd->workspace_bytes;
+  v->persistent_bytes = vd->persistent_bytes;
+  v->cot_offset = cplx ? vd->cotangent_offset : -1;
+  cudaError_t e = cudaMalloc((void**)&v->d_descs, v->descs.size() * sizeof(int64_t) + 8);
+  if (e == cudaSuccess)
+    e = cudaMemcpy(v->d_descs, v->descs.data(), v->descs.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    std::string msg = cudaGetErrorString(e);
+    ctgb_vjp_destroy(v);
+    return fail(CTGB_E_CUDA, "VJP plan upload: " + msg);
+  }
+  *out = v;
+  return CTGB_OK;
+}
+
+void ctgb_vjp_destroy(ctgb_vjp* v) {
+  if (!v) return;
+  if (v->d_descs) cudaFree(v->d_descs);
+  delete v;
+}
+
+size_t ctgb_vjp_workspace_bytes(const ctgb_vjp* v) {
+  return v ? (size_t)(v->workspace_bytes + v->persistent_bytes) : 0;
+}
+
+int ctgb_vjp_execute(ctgb_vjp* v, const void* const* inputs, const void* cotangent, void* const* grads,
+                     void* workspace, size_t workspace_bytes, int64_t slice_begin, int64_t slice_step,
+                     int64_t slice_count, void* stream) {
+  if (!v) return fail(CTGB_E_VALUE, "null VJP plan");
+  if (workspace_bytes < (size_t)(v->workspace_bytes + v->persistent_bytes))
+    return fail(CTGB_E_MEMORY, "workspace too small");
+  if (!inputs || !cotangent || !grads) return fail(CTGB_E_VALUE, "null argument");
+  for (int i = 0; i < v->n_inputs; ++i)
+    if (v->grad_elems[i] > 0 && !grads[i]) return fail(CTGB_E_VALUE, "missing gradient buffer of a differentiated input");
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t es = elem_size(v->dtype);
+  std::vector<int64_t> digits(v->radix.size(), 0);
+  ctgb_slice_mem mem;
+  mem.inputs = inputs;
+  mem.grads = grads;
+  mem.persistent = (char*)workspace;
+  mem.scratch = mem.persistent + v->persistent_bytes;
+  mem.cot = (const char*)cotangent;
+  mem.es = es;
+  mem.digits = digits.data();
+  int rc;
+  if (v->cot_offset >= 0) {
+    // H of the root = conj(cotangent): conjugate a copy, the caller's tensor stays as it is
+    char* copy = mem.persistent + v->cot_offset;
+    CUDA_TRY(cudaMemcpyAsync(copy, cotangent, (size_t)v->out_elements * es, cudaMemcpyDeviceToDevice, st));
+    if ((rc = conj_inplace(v->dtype, copy, v->out_elements, st))) return rc;
+    mem.cot = copy;
+  }
+  auto run_phase = [&](int phase, int64_t out_off) -> int {
+    for (const auto& n : v->nodes) {
+      if (n.phase != phase) continue;
+      char* A = resolve_tensor(v->tensors[n.a], mem, out_off);
+      char* B = n.kind == 0 ? resolve_tensor(v->tensors[n.b], mem, out_off) : nullptr;
+      char* C = resolve_tensor(v->tensors[n.c], mem, out_off);
+      if (n.zero_fill) CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)v->tensors[n.c].nbytes, st));
+      if (int r = launch_node(n.kind, v->descs.data() + n.desc_off, v->d_descs + n.desc_off, A, B, C, st)) return r;
+    }
+    return CTGB_OK;
+  };
+  // invariant forward: once per call into the persistent arena
+  if ((rc = run_phase(0, 0))) return rc;
+  // H accumulators of slice-invariant tensors collect every slice of the call
+  for (const auto& q : v->tensors)
+    if (q.kind == 6) CUDA_TRY(cudaMemsetAsync(mem.persistent + q.offset, 0, (size_t)q.nbytes, st));
+  for (int64_t k = 0; k < slice_count; ++k) {
+    const int64_t out_off = decode_slice(slice_begin + k * slice_step, v->radix, v->project, v->out_stride, digits);
+    if ((rc = run_phase(1, out_off))) return rc;
+    if ((rc = run_phase(2, out_off))) return rc;
+  }
+  // the invariant subtrees are differentiated once, from the accumulated H
+  std::fill(digits.begin(), digits.end(), 0);
+  if ((rc = run_phase(3, 0))) return rc;
+  for (int i = 0; i < v->n_inputs; ++i)
+    if (v->grad_elems[i] > 0 && (rc = conj_inplace(v->dtype, grads[i], v->grad_elems[i], st))) return rc;
   return CTGB_OK;
 }
 

@@ -85,8 +85,10 @@ enum : int {
   // (17: a DMMA-fragments-from-global variant of the next one, measured slower -- 11.1 vs 10.1 ms on
   //  the M = N = 32, K = 2^25 node -- and removed)
   VAR_ROWSTREAM_K = 19,    // N <= 8, 8 < K <= 64, 8-byte and narrower types: the row stream in chunks of 8 k
-  VAR_DMMA_32x32 = 18      // fp64 DMMA, one 32 x 32 tile with split-K over all SMs, two CTAs per SM: a few
+  VAR_DMMA_32x32 = 18,     // fp64 DMMA, one 32 x 32 tile with split-K over all SMs, two CTAs per SM: a few
                            // peeled stem tails times the other stem (M, N <= 32 over K ~ 2^25)
+  VAR_TF32_32x32 = 20      // its float32 / complex64 counterpart (3xTF32 mma.sync); chosen by VJP plans only,
+                           // for the small-result backward nodes of stem absorptions
 };
 
 // ---- single-operand descriptor (cotengra/contract.py:332-361) -------------

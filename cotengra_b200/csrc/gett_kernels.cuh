@@ -827,4 +827,11 @@ __global__ void sum_log_kernel(const double* __restrict__ f, const int* __restri
 }
 __global__ void set_double_kernel(double* p, double v) { *p = v; }
 
+// in-place complex conjugate (VJP plans: the incoming cotangent's copy and the finished input gradients)
+template <typename T>
+__global__ void conj_kernel(T* __restrict__ p, long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    p[i].y = -p[i].y;
+}
+
 }  // namespace ctgb

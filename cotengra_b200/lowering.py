@@ -60,7 +60,7 @@ VAR_SIMT_64x64, VAR_KRED, VAR_DMMA_128x64, VAR_DMMA_64x128, VAR_DMMA_256x32 = 0,
 VAR_DMMA_256x16, VAR_ROW_128x8, VAR_ROW_256x4, VAR_ROWSTREAM = 5, 6, 7, 8
 VAR_TC05_128x64, VAR_TC05_128x32, VAR_TC05_128x16 = 9, 10, 11
 VAR_DMMA3M_128x32, VAR_DMMA3M_256x16, VAR_DMMASTREAM, VAR_DOTSTREAM, VAR_DOTSTREAM4 = 12, 13, 14, 15, 16
-VAR_DMMA_32x32, VAR_ROWSTREAM_K = 18, 19
+VAR_DMMA_32x32, VAR_ROWSTREAM_K, VAR_TF32_32x32 = 18, 19, 20
 DMMASTREAM_MAX_N = 16  # the kernel takes N <= 32, but at N = 32 the staged 256x32 policy is faster (31.8 vs 26 TFLOP/s)
 TC05_VARIANTS = (VAR_TC05_128x64, VAR_TC05_128x32, VAR_TC05_128x16)
 TC05_MAX_K = 16384       # 1024 k-steps (the kernel's k table); beyond 256 in chunks of 256
@@ -87,6 +87,7 @@ VARIANT_TILES = {
     VAR_DOTSTREAM4: (4, 4, 1024),
     VAR_DMMA_32x32: (32, 32, 16),
     VAR_ROWSTREAM_K: (256, 8, 64),
+    VAR_TF32_32x32: (32, 32, 16),
 }
 
 DTYPE_CODES = {"float32": 0, "float64": 1, "complex64": 2, "complex128": 3}
@@ -425,6 +426,8 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
 
     if variant is None:
         variant = choose_variant(dtype, B, M, N, K, allow_dmma)
+    if variant == VAR_TF32_32x32 and dtype in ("float64", "complex128"):
+        variant = VAR_DMMA_32x32  # the same tile on the fp64 tensor cores
     if variant in (VAR_DMMA3M_128x32, VAR_DMMA3M_256x16) and dtype != "complex128":
         # the 3M identity is a complex128 kernel: other dtypes take the plain tensor-core tiles
         variant = VAR_DMMA_256x32 if variant == VAR_DMMA3M_128x32 else VAR_DMMA_256x16
@@ -493,7 +496,7 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
             splitk = min(steps_k, -(-2 * sm_count // tiles))
         if variant == VAR_KRED:
             splitk = min(steps_k, 4 * sm_count)
-        if variant == VAR_DMMA_32x32 and tiles == 1:
+        if variant in (VAR_DMMA_32x32, VAR_TF32_32x32) and tiles == 1:
             splitk = min(steps_k, 2 * sm_count)  # two resident CTAs per SM
     if splitk > 1:
         per = -(-steps_k // splitk)

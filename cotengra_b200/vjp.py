@@ -1,0 +1,456 @@
+"""Reverse mode through the tree executor: the vector-Jacobian product of a whole sliced tree
+compiled into one ``ctgb_vjp`` whose slice loop runs in C++/CUDA.
+
+The plan propagates the *conjugated* cotangent ``H = conj(g)``.  For a pairwise node
+``p = contract(l, r)`` torch's convention ``g_l = g_p . conj(r)^T`` becomes
+
+    H_l = contract(H_p, r -> term_l)        H_r = contract(l, H_p -> term_r)
+
+plain contractions without any conjugation, so every backward step is an ordinary pairwise
+descriptor (``lowering.build_pair_desc``) and runs on the existing kernels.  A single-operand
+node (diagonal, sum, transpose) is a real linear map: its adjoint is one single-operand
+descriptor -- a sum becomes a stride-0 read, a transpose strides, a diagonal a write along
+summed strides.  Conjugation happens only on a copy of the incoming cotangent and on the
+finished input gradients (complex dtypes).
+
+Schedule (``ctgb_vjp_execute`` runs the phases in this order):
+
+    0  invariant forward   once per call, into the persistent arena (as ``ExecPlan`` hoists)
+       -- the H accumulators of slice-invariant tensors are zeroed --
+    1  variant forward     per slice; the root is not run (it only receives H_root)
+    2  variant backward    per slice, nodes in reverse; H_root is the cotangent's slice view,
+                           input gradients accumulate through the inputs' sliced views and the
+                           H of invariant tensors accumulates in persistent buffers
+    3  invariant backward  once, from the accumulated H
+
+Only nodes on a path from the root to an input in ``wrt`` are differentiated, and a forward
+node runs only if some backward step reads its value.  Intermediates live until their last
+backward use; both arenas are laid out by liveness over the whole schedule.  The per-slice
+arena keeps every intermediate the backward needs (no recomputation).
+"""
+
+from __future__ import annotations
+
+import ctypes as C
+import math
+
+import numpy as np
+
+from . import _lib
+from .executor import ExecPlan, _align, _Arena
+from .lowering import (
+    DTYPE_CODES,
+    VAR_TF32_32x32,
+    PairDims,
+    build_pair_desc,
+    build_single_desc,
+    row_major_strides,
+    split_equation,
+    tensordot_terms,
+)
+
+PHASE_INV_FWD, PHASE_VAR_FWD, PHASE_VAR_BWD, PHASE_INV_BWD = 0, 1, 2, 3
+# tensor kinds of a VJP plan (include/ctg_b200.h)
+K_INPUT, K_SCRATCH, K_PERSISTENT, K_COT, K_GRAD, K_HACC = 0, 1, 2, 4, 5, 6
+
+
+def choose_vjp_variant(dtype, B, M, N, K):
+    """``VAR_TF32_32x32`` for the single-precision backward nodes with a small result over a long
+    contracted range (``H_B[K, N] = sum_m A[m, K] H_p[m, N]`` of a stem absorption), else None
+    (``choose_variant``'s pick).  The dot-stream kernels keep the shapes they already serve."""
+    M, N = max(M, N), min(M, N)
+    if dtype not in ("float32", "complex64") or B != 1 or M > 32 or M * N < 4 or K < 1 << 14:
+        return None
+    if M <= 4 and N <= 4 and K >= 1 << 20:
+        return None  # DOTSTREAM4
+    return VAR_TF32_32x32
+
+
+class _V:
+    """A tensor slot of the VJP schedule."""
+
+    __slots__ = ("shape", "strides", "kind", "input_index", "slice_pos", "slice_stride", "nbytes",
+                 "offset", "first", "last", "slot")
+
+    def __init__(self, shape, strides, kind, nbytes, input_index=-1, slice_pos=(), slice_stride=()):
+        self.shape = tuple(int(d) for d in shape)
+        self.strides = [int(s) for s in strides]
+        self.kind = kind
+        self.nbytes = int(nbytes)
+        self.input_index = input_index
+        self.slice_pos = list(slice_pos)
+        self.slice_stride = list(slice_stride)
+        self.offset = 0
+        self.first = None
+        self.last = -1
+        self.slot = -1
+
+
+def _axes(term, shape, strides):
+    """extent and (summed, for repeated labels) stride of every label of extent > 1"""
+    ext, st = {}, {}
+    for ix, d, s in zip(term, shape, strides):
+        if int(d) == 1:
+            continue
+        ext[ix] = int(d)
+        st[ix] = st.get(ix, 0) + int(s)
+    return ext, st
+
+
+def _is_diagonal(term, shape):
+    seen = set()
+    for ix, d in zip(term, shape):
+        if int(d) != 1:
+            if ix in seen:
+                return True
+            seen.add(ix)
+    return False
+
+
+def vjp_pair_dims(x, y, t):
+    """Index classes of the backward contraction ``T[t] (+)= sum X[x] Y[y]``; each argument is
+    ``(term, shape, strides)``.  Beyond ``classify_pair``:
+
+    * a label of the target that neither operand carries (an index summed on one operand only in
+      the forward) is a kept dim with stride 0 on both operands -- a broadcast, no copy;
+    * a label of extent 1 on the target but longer on an operand (a size-1 broadcast in the
+      forward) is contracted;
+    * a label repeated on the target (a diagonal) writes along the summed strides.
+    """
+    (ex, sx), (ey, sy), (et, stt) = _axes(*x), _axes(*y), _axes(*t)
+    order = []
+    for term in (t[0], x[0], y[0]):
+        for ix in term:
+            if ix not in order:
+                order.append(ix)
+    dims = PairDims(out_shape=tuple(int(d) for d in t[1]))
+    for ix in order:
+        a, b = sx.get(ix, 0), sy.get(ix, 0)
+        if ix in et:
+            rec = [et[ix], a, b, stt[ix]]
+            if ix in sx and ix in sy:
+                dims.batch.append(rec)
+            elif ix in sy:
+                dims.n.append(rec)
+            else:
+                dims.m.append(rec)
+        else:
+            e = ex.get(ix, ey.get(ix))
+            if e is not None:
+                dims.k.append([e, a, b, 0])
+    return dims
+
+
+def vjp_single_dims(h, t):
+    """Output dims ``[ext, sH, sT]`` of the adjoint of a single-operand node: ``T[t] (+)= H[h]``
+    broadcast over the labels ``h`` lacks (the summed ones)."""
+    (_eh, sh), (et, stt) = _axes(*h), _axes(*t)
+    order = []
+    for ix in t[0]:
+        if ix in et and ix not in order:
+            order.append(ix)
+    return [[et[ix], sh.get(ix, 0), stt[ix]] for ix in order]
+
+
+class VjpPlan:
+    """Compile the VJP of ``contractions`` (the executed IR, stem fusion included) for fixed
+    input shapes and dtype.  Same arguments as ``ExecPlan`` plus ``wrt``, the inputs that need a
+    gradient (default: all).  ``variant`` forces the kernel of every backward pairwise node."""
+
+    def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
+                 wrt=None, strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
+                 variant=None):
+        if strip_exponent:
+            raise NotImplementedError("gradients of strip_exponent results are not supported")
+        fwd = ExecPlan(contractions, inputs, output, size_dict, sliced, dtype=dtype, hoist=hoist,
+                       allow_dmma=allow_dmma, sm_count=sm_count)
+        self.fwd = fwd
+        self.dtype, self.esize, self.sm_count = fwd.dtype, fwd.esize, fwd.sm_count
+        self.inputs, self.output, self.sliced = fwd.inputs, fwd.output, fwd.sliced
+        self.nslices, self.out_shape, self.out_elements = fwd.nslices, fwd.out_shape, fwd.out_elements
+        n_in = len(self.inputs)
+        wrt = set(range(n_in)) if wrt is None else {int(i) for i in wrt}
+        if any(i < 0 or i >= n_in for i in wrt):
+            raise ValueError(f"wrt {sorted(wrt)} names inputs outside 0..{n_in - 1}")
+        self.wrt = tuple(sorted(wrt))
+        self.handle = None
+        self._keep = []
+        self._build(tuple(contractions), allow_dmma, variant)
+
+    # ------------------------------------------------------------------ build
+    def _build(self, contractions, allow_dmma, variant):
+        fwd, es, dtype = self.fwd, self.esize, self.dtype
+        nodes = fwd.nodes
+        # local index terms of every node: [(operand, term)], output term
+        ops = []
+        for (p, l, r, tdot, arg, perm), nd in zip(contractions, nodes):
+            if r is None:
+                terms, to = split_equation(arg)
+                ops.append(([(nd["a"], tuple(terms[0]))], tuple(to)))
+                continue
+            A, Bt = (nd["b"], nd["a"]) if nd["plan"].swapped else (nd["a"], nd["b"])
+            if tdot:
+                ta, tb, to = tensordot_terms((tuple(arg[0]), tuple(arg[1])), len(A.shape), len(Bt.shape), perm)
+            else:
+                (ta, tb), to = split_equation(arg)
+            ops.append(([(A, tuple(ta)), (Bt, tuple(tb))], tuple(to)))
+
+        # which tensors lead to an input in wrt (only they get an H)
+        needs = {}
+        for nd, (opl, _to) in zip(nodes, ops):
+            for t, _term in opl:
+                if t.kind == 0:
+                    needs[id(t)] = t.input_index in self.wrt
+            needs[id(nd["c"])] = any(needs[id(t)] for t, _ in opl)
+        need = lambda t: needs.get(id(t), False)  # noqa: E731
+
+        # which forward values are read (by a backward step or a forward node that runs)
+        n_nodes = len(nodes)
+        value, runs = set(), [False] * n_nodes
+        for i in range(n_nodes - 1, -1, -1):
+            nd, (opl, _to) = nodes[i], ops[i]
+            if i < n_nodes - 1 and id(nd["c"]) in value:
+                runs[i] = True
+                value.update(id(t) for t, _ in opl)
+            if need(nd["c"]) and len(opl) == 2:
+                (A, _), (Bt, _) = opl
+                if need(A):
+                    value.add(id(Bt))
+                if need(Bt):
+                    value.add(id(A))
+
+        # forward values
+        vals = {}
+        for t in (t for opl, _ in ops for t, _ in opl):
+            if t.kind == 0 and id(t) not in vals:
+                vals[id(t)] = _V(t.shape, t.strides, K_INPUT, fwd.input_nbytes[t.input_index], t.input_index,
+                                 t.slice_pos, t.slice_stride)
+        for i, nd in enumerate(nodes):
+            if runs[i]:
+                c = nd["c"]
+                kind = K_PERSISTENT if nd["invariant"] else K_SCRATCH
+                vals[id(c)] = _V(c.shape, row_major_strides(c.shape), kind, max(math.prod(c.shape), 1) * es)
+
+        # H of the root: the (conjugated) cotangent at the slice's output view
+        sliced_inds = {s[0] for s in self.sliced}
+        full_strides = row_major_strides(self.out_shape)
+        root_strides = [s for ix, s in zip(self.output, full_strides) if ix not in sliced_inds]
+        root = nodes[-1]
+        hs = {id(root["c"]): _V(root["c"].shape, root_strides, K_COT, self.out_elements * es)}
+        producer_invariant = {id(nd["c"]): bool(nd["invariant"]) for nd in nodes}
+
+        def h_of(t, consumer_invariant):
+            v = hs.get(id(t))
+            if v is None:
+                if t.kind == 0:
+                    v = _V(t.shape, t.strides, K_GRAD, fwd.input_nbytes[t.input_index], t.input_index,
+                           t.slice_pos, t.slice_stride)
+                else:
+                    # H of an invariant tensor read by the slice loop collects every slice
+                    hoisted = producer_invariant[id(t)] and not consumer_invariant
+                    kind = K_HACC if hoisted else K_SCRATCH
+                    v = _V(t.shape, row_major_strides(t.shape), kind, max(math.prod(t.shape), 1) * es)
+                hs[id(t)] = v
+            return v
+
+        fwd_nodes = {PHASE_INV_FWD: [], PHASE_VAR_FWD: []}
+        for i, nd in enumerate(nodes):
+            if runs[i]:
+                a = vals[id(nd["a"])]
+                b = vals[id(nd["b"])] if nd["b"] is not None else None
+                ph = PHASE_INV_FWD if nd["invariant"] else PHASE_VAR_FWD
+                rec = dict(kind=nd["kind"], a=a, b=b, c=vals[id(nd["c"])], words=nd["words"], phase=ph,
+                           zero_fill=False, fwd_index=i)
+                if nd["kind"] == 0:
+                    rec["plan"] = nd["plan"]
+                fwd_nodes[ph].append(rec)
+
+        bwd_nodes = {PHASE_VAR_BWD: [], PHASE_INV_BWD: []}
+        self.macs_fwd = [0, 0]  # (per slice, once per call)
+        self.macs_bwd = [0, 0]
+        for rec in fwd_nodes[PHASE_INV_FWD] + fwd_nodes[PHASE_VAR_FWD]:
+            if rec["kind"] == 0:
+                Bn, M, N, K = rec["plan"].sizes
+                self.macs_fwd[rec["phase"] == PHASE_INV_FWD] += Bn * M * N * K
+        for i in range(n_nodes - 1, -1, -1):
+            nd, (opl, to) = nodes[i], ops[i]
+            if not need(nd["c"]):
+                continue
+            inv = bool(nd["invariant"])
+            ph = PHASE_INV_BWD if inv else PHASE_VAR_BWD
+            Hc = hs[id(nd["c"])]
+            hc_arg = (to, nd["c"].shape, Hc.strides)
+            if len(opl) == 1:
+                (X, tx), = opl
+                if not need(X):
+                    continue
+                HX = h_of(X, inv)
+                odims = vjp_single_dims(hc_arg, (tx, X.shape, HX.strides))
+                diag = _is_diagonal(tx, X.shape)
+                acc = HX.kind in (K_GRAD, K_HACC) or diag
+                words = build_single_desc(odims, [], dtype, accumulate=acc)
+                bwd_nodes[ph].append(dict(kind=1, a=Hc, b=None, c=HX, words=words, phase=ph,
+                                          zero_fill=diag and HX.kind == K_SCRATCH, fwd_index=i))
+                continue
+            n_h = 0
+            for (X, tx), (Y, ty) in ((opl[0], opl[1]), (opl[1], opl[0])):
+                if not need(X):
+                    continue
+                HX = h_of(X, inv)
+                Yv = vals[id(Y)]
+                dims = vjp_pair_dims(hc_arg, (ty, Y.shape, Yv.strides), (tx, X.shape, HX.strides))
+                diag = _is_diagonal(tx, X.shape)
+                acc = HX.kind in (K_GRAD, K_HACC) or diag
+                dense = 0 if acc else math.prod(X.shape)
+                v = variant
+                if v is None:
+                    v = choose_vjp_variant(dtype, *dims.sizes())
+                plan = build_pair_desc(dims, dtype, accumulate=acc, sm_count=self.sm_count,
+                                       allow_dmma=allow_dmma, c_dense_elems=dense, variant=v)
+                a, b = (Yv, Hc) if plan.swapped else (Hc, Yv)
+                bwd_nodes[ph].append(dict(kind=0, a=a, b=b, c=HX, words=plan.words, phase=ph,
+                                          zero_fill=diag and HX.kind == K_SCRATCH, plan=plan, fwd_index=i))
+                n_h += 1
+            if n_h:
+                Bn, M, N, K = nd["plan"].sizes
+                self.macs_bwd[inv] += n_h * Bn * M * N * K
+
+        sched = (fwd_nodes[PHASE_INV_FWD] + [None] + fwd_nodes[PHASE_VAR_FWD] + bwd_nodes[PHASE_VAR_BWD]
+                 + bwd_nodes[PHASE_INV_BWD])
+        self.nodes = [nd for nd in sched if nd is not None]
+        self.n_backward_nodes = len(bwd_nodes[PHASE_VAR_BWD]) + len(bwd_nodes[PHASE_INV_BWD])
+        self.differentiated = sorted({nd["fwd_index"] for nd in self.nodes if nd["phase"] >= PHASE_VAR_BWD})
+        self._layout(sched)
+        self._marshal()
+
+    def _layout(self, sched):
+        """Offsets in the two arenas by liveness over the whole forward + backward schedule."""
+        zero_pos = sched.index(None)
+        end_loop = zero_pos
+        for pos, nd in enumerate(sched):
+            if nd is not None and nd["phase"] in (PHASE_VAR_FWD, PHASE_VAR_BWD):
+                end_loop = pos
+        tensors = []
+        for pos, nd in enumerate(sched):
+            if nd is None:
+                continue
+            for t in (nd["a"], nd["b"], nd["c"]):
+                if t is not None and t.slot < 0:
+                    t.slot = len(tensors)
+                    tensors.append(t)
+            c = nd["c"]
+            if c.first is None:
+                c.first = zero_pos if c.kind == K_HACC else pos
+            for s in (nd["a"], nd["b"]):
+                if s is None:
+                    continue
+                s.last = max(s.last, pos)
+                # persistent values read inside the slice loop must survive every slice
+                if s.kind == K_PERSISTENT and nd["phase"] in (PHASE_VAR_FWD, PHASE_VAR_BWD):
+                    s.last = max(s.last, end_loop)
+        self.tensors = tensors
+        persistent, scratch = _Arena(), _Arena()
+        self.cotangent_offset = -1
+        if self.dtype.startswith("complex"):
+            self.cotangent_offset = persistent.alloc(self.out_elements * self.esize)
+        arena = {K_SCRATCH: scratch, K_PERSISTENT: persistent, K_HACC: persistent}
+        placed = [t for t in tensors if t.kind in arena]
+        for t in placed:
+            t.last = max(t.last, t.first)
+        for pos in range(len(sched)):
+            for t in placed:
+                if t.first == pos:
+                    t.offset = arena[t.kind].alloc(t.nbytes)
+            for t in placed:
+                if t.last == pos:
+                    arena[t.kind].release(t.offset, t.nbytes)
+        self.workspace_bytes = _align(scratch.peak)
+        self.persistent_bytes = _align(persistent.peak)
+        self.total_bytes = self.workspace_bytes + self.persistent_bytes
+
+    def _marshal(self):
+        n_t = len(self.tensors)
+        ct = (_lib.CtgbTensor * max(n_t, 1))()
+        for i, t in enumerate(self.tensors):
+            ct[i].kind = t.kind
+            ct[i].input_index = t.input_index
+            ct[i].offset = t.offset
+            ct[i].nbytes = t.nbytes
+            ct[i].n_sliced = len(t.slice_pos)
+            if t.slice_pos:
+                pos = (C.c_int32 * len(t.slice_pos))(*t.slice_pos)
+                st = (C.c_int64 * len(t.slice_stride))(*t.slice_stride)
+                self._keep += [pos, st]
+                ct[i].slice_pos = C.cast(pos, C.POINTER(C.c_int32))
+                ct[i].slice_stride = C.cast(st, C.POINTER(C.c_int64))
+        cn = (_lib.CtgbVjpNode * max(len(self.nodes), 1))()
+        for i, nd in enumerate(self.nodes):
+            words = np.ascontiguousarray(nd["words"], dtype=np.int64)
+            self._keep.append(words)
+            cn[i].kind = nd["kind"]
+            cn[i].a = nd["a"].slot
+            cn[i].b = nd["b"].slot if nd["b"] is not None else -1
+            cn[i].c = nd["c"].slot
+            cn[i].phase = nd["phase"]
+            cn[i].zero_fill = int(nd["zero_fill"])
+            cn[i].desc = words.ctypes.data_as(C.POINTER(C.c_int64))
+        ns = len(self.sliced)
+        radix = (C.c_int64 * max(ns, 1))(*[s for _i, s, _p in self.sliced])
+        proj = (C.c_int64 * max(ns, 1))(*[(-1 if p is None else p) for _i, _s, p in self.sliced])
+        ostr = (C.c_int64 * max(ns, 1))(*[int(self.fwd._pd.slice_out_stride[j]) for j in range(ns)])
+        vd = _lib.CtgbVjpDesc()
+        vd.dtype = DTYPE_CODES[self.dtype]
+        vd.n_inputs = len(self.inputs)
+        vd.n_tensors = n_t
+        vd.tensors = C.cast(ct, C.POINTER(_lib.CtgbTensor))
+        vd.n_nodes = len(self.nodes)
+        vd.nodes = C.cast(cn, C.POINTER(_lib.CtgbVjpNode))
+        vd.n_sliced = ns
+        vd.slice_radix = C.cast(radix, C.POINTER(C.c_int64))
+        vd.slice_project = C.cast(proj, C.POINTER(C.c_int64))
+        vd.slice_out_stride = C.cast(ostr, C.POINTER(C.c_int64))
+        vd.out_elements = self.out_elements
+        vd.workspace_bytes = self.workspace_bytes
+        vd.persistent_bytes = self.persistent_bytes
+        vd.cotangent_offset = self.cotangent_offset
+        self._keep += [ct, cn, radix, proj, ostr]
+        self._vd = vd
+
+    # ------------------------------------------------------------------ work
+    def vjp_macs(self, count):
+        """Scalar MACs of one call over ``count`` slices: the recomputed forward (root excluded)
+        plus, for every differentiated pairwise node, its MACs times the number of H it forms."""
+        return (self.macs_fwd[0] + self.macs_bwd[0]) * count + self.macs_fwd[1] + self.macs_bwd[1]
+
+    def variants(self, phases=(PHASE_VAR_BWD, PHASE_INV_BWD)):
+        """Kernel variants of the pairwise nodes of the given phases (the backward ones by default)."""
+        return [int(nd["words"][32]) for nd in self.nodes if nd["kind"] == 0 and nd["phase"] in phases]
+
+    # ------------------------------------------------------------------ device side
+    def create(self):
+        """Upload the plan to the current CUDA device."""
+        if self.handle is not None:
+            return self
+        lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(lib.ctgb_vjp_create(C.byref(self._vd), C.byref(h)))
+        self.handle = h
+        return self
+
+    def execute(self, input_ptrs, cot_ptr, grad_ptrs, ws_ptr, ws_bytes, begin, step, count, stream=0):
+        lib = _lib.load()
+        arr = (C.c_void_p * len(input_ptrs))(*input_ptrs)
+        grads = (C.c_void_p * len(grad_ptrs))(*grad_ptrs)
+        _lib.check(lib.ctgb_vjp_execute(self.handle, arr, cot_ptr, grads, ws_ptr, ws_bytes, int(begin),
+                                        int(step), int(count), stream))
+
+    def destroy(self):
+        if self.handle is not None:
+            _lib.load().ctgb_vjp_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass

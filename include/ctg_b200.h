@@ -192,6 +192,62 @@ int ctgb_plan_profile_read(ctgb_plan* plan, float* ms, int n_nodes);
  * only HBM and bf16 numbers). */
 int ctgb_probe_fp64_peaks(double* dmma_tflops, double* dfma_tflops, void* stream);
 
+/* ---- reverse mode (vector-Jacobian products) ----------------------------- */
+
+typedef struct ctgb_vjp ctgb_vjp;
+
+/* A VJP plan propagates H = conj(cotangent) from the root to the inputs; every
+ * backward step is an ordinary pairwise or single-operand descriptor.  Its
+ * tensor slots are ctgb_tensor records with kinds 0-2 as in plans plus
+ *   4 = the cotangent's view of the slice (element offset as the root's output
+ *       view, slice_out_stride),
+ *   5 = the gradient of network input `input_index` (slice offset as kind 0),
+ *   6 = a persistent accumulator at byte offset `offset` of the persistent
+ *       arena, zeroed before the slice loop (H of a slice-invariant tensor). */
+typedef struct {
+  int32_t kind;       /* 0 = pairwise, 1 = single-operand                       */
+  int32_t a, b, c;    /* tensor slots (b unused for kind 1)                     */
+  int32_t phase;      /* 0 invariant forward (once), 1 variant forward, 2 variant
+                         backward (per slice), 3 invariant backward (once, last) */
+  int32_t zero_fill;  /* 1: zero tensor c (nbytes) before the launch           */
+  const int64_t* desc;
+} ctgb_vjp_node;
+
+typedef struct {
+  int32_t dtype;
+  int32_t n_inputs;
+  int32_t n_tensors;
+  const ctgb_tensor* tensors;
+  int32_t n_nodes;
+  const ctgb_vjp_node* nodes;
+  int32_t n_sliced;
+  const int64_t* slice_radix;
+  const int64_t* slice_project;
+  const int64_t* slice_out_stride;
+  int64_t out_elements;       /* elements of the full output (the cotangent) */
+  int64_t workspace_bytes;    /* per-slice arena                              */
+  int64_t persistent_bytes;   /* arena kept over the whole call               */
+  int64_t cotangent_offset;   /* complex dtypes: byte offset of the conjugated
+                                 cotangent copy in the persistent arena        */
+} ctgb_vjp_desc;
+
+int ctgb_vjp_create(const ctgb_vjp_desc* desc, ctgb_vjp** vjp);
+void ctgb_vjp_destroy(ctgb_vjp* vjp);
+size_t ctgb_vjp_workspace_bytes(const ctgb_vjp* vjp);
+/* The input gradients of the sum of slices slice_begin, slice_begin +
+ * slice_step, ... (slice_count of them) for the output cotangent `cotangent`
+ * (device, out_elements).  `grads` is a host array of n_inputs device
+ * pointers, null for inputs that are not differentiated; the caller zeroes the
+ * buffers (the final conjugation of complex gradients acts on the whole
+ * buffer), and on return they hold the finished gradients in torch's
+ * convention (grad_x = sum over outputs of grad_out * conj(d out / d x)).  A workspace smaller than ctgb_vjp_workspace_bytes()
+ * fails with CTGB_E_MEMORY before any launch.  Asynchronous on `stream`. */
+int ctgb_vjp_execute(ctgb_vjp* vjp, const void* const* inputs,
+                     const void* cotangent, void* const* grads,
+                     void* workspace, size_t workspace_bytes,
+                     int64_t slice_begin, int64_t slice_step,
+                     int64_t slice_count, void* stream);
+
 /* Number of kernels this library has launched since load (bench.py's
  * `gpu_launches`). */
 int64_t ctgb_launch_count(void);

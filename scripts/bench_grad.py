@@ -1,0 +1,106 @@
+"""Gradient benchmark: forward + VJP of one BASELINE configuration on one GPU, against the same
+tree under torch GPU autograd.  Prints one JSON line with the card name and power limit.
+
+    python scripts/bench_grad.py --config peps8x8 --dtype complex64 [--steps 10 --warmup 3]
+                                 [--slices-per-gpu 2] [--no-fuse]
+
+Gradient TFLOP/s are quoted on the VJP work: the recomputed forward (root excluded) plus, for each
+differentiated pairwise node, its MACs times the number of H it forms (8 flops per complex
+multiply-add, 2 per real one).  Trees whose VJP workspace does not fit the card report the bytes
+they need.  Writes nothing to the tree.
+"""
+import argparse
+import json
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np  # noqa: E402
+
+import bench  # noqa: E402
+
+
+def run_grad(args):
+    """Forward + VJP (``TreeExecutor.vjp``, every input differentiated, cotangent of ones)
+    on one GPU, against the same tree under torch GPU autograd (``torch.einsum`` / ``tensordot`` per
+    node, cuBLAS).  Gradient TFLOP/s are quoted on the VJP work: the recomputed forward (root
+    excluded) plus, per differentiated pairwise node, its MACs times the number of H it forms."""
+    import subprocess
+
+    import torch
+
+    import cotengra_b200 as cb
+
+    try:
+        card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception:
+        card = torch.cuda.get_device_name(0) + ", power limit unknown"
+    spec, arrays, desc = bench.load_workload(args.config, args.dtype)
+    ex = cb.TreeExecutor(spec, dtype=args.dtype, fuse=not args.no_fuse)
+    count = min(ex.nslices, args.slices_per_gpu)
+    plan = ex.vjp_plan()
+    line = {"metric": f"{args.config}_grad", "config": args.config, "dtype": args.dtype, "workload": desc,
+            "card": card, "slices": count, "vjp_workspace_bytes": plan.total_bytes}
+    free = torch.cuda.mem_get_info()[0]
+    if plan.total_bytes > 0.8 * free:
+        line["note"] = f"the VJP workspace ({plan.total_bytes} bytes) does not fit the card ({free} bytes free)"
+        print(json.dumps(line))
+        return
+    dev = [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in arrays]
+    cot = torch.ones(ex.plan.out_shape, dtype=dev[0].dtype, device="cuda")
+
+    def timed(fn):
+        for _ in range(args.warmup):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.steps):
+            res = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / 1e3 / args.steps, res
+
+    t_fwd, _ = timed(lambda: ex.contract_device(dev, 0, 1, count))
+    t_vjp, grads = timed(lambda: ex.vjp(dev, cot, 0, 1, count))
+    t_both, _ = timed(lambda: (ex.contract_device(dev, 0, 1, count), ex.vjp(dev, cot, 0, 1, count)))
+    per_mac = 8 if "complex" in args.dtype else 2
+
+    def torch_step():
+        # the caller's tree, slice by slice (every config here has no sliced output index)
+        ts = [t.detach().requires_grad_() for t in dev]
+        out = None
+        for i in range(count):
+            r = bench.torch_run_contractions(spec.contractions(), bench.torch_slice_arrays(spec, ts, i))
+            out = r if out is None else out + r
+        return torch.autograd.grad(out, ts, grad_outputs=torch.ones_like(out))
+
+    t_torch, tgrads = timed(torch_step)
+    diff = max(float(torch.linalg.vector_norm(g - w) / max(float(torch.linalg.vector_norm(w)), 1e-300))
+               for g, w in zip(grads, tgrads))
+    line.update({
+        "grad_tflops": per_mac * plan.vjp_macs(count) / t_vjp / 1e12,
+        "flops_convention": f"{per_mac} flops per scalar multiply-add on the VJP work "
+                            "(recomputed forward without the root + MACs x H formed per differentiated node)",
+        "forward_s": t_fwd, "vjp_s": t_vjp, "forward_plus_vjp_s": t_both,
+        "ratio_forward_plus_vjp_over_forward": t_both / t_fwd,
+        "torch_autograd_s": t_torch, "speedup_vs_torch_autograd": t_torch / t_both,
+        "max_rel_grad_diff_vs_torch": diff,
+    })
+    print(json.dumps(line))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--config", default="peps8x8", choices=sorted(bench.METRICS))
+    ap.add_argument("--dtype", default="complex64", choices=["complex128", "complex64"])
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--slices-per-gpu", type=int, default=2)
+    ap.add_argument("--no-fuse", action="store_true", help="differentiate the reference's node sequence one to one")
+    run_grad(ap.parse_args())
+
+
+if __name__ == "__main__":
+    main()
