@@ -787,8 +787,8 @@ int ctgb_probe_fp64_peaks(double* dmma_tflops, double* dfma_tflops, void* stream
     return CTGB_OK;
   };
   int rc = CTGB_OK;
-  // one DMMA = 8*8*4 MACs per warp = 512 flop / 32 lanes; 8 per iteration
-  if (dmma_tflops) rc = timed(0, 8 * 512.0 / 32.0, dmma_tflops);
+  // one DMMA = 16*8*4 MACs per warp = 1024 flop / 32 lanes; 8 per iteration
+  if (dmma_tflops) rc = timed(0, 8 * 1024.0 / 32.0, dmma_tflops);
   if (!rc && dfma_tflops) rc = timed(1, 8 * 2.0, dfma_tflops);
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);

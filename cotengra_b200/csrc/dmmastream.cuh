@@ -2,11 +2,11 @@
 // (N <= 8*NJ, K <= 64, no batch): the rowstream idea with DMMA fragments.
 //
 // Every warp owns blocks of 32 output rows and runs them start to finish on its own:
-// A fragments straight from global memory into registers (a lane of the m8k4 A fragment
-// holds one complex element: one LDG.128, 16 of them in flight per lane), B fragments from
-// a zero-padded shared-memory copy made once per CTA, 4 real DMMAs per fragment pair, 128-bit
-// stores.  No operand staging, no producer warps, no CTA barriers in the loop: the warps of
-// an SM drift apart, so loads, DMMAs and stores of different row blocks overlap by themselves
+// A fragments straight from global memory into registers (a lane holds one complex element
+// per 8-row group: two LDG.64, 32 of them in flight per lane), B fragments from a
+// zero-padded shared-memory copy made once per CTA, 4 real m16n8k4 DMMAs per pair of 8-row
+// groups and B fragment, 128-bit stores.  No operand staging, no producer warps, no CTA
+// barriers in the loop: the warps of an SM drift apart, so loads, DMMAs and stores of different row blocks overlap by themselves
 // -- which the staged 256x16 policy could not do (all consumer warps share one phase: ncu
 // showed its N=16 K=16 node with compute and HBM time adding up instead of overlapping).
 // (included inside namespace ctgb)
@@ -96,7 +96,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
   const unsigned long long wstride = (unsigned long long)gridDim.x * (blockDim.x >> 5);
   for (unsigned long long blk = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (tid >> 5); blk < nblk;
        blk += wstride) {
-    // the lane's four rows (one per m8 fragment)
+    // the lane's four rows, one per 8-row group (groups 0,1 and 2,3 each form an m16 fragment)
     long long oa[4], oc[4];
     bool live[4];
 #pragma unroll
@@ -131,7 +131,10 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
 #pragma unroll
       for (int j = 0; j < NJ; ++j) re[i][j][0] = re[i][j][1] = im[i][j][0] = im[i][j][1] = 0.0;
     for (int kc = 0; kc < kchunks; ++kc) {
-      // 16 independent 128-bit loads per lane: element (row i*8 + frow, k = kc*16 + k4*4 + fk)
+      // 32 independent 64-bit loads per lane: element (row i*8 + frow, k = kc*16 + k4*4 + fk).
+      // Not one 128-bit load per element: an m16n8k4 A operand is the real (or imaginary)
+      // parts of two rows in adjacent registers, and 128-bit loads make ptxas copy them
+      // there, which spilled the NJ = 2 kernels.
       double2 a[4][4];
 #pragma unroll
       for (int k4 = 0; k4 < 4; ++k4) {
@@ -139,7 +142,11 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
         const long long ko = s_akoff[kk & (DS_KMAX - 1)];
         const bool kin = kk < K;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) a[i][k4] = kin ? A[oa[i] + ko] : make_double2(0.0, 0.0);
+        for (int i = 0; i < 4; ++i) {
+          const double* pa = reinterpret_cast<const double*>(A + oa[i] + ko);
+          a[i][k4].x = kin ? __ldg(pa) : 0.0;
+          a[i][k4].y = kin ? __ldg(pa + 1) : 0.0;
+        }
       }
 #pragma unroll
       for (int k4 = 0; k4 < 4; ++k4) {
@@ -149,25 +156,25 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
 #pragma unroll
         for (int j = 0; j < NJ; ++j) b[j] = s_B[(kc * 16 + k4 * 4 + fk) * DS_NMAX + j * 8 + frow];
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; i += 2)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
-            if (j < n8s) dmma8x8x4(re[i][j][0], re[i][j][1], a[i][k4].x, b[j].x);
+            if (j < n8s) dmma16x8x4(re[i][j], re[i + 1][j], a[i][k4].x, a[i + 1][k4].x, b[j].x);
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int j = 0; j < NJ; ++j)
-            if (j < n8s) dmma8x8x4(im[i][j][0], im[i][j][1], a[i][k4].x, b[j].y);
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; i += 2)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
-            if (j < n8s) dmma8x8x4(re[i][j][0], re[i][j][1], -a[i][k4].y, b[j].y);
+            if (j < n8s) dmma16x8x4(im[i][j], im[i + 1][j], a[i][k4].x, a[i + 1][k4].x, b[j].y);
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; i += 2)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
-            if (j < n8s) dmma8x8x4(im[i][j][0], im[i][j][1], a[i][k4].y, b[j].x);
+            if (j < n8s) dmma16x8x4(re[i][j], re[i + 1][j], a[i][k4].y, a[i + 1][k4].y, -b[j].y);
+#pragma unroll
+        for (int i = 0; i < 4; i += 2)
+#pragma unroll
+          for (int j = 0; j < NJ; ++j)
+            if (j < n8s) dmma16x8x4(im[i][j], im[i + 1][j], a[i][k4].y, a[i + 1][k4].y, b[j].x);
       }
     }
     if constexpr (STRIP) {

@@ -67,7 +67,7 @@ constexpr int64_t DESC_MAGIC = 0x43544742'32303031LL;  // "CTGB2001"
 enum : int {
   VAR_SIMT_64x64 = 0,  // generic FMA tile kernel, any dtype / any extents
   VAR_KRED = 1,        // tiny M x N, huge K: per-thread k partial sums
-  VAR_DMMA_128x64 = 2, // fp64 tensor-core (mma.sync m8n8k4) tile kernel
+  VAR_DMMA_128x64 = 2, // fp64 tensor-core (mma.sync m16n8k4) tile kernel
   VAR_DMMA_64x128 = 3,
   VAR_DMMA_256x32 = 4,
   VAR_DMMA_256x16 = 5,

@@ -10,7 +10,7 @@
 //   * a 3-4 stage shared-memory ring hides HBM/L2 latency;
 //   * the compute policy is pluggable: FMA register tiles (any dtype), per-thread
 //     k partial sums (dot-product-like nodes), or fp64 tensor-core mma.sync
-//     (DMMA m8n8k4) for float64 / complex128;
+//     (DMMA m16n8k4) for float64 / complex128;
 //   * results are stored straight into the parent's index order (strided C),
 //     optionally accumulated (slice sums, core.py:3842-3844) or atomically
 //     added (split-K).
@@ -462,21 +462,35 @@ struct RowPolicy {
   }
 };
 
-// fp64 tensor-core policy: mma.sync.aligned.m8n8k4 (DMMA).  wgmma has no f64
+// fp64 tensor-core policy: mma.sync.aligned.m16n8k4 (DMMA).  wgmma has no f64
 // kind (f16/bf16/tf32/fp8/int8 only), so the double-precision tensor path on
-// sm_90a is the warp-level DMMA.
-// Complex products are four real DMMAs per (A-frag, B-frag) pair:
-//   Cr += Ar*Br;  Cr += (-Ai)*Bi;  Ci += Ar*Bi;  Ci += Ai*Br
-// or, with M3 ("3M", the ZGEMM3M identity), three:
+// sm_90a is the warp-level DMMA, and m16n8k4 is the smallest f64 shape sm_90a runs
+// at the full rate (m8n8k4 runs at half of it; DESIGN.md section 4).
+//
+// dmma16x8x4: D[16x8] += A[16x4] * B[4x8].  With g = lane / 4 and t = lane % 4 a
+// lane holds A rows g (a0) and g + 8 (a1) at k = t, the B element of k = t, column
+// g, and D rows g (lo) and g + 8 (hi) at columns 2t, 2t + 1.
+__device__ __forceinline__ void dmma16x8x4(double (&lo)[2], double (&hi)[2], double a0, double a1, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+               : "+d"(lo[0]), "+d"(lo[1]), "+d"(hi[0]), "+d"(hi[1])
+               : "d"(a0), "d"(a1), "d"(b));
+}
+
+// Complex products (TR, the default complex path) run transposed, C^T = B^T A^T,
+// with the 16 rows of the instruction's A being the real and the imaginary part of
+// 8 columns of B:
+//   [Cr; Ci]^T += [ Br;  Bi] * Ar        [Cr; Ci]^T += [-Bi;  Br] * Ai
+// so a lane's A operand is one complex B element as it comes out of shared memory
+// (no register shuffling), each accumulator sees the same products in the same
+// order as Cr += Ar*Br, Cr += (-Ai)*Bi, Ci += Ar*Bi, Ci += Ai*Br, and a lane owns two
+// adjacent rows of C in one column.  Real products and M3 ("3M", the ZGEMM3M
+// identity, three DMMAs per fragment pair:
 //   P1 += Ar*Br;  P2 += Ai*Bi;  P3 += (Ar+Ai)*(Br+Bi);   Cr = P1 - P2,  Ci = P3 - P1 - P2
 // -- 25 % fewer tensor-pipe cycles for 50 % more accumulator registers (hence the
 // narrower warp tiles of the 3M variants) and a normwise (not componentwise) error
-// bound of the same order, K*eps*|A||B|.
-__device__ __forceinline__ void dmma8x8x4(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
+// bound of the same order, K*eps*|A||B|) pair two 8-row A fragments per instruction
+// instead: rows g and g + 8 of the instruction are rows g of fragments i and i + 1,
+// and a lane owns two adjacent columns of C in one row.
 
 template <typename T, int WARPS_M, int WARPS_N, int FM, int FN, int KT_, int STAGES_, bool M3_ = false>
 struct DmmaPolicy {
@@ -492,6 +506,8 @@ struct DmmaPolicy {
   static constexpr bool HAS_BCACHE = false;
   static constexpr int MIN_BLOCKS = THREADS <= 128 ? 2 : 1;  // the 32 x 32 split-K policy: two CTAs per SM
   static_assert(KT % 4 == 0, "KT must be a multiple of the DMMA k");
+  static_assert(FM % 2 == 0, "real and 3M products issue one m16n8k4 DMMA per two 8-row fragments");
+  static constexpr bool TR = CPLX && !M3;  // transposed complex product (see above)
   static constexpr bool SCAN_OK = true;
   struct Acc {
     double re[FM][FN][2];
@@ -528,52 +544,43 @@ struct DmmaPolicy {
 #pragma unroll
       for (int j = 0; j < FN; ++j) b[j] = pb[(k4 * NT + j * 8) * 4];
       if constexpr (M3) {
-        // three passes of FM*FN independent DMMAs
+        // three passes of FM/2*FN independent DMMAs
         double as[FM], bs[FN];
 #pragma unroll
         for (int i = 0; i < FM; ++i) as[i] = a[i].x + a[i].y;
 #pragma unroll
         for (int j = 0; j < FN; ++j) bs[j] = b[j].x + b[j].y;
 #pragma unroll
-        for (int i = 0; i < FM; ++i)
+        for (int i = 0; i < FM; i += 2)
 #pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.re[i][j][0], acc.re[i][j][1], a[i].x, b[j].x);
+          for (int j = 0; j < FN; ++j) dmma16x8x4(acc.re[i][j], acc.re[i + 1][j], a[i].x, a[i + 1].x, b[j].x);
 #pragma unroll
-        for (int i = 0; i < FM; ++i)
+        for (int i = 0; i < FM; i += 2)
 #pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.im[i][j][0], acc.im[i][j][1], a[i].y, b[j].y);
+          for (int j = 0; j < FN; ++j) dmma16x8x4(acc.im[i][j], acc.im[i + 1][j], a[i].y, a[i + 1].y, b[j].y);
 #pragma unroll
-        for (int i = 0; i < FM; ++i)
+        for (int i = 0; i < FM; i += 2)
 #pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.p3[i][j][0], acc.p3[i][j][1], as[i], bs[j]);
+          for (int j = 0; j < FN; ++j) dmma16x8x4(acc.p3[i][j], acc.p3[i + 1][j], as[i], as[i + 1], bs[j]);
       } else if constexpr (CPLX) {
-        // four passes of FM*FN independent DMMAs: the two updates of one
-        // accumulator are FM*FN*2 instructions apart, so the tensor pipe never
-        // waits on its own result
-        double nai[FM];
+        // two passes of FM*FN independent DMMAs: the two updates of one accumulator
+        // are FM*FN instructions apart, so the tensor pipe never waits on its own result
+        double2 nb[FN];
 #pragma unroll
-        for (int i = 0; i < FM; ++i) nai[i] = -a[i].y;
-#pragma unroll
-        for (int i = 0; i < FM; ++i)
-#pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.re[i][j][0], acc.re[i][j][1], a[i].x, b[j].x);
+        for (int j = 0; j < FN; ++j) nb[j] = make_double2(-b[j].y, b[j].x);
 #pragma unroll
         for (int i = 0; i < FM; ++i)
 #pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.im[i][j][0], acc.im[i][j][1], a[i].x, b[j].y);
+          for (int j = 0; j < FN; ++j) dmma16x8x4(acc.re[i][j], acc.im[i][j], b[j].x, b[j].y, a[i].x);
 #pragma unroll
         for (int i = 0; i < FM; ++i)
 #pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.re[i][j][0], acc.re[i][j][1], nai[i], b[j].y);
-#pragma unroll
-        for (int i = 0; i < FM; ++i)
-#pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.im[i][j][0], acc.im[i][j][1], a[i].y, b[j].x);
+          for (int j = 0; j < FN; ++j) dmma16x8x4(acc.re[i][j], acc.im[i][j], nb[j].x, nb[j].y, a[i].y);
       } else {
 #pragma unroll
-        for (int i = 0; i < FM; ++i)
+        for (int i = 0; i < FM; i += 2)
 #pragma unroll
-          for (int j = 0; j < FN; ++j) dmma8x8x4(acc.re[i][j][0], acc.re[i][j][1], a[i], b[j]);
+          for (int j = 0; j < FN; ++j) dmma16x8x4(acc.re[i][j], acc.re[i + 1][j], a[i], a[i + 1], b[j]);
       }
     }
   }
@@ -602,6 +609,14 @@ struct DmmaPolicy {
     for (int i = 0; i < FM; ++i)
 #pragma unroll
       for (int j = 0; j < FN; ++j) {
+        if constexpr (TR) {
+          // a lane owns rows fc, fc + 1 of column frow of the fragment
+          const int r = (wm * FM + i) * 8 + fc;
+          const int c = (wn * FN + j) * 8 + frow;
+          store(r, c, make_double2(acc.re[i][j][0], acc.im[i][j][0]));
+          store(r + 1, c, make_double2(acc.re[i][j][1], acc.im[i][j][1]));
+          continue;
+        }
         const int r = (wm * FM + i) * 8 + frow;
         const int c = (wn * FN + j) * 8 + fc;
         if constexpr (CPLX) {

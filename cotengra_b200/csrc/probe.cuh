@@ -1,25 +1,23 @@
 // probe.cuh -- register-resident microbenchmarks for the fp64 roofline
-// denominators (DMMA m8n8k4 tensor pipe and DFMA pipe) on the current device.
+// denominators (the m16n8k4 DMMA the fp64 tensor-core kernels issue, and the
+// DFMA pipe) on the current device.  Include after gett_kernels.cuh.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace ctgb {
 
 __global__ void __launch_bounds__(256) probe_dmma_kernel(double* sink, int iters) {
-  double c[8][2];
+  double c[8][2][2];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) c[i][0] = c[i][1] = 0.0;
+  for (int i = 0; i < 8; ++i) c[i][0][0] = c[i][0][1] = c[i][1][0] = c[i][1][1] = 0.0;
   double a = 1.0 + threadIdx.x * 1e-9, b = 1.0 - threadIdx.x * 1e-9;
   for (int it = 0; it < iters; ++it) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                   : "+d"(c[i][0]), "+d"(c[i][1])
-                   : "d"(a), "d"(b));
+    for (int i = 0; i < 8; ++i) dmma16x8x4(c[i][0], c[i][1], a, a, b);
   }
   double s = 0.0;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1];
+  for (int i = 0; i < 8; ++i) s += c[i][0][0] + c[i][0][1] + c[i][1][0] + c[i][1][1];
   if (s == 123.456) sink[0] = s;
 }
 

@@ -186,7 +186,7 @@ int ctgb_plan_execute_host(ctgb_plan* plan, const void* const* host_inputs,
 int ctgb_plan_profile(ctgb_plan* plan, int enable);
 int ctgb_plan_profile_read(ctgb_plan* plan, float* ms, int n_nodes);
 
-/* Measured fp64 tensor-core (DMMA m8n8k4) and fp64 FMA peaks of the current
+/* Measured fp64 tensor-core (DMMA m16n8k4) and fp64 FMA peaks of the current
  * device in TFLOP/s, from a register-resident microbenchmark kernel: the
  * denominators bench.py uses for the fp64 roofline (MEASURED_PEAKS.json holds
  * only HBM and bf16 numbers). */
