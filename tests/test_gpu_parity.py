@@ -104,22 +104,48 @@ def test_tensordot_golden_shapes():
         assert rel_err(got, want) < 1e-12
 
 
+_RAGGED_GEMMS = [(130, 70, 19), (257, 3, 33), (5, 300, 9), (512, 128, 64), (1000, 96, 40)]
+# (m, n, k) that each non-staged variant accepts as it is (build_pair_desc falls back otherwise)
+_GEMMS_ACCEPTED = {
+    L.VAR_ROWSTREAM: [(200, 3, 4), (512, 2, 7), (768, 8, 8), (1024, 6, 5), (256, 5, 2)],
+    L.VAR_DMMASTREAM: [(4096, 16, 16), (1024, 9, 32), (768, 32, 7), (512, 8, 64), (200, 24, 20)],
+    L.VAR_DOTSTREAM: [(1, 1, 6144), (1, 1, 2048), (1, 1, 1000), (1, 1, 10240), (1, 1, 4096)],
+    **{v: [(256, 64, 32), (384, 64, 48), (128, 48, 16), (512, 96, 64), (1000, 64, 40)] for v in L.TC05_VARIANTS},
+}
+
+
+def _variant_that_runs(variant, dtype, m, n, k):
+    """The forced variant, or what build_pair_desc documents for a dtype the kernel does not take."""
+    if variant in (L.VAR_DMMA3M_128x32, L.VAR_DMMA3M_256x16) and dtype != "complex128":
+        return L.VAR_DMMA_256x32 if variant == L.VAR_DMMA3M_128x32 else L.VAR_DMMA_256x16
+    if variant == L.VAR_DMMASTREAM and dtype != "complex128":
+        return L.VAR_DMMA_256x16
+    if variant in L.TC05_VARIANTS and dtype != "complex64":
+        # the mma.sync policy the heuristic picks without the wgmma kernel
+        return L.choose_variant(dtype, 1, max(m, n), min(m, n), k, allow_tc05=False)
+    return variant
+
+
 @pytest.mark.parametrize("variant", [L.VAR_SIMT_64x64, L.VAR_DMMA_128x64, L.VAR_DMMA_64x128,
                                      L.VAR_DMMA_256x32, L.VAR_DMMA_256x16, L.VAR_ROW_128x8, L.VAR_ROW_256x4, L.VAR_ROWSTREAM, L.VAR_TC05_128x64, L.VAR_TC05_128x32, L.VAR_TC05_128x16,
                                      L.VAR_DMMA3M_128x32, L.VAR_DMMA3M_256x16, L.VAR_DMMASTREAM, L.VAR_DOTSTREAM])
 @pytest.mark.parametrize("dtype", ["complex128", "float64", "complex64", "float32"])
 def test_every_kernel_variant_ragged_gemm(variant, dtype):
+    """Each variant on GEMMs it runs as forced (the plan's variant is asserted), into a NaN-filled C.
+    The staged variants take ragged shapes; the stream and wgmma variants shapes they accept.
+    tests/test_gpu_kernel_paths.py covers each kernel's code paths one by one."""
     import torch
 
     from cotengra_b200 import _lib
 
-    for (m, n, k) in [(130, 70, 19), (257, 3, 33), (5, 300, 9), (512, 128, 64), (1000, 96, 40)]:
-        a, b = make_arrays([(m, k), (k, n)], dtype, seed=m + n + k)
+    for (m, n, k) in _GEMMS_ACCEPTED.get(variant, _RAGGED_GEMMS):
+        a, b = make_arrays([(m, k), (k, n)], dtype, seed=m + n + k + 1000 * variant)
         dims = L.classify_pair("ab", a.shape, "bc", b.shape, "ac")
         plan = L.build_pair_desc(dims, dtype, variant=variant, c_dense_elems=m * n,
                                  sm_count=_lib.device_info()["sm_count"])
+        assert plan.variant == _variant_that_runs(variant, dtype, m, n, k), (m, n, k, variant, dtype, plan.variant)
         ta, tb = torch.from_numpy(a).cuda(), torch.from_numpy(b).cuda()
-        c = torch.empty((m, n), dtype=ta.dtype, device="cuda")
+        c = torch.full((m, n), float("nan"), dtype=ta.dtype, device="cuda")
         pa, pb = (tb, ta) if plan.swapped else (ta, tb)
         _lib.check(_lib.load().ctgb_contract_pair(plan.words.ctypes.data, pa.data_ptr(),
                                                   pb.data_ptr(), c.data_ptr(), 0))
