@@ -42,7 +42,9 @@ EXPORTS = (
     "ctgb_vjp_destroy",
     "ctgb_vjp_workspace_bytes",
     "ctgb_vjp_execute",
+    "ctgb_tc05_launch_config",
 )
+TC05_LAUNCH_FIELDS = ("b_stat", "nb", "sa", "grid", "smem", "tm_rank", "bulk", "chunk_steps", "chunks")
 
 
 class CtgbTensor(C.Structure):
@@ -177,6 +179,8 @@ def load():
         C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p,
         C.c_size_t, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
     ]
+    lib.ctgb_tc05_launch_config.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_uint64,
+                                            C.POINTER(C.c_int64), C.c_int]
     if lib.ctgb_abi_version() != 1:
         raise ImportError("libctgb200.so: ABI version mismatch")
     if lib.ctgb_desc_words() != lowering.DESC_WORDS:
@@ -214,3 +218,16 @@ def launch_count() -> int:
 def tensor_map_launches() -> int:
     """wgmma launches so far whose A tiles were fetched by tensor-map TMA."""
     return int(load().ctgb_tensor_map_launches())
+
+
+def tc05_launch_config(words, a_addr, sms, smem_optin) -> dict:
+    """The launch-time choices of the wgmma kernel for descriptor ``words`` (int64 numpy array) with
+    A at device address ``a_addr`` on a device with ``sms`` SMs and ``smem_optin`` bytes of opt-in
+    shared memory (include/ctg_b200.h).  Needs no device."""
+    import numpy as np
+
+    w = np.ascontiguousarray(words, dtype=np.int64)
+    out = (C.c_int64 * len(TC05_LAUNCH_FIELDS))()
+    check(load().ctgb_tc05_launch_config(w.ctypes.data, int(a_addr), int(sms), int(smem_optin), out,
+                                         len(TC05_LAUNCH_FIELDS)))
+    return dict(zip(TC05_LAUNCH_FIELDS, (int(x) for x in out)))

@@ -276,26 +276,19 @@ std::atomic<int64_t> g_tmap_launches{0};
 // each other coalesce into box dims.  If at most four box dims remain, the innermost is contiguous
 // and everything is 16-byte granular, ONE cp.async.bulk.tensor fetches the tile: dims 0..n-1 are
 // the box (coordinates 0), and one more dim of stride 16 bytes carries the tile's base offset as
-// its coordinate (tensor-map strides need not nest).  Returns the rank (2..5) or 0.
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-int tc05_make_tensor_map(const int64_t* h, const void* A, CUtensorMap* tm) {
-  static EncodeTiledFn encode = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      encode = (EncodeTiledFn)fn;
-    else
-      cudaGetLastError();
-  }
-  if (!encode || ((uintptr_t)A & 15u)) return 0;
-  struct Dim { uint64_t ext, stride; } box[8];
-  int nb = 0;
+// its coordinate (tensor-map strides need not nest).
+//
+// tc05_tensor_map_box derives the box (pure host code, no CUDA calls) and returns the rank of the
+// tensor map it describes (2..5), or 0 when the tile is not such a box.
+struct Tc05Box {
+  int nb = 0;  // box dims (the rank is nb + 1)
+  struct Dim { uint64_t ext, stride; } dim[8];
+};
+int tc05_tensor_map_box(const int64_t* h, uint64_t a_addr, Tc05Box& bx) {
+  if (a_addr & 15u) return 0;
+  auto& box = bx.dim;
+  int& nb = bx.nb;
+  nb = 0;
   const int n_lda = (int)h[W_NLDA];
   for (int i = 0; i < n_lda; ++i) {
     const uint64_t ext = (uint64_t)h[OFF_LDA + 4 * i], st = (uint64_t)h[OFF_LDA + 4 * i + 1];
@@ -342,13 +335,38 @@ int tc05_make_tensor_map(const int64_t* h, const void* A, CUtensorMap* tm) {
   if (!grid(OFF_GM, (int)h[W_NGM], 4, 2) || !grid(OFF_GK, (int)h[W_NGK], 4, 2) || !grid(OFF_GB, (int)h[W_NGB], 5, 2))
     return 0;
   if (reach >= (1ull << 32)) return 0;
+  return nb + 1;
+}
+
+// Encodes the tensor map of tc05_tensor_map_box.  Returns its rank, or 0 when the tile is not a
+// box, the driver has no encoder or the encode fails.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+int tc05_make_tensor_map(const int64_t* h, const void* A, CUtensorMap* tm) {
+  Tc05Box bx;
+  if (!tc05_tensor_map_box(h, (uint64_t)(uintptr_t)A, bx)) return 0;
+  static EncodeTiledFn encode = nullptr;
+  static bool tried = false;
+  if (!tried) {
+    tried = true;
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      encode = (EncodeTiledFn)fn;
+    else
+      cudaGetLastError();
+  }
+  if (!encode) return 0;
+  const int nb = bx.nb;
   cuuint64_t gdim[5], gstr[4];
   cuuint32_t bdim[5], estr[5];
   for (int i = 0; i < nb; ++i) {
-    gdim[i] = box[i].ext;
-    bdim[i] = (cuuint32_t)box[i].ext;
+    gdim[i] = bx.dim[i].ext;
+    bdim[i] = (cuuint32_t)bx.dim[i].ext;
     estr[i] = 1;
-    if (i) gstr[i - 1] = box[i].stride * 8;
+    if (i) gstr[i - 1] = bx.dim[i].stride * 8;
   }
   gdim[nb] = 1ull << 31;  // offset dim: coordinate = base offset in 16-byte units
   bdim[nb] = 1;
@@ -360,12 +378,25 @@ int tc05_make_tensor_map(const int64_t* h, const void* A, CUtensorMap* tm) {
   return rc == CUDA_SUCCESS ? nb + 1 : 0;
 }
 
-// complex64 on wgmma: prepare B' (hi/lo, tile order) once, then the warp-specialised kernel
+// Launch-time choices of the wgmma kernel, from the descriptor, the A pointer and the device's SM
+// count and opt-in shared memory.  tc05_launch_config is pure host code (no CUDA calls), so
+// ctgb_tc05_launch_config reports exactly what launch_tc05 runs.
+struct Tc05Launch {
+  int b_stat = 0;        // B' resident (one slot per k-step, loaded once) instead of a ring
+  long long nb = 0;      // B' slots
+  long long sa = 0;      // A staging depth
+  uint64_t grid = 0;     // CTAs (0: nothing to do)
+  size_t smem = 0;       // dynamic shared memory of one CTA
+  int tm_rank = 0;       // rank of the A tensor map tc05_tensor_map_box describes, 0 if none
+  int bulk = 0;          // A runs fetched by bulk copies (tc05_bulk_a)
+  unsigned chunk = 0;    // k-steps per register accumulation (tc05_chunk_steps)
+  unsigned chunks = 0;   // accumulations of the longest contracted range of a work item
+};
+
 template <int NT>
-int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
+int tc05_launch_config(const int64_t* h, uint64_t a_addr, int sms, uint64_t smem_optin, Tc05Launch& lc) {
   using Cfg = Tc05Cfg<NT>;
-  DevInfo& di = devinfo();
-  if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
+  lc = Tc05Launch();
   auto exact = [&](int pg, int full, int text) { return h[pg] < 0 || (h[full] % h[text]) == 0; };
   // every tile has the same shape: the full 128 x NT x 16, or exact divisors of the index extents
   // (MTa <= 128 rows, NTa <= NT columns, KTa a multiple of 4 up to 16)
@@ -378,22 +409,14 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   const uint64_t work = (uint64_t)h[W_TILES_M] * (uint64_t)h[W_TILES_N] * (uint64_t)h[W_TILES_B] * (uint64_t)h[W_SPLITK];
   if (work == 0) return CTGB_OK;
   if (work >= (1ull << 31)) return fail(CTGB_E_VALUE, "too many tiles for one launch");
-  static thread_local int attr_dev = -1;
-  int dev;
-  cudaGetDevice(&dev);
-  if (attr_dev != dev) {
-    CUDA_TRY(cudaFuncSetAttribute(tc05_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)di.smem_optin - 1024));
-    attr_dev = dev;
-  }
   // ring depths: B' resident (one slot per k-step) when this CTA's B' tiles never change and
   // still leave room for >= 3 A stages; otherwise a 3-slot B' ring.  A gets the rest.
-  const long long pool = (long long)di.smem_optin - 1024 /* static + slack */ - (long long)Cfg::fixed_bytes();
+  const long long pool = (long long)smem_optin - 1024 /* static + slack */ - (long long)Cfg::fixed_bytes();
   const long long steps_k = h[W_STEPS_K], tiles_n = h[W_TILES_N];
-  uint64_t grid = (uint64_t)di.sms;
+  uint64_t grid = (uint64_t)sms;
   int b_stat = 0;
   long long nb = 3;
-  if (h[W_TILES_B] == 1 && h[W_SPLITK] == 1 && steps_k <= Cfg::NB_MAX && tiles_n <= (long long)di.sms &&
+  if (h[W_TILES_B] == 1 && h[W_SPLITK] == 1 && steps_k <= Cfg::NB_MAX && tiles_n <= (long long)sms &&
       pool - steps_k * Cfg::PAIR_BYTES >= 3ll * Cfg::A_TILE * 8) {
     b_stat = 1;
     nb = steps_k;
@@ -402,13 +425,43 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   long long sa = (pool - nb * Cfg::PAIR_BYTES) / ((long long)Cfg::A_TILE * 8);
   if (sa > Cfg::SA_MAX) sa = Cfg::SA_MAX;
   if (sa < 2) return fail(CTGB_E_CUDA, "wgmma kernel needs more shared memory than the device offers");
-  if (grid > work) {
-    grid = work;
-    if (b_stat && grid % (uint64_t)tiles_n != 0) b_stat = 0, nb = nb < 3 ? 3 : nb;  // tiny launch: plain ring
-  }
+  // (a resident B' keeps grid a multiple of tiles_n here too: it needs one batch and no split-K, so
+  // work = tiles_m * tiles_n)
+  if (grid > work) grid = work;
   const size_t smem = Cfg::smem_bytes((int)sa, (int)nb);
-  if (smem + 1024 > di.smem_optin)
+  if (smem + 1024 > smem_optin)
     return fail(CTGB_E_CUDA, "wgmma kernel needs more shared memory than the device offers");
+  const unsigned steps_per_split = (unsigned)((steps_k + h[W_SPLITK] - 1) / h[W_SPLITK]);
+  Tc05Box bx;
+  lc.b_stat = b_stat;
+  lc.nb = nb;
+  lc.sa = sa;
+  lc.grid = grid;
+  lc.smem = smem;
+  lc.tm_rank = tc05_tensor_map_box(h, a_addr, bx);
+  lc.bulk = tc05_bulk_a(h[W_FLAGS], a_addr);
+  lc.chunk = tc05_chunk_steps(steps_per_split, (unsigned)(h[W_KTA] >> 2));
+  lc.chunks = (steps_per_split + lc.chunk - 1) / lc.chunk;
+  return CTGB_OK;
+}
+
+// complex64 on wgmma: prepare B' (hi/lo, tile order) once, then the warp-specialised kernel
+template <int NT>
+int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
+  using Cfg = Tc05Cfg<NT>;
+  DevInfo& di = devinfo();
+  if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
+  Tc05Launch lc;
+  if (int rc = tc05_launch_config<NT>(h, (uint64_t)(uintptr_t)A, di.sms, di.smem_optin, lc)) return rc;
+  if (lc.grid == 0) return CTGB_OK;
+  static thread_local int attr_dev = -1;
+  int dev;
+  cudaGetDevice(&dev);
+  if (attr_dev != dev) {
+    CUDA_TRY(cudaFuncSetAttribute(tc05_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)di.smem_optin - 1024));
+    attr_dev = dev;
+  }
 
   const unsigned long long tiles = (unsigned long long)h[W_TILES_B] * h[W_TILES_N] * h[W_STEPS_K];
   const size_t bytes = (size_t)tiles * Cfg::PAIR_BYTES;
@@ -432,8 +485,9 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   static const bool tm_off = getenv("CTGB_NO_TENSOR_MAP") != nullptr;
   const int tm_rank = tm_off ? 0 : tc05_make_tensor_map(h, A, &tm);
   if (tm_rank) g_tmap_launches.fetch_add(1, std::memory_order_relaxed);
-  tc05_kernel<NT><<<(unsigned)grid, Cfg::THREADS, smem, st>>>(d, (const float2*)A, Bp, (float2*)C, (unsigned)sa,
-                                                              (unsigned)nb, b_stat, tm, tm_rank);
+  tc05_kernel<NT><<<(unsigned)lc.grid, Cfg::THREADS, lc.smem, st>>>(d, (const float2*)A, Bp, (float2*)C,
+                                                                    (unsigned)lc.sa, (unsigned)lc.nb, lc.b_stat, tm,
+                                                                    tm_rank);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
   cudaFreeAsync(Bp, st);
@@ -749,6 +803,27 @@ int ctgb_single_desc_words(void) { return SDESC_WORDS; }
 const char* ctgb_last_error(void) { return g_err.c_str(); }
 int64_t ctgb_launch_count(void) { return g_launches.load(); }
 int64_t ctgb_tensor_map_launches(void) { return g_tmap_launches.load(); }
+
+int ctgb_tc05_launch_config(const int64_t* words, uint64_t a_addr, int sms, uint64_t smem_optin, int64_t* out,
+                            int n_out) {
+  if (!words || !out) return fail(CTGB_E_VALUE, "null argument");
+  if (words[W_MAGIC] != DESC_MAGIC) return fail(CTGB_E_VALUE, "bad descriptor");
+  if (n_out < 9) return fail(CTGB_E_VALUE, "ctgb_tc05_launch_config writes 9 words");
+  if (sms < 1) return fail(CTGB_E_VALUE, "sms must be positive");
+  Tc05Launch lc;
+  int rc;
+  switch (words[W_VARIANT]) {
+    case VAR_TC05_128x64: rc = tc05_launch_config<64>(words, a_addr, sms, smem_optin, lc); break;
+    case VAR_TC05_128x32: rc = tc05_launch_config<32>(words, a_addr, sms, smem_optin, lc); break;
+    case VAR_TC05_128x16: rc = tc05_launch_config<16>(words, a_addr, sms, smem_optin, lc); break;
+    default: return fail(CTGB_E_VALUE, "not a wgmma descriptor");
+  }
+  if (rc) return rc;
+  const int64_t v[9] = {lc.b_stat, lc.nb, lc.sa, (int64_t)lc.grid, (int64_t)lc.smem, lc.tm_rank, lc.bulk,
+                        (int64_t)lc.chunk, (int64_t)lc.chunks};
+  for (int i = 0; i < 9; ++i) out[i] = v[i];
+  return CTGB_OK;
+}
 
 int ctgb_device_info(int* sm_count, int* cc_major, int* cc_minor, size_t* smem_optin_bytes) {
   DevInfo& d = devinfo();

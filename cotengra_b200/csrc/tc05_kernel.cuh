@@ -46,6 +46,12 @@ __host__ __device__ inline unsigned tc05_chunk_steps(unsigned steps, unsigned nq
   const unsigned n = (steps + cap - 1) / cap;
   return n ? (steps + n - 1) / n : 1u;
 }
+// A is fetched as contiguous runs by TMA bulk copies when the descriptor says its tile is made of such
+// runs (flags bit6) and A is 16-byte aligned (cp.async.bulk's source alignment); the launcher reports the
+// same rule (tc05_launch_config)
+__host__ __device__ inline bool tc05_bulk_a(long long flags, unsigned long long a_addr) {
+  return (flags & 64) != 0 && (a_addr & 15ull) == 0;
+}
 // k-steps whose A base offsets are tabulated (the contracted range of one node: K <= 16384)
 constexpr int TC05_KTAB = 1024;
 
@@ -172,7 +178,7 @@ tc05_kernel(const int64_t* __restrict__ D, const float2* __restrict__ A, const f
   const unsigned a_elems = MTa * KTa;       // elements of one staged A tile
   const unsigned nq = KTa >> 2;             // k8 groups per k-step (KTa is a multiple of 4)
   // flags bit6: the A tile is made of contiguous runs of run_a elements (>= 128 B, even offsets)
-  const bool bulk_a = (D[W_FLAGS] & 64) != 0 && (reinterpret_cast<unsigned long long>(A) & 15ull) == 0;
+  const bool bulk_a = tc05_bulk_a(D[W_FLAGS], reinterpret_cast<unsigned long long>(A));
   const unsigned lbo_a = (unsigned)Cfg::LBO_BASE + 16u * (unsigned)D[W_LBOPAD];
   auto digit_of = [&](unsigned idx, unsigned div, unsigned ext) -> unsigned {
     return g_pow2 ? ((idx >> (31 - __clz(div))) & (ext - 1)) : ((idx / div) % ext);

@@ -34,7 +34,7 @@ MAX_T, MAX_G, MAX_GB, MAX_LD = 12, 40, 12, 24
 (W_MAGIC, W_DTYPE, W_NTM, W_NTN, W_NTK, W_NGM, W_NGN, W_NGK, W_NGB, W_MTA,
  W_NTA, W_KTA, W_TILES_M, W_TILES_N, W_TILES_B, W_STEPS_K, W_SPLITK, W_PGM,
  W_MFULL, W_MTEXT, W_MW, W_PGN, W_NFULL, W_NTEXT, W_NW, W_PGK, W_KFULL,
- W_KTEXT, W_KW, W_NLDA, W_NLDB, W_FLAGS, W_VARIANT, W_CELEMS) = range(34)
+ W_KTEXT, W_KW, W_NLDA, W_NLDB, W_FLAGS, W_VARIANT, W_CELEMS, W_RUNA, W_LBOPAD) = range(36)
 W_HDR = 40
 OFF_TM = W_HDR
 OFF_TN = OFF_TM + MAX_T * 3
@@ -637,8 +637,8 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
                     slots[slot] = slots.get(slot, 0) + 1
                 worst += max(slots.values())
             return worst
-        W[35] = min((0, 1, 2, 4), key=_conflicts)  # W_LBOPAD
-    W[34] = run_a  # W_RUNA
+        W[W_LBOPAD] = min((0, 1, 2, 4), key=_conflicts)
+    W[W_RUNA] = run_a
     W[W_FLAGS] = ((1 if accumulate else 0) | (2 if pair_ok else 0) | (4 if grid_pow2 else 0)
                   | (8 if m_pow2 else 0) | (16 if _cols_ok(4) else 0) | (32 if _cols_ok(2) else 0)
                   | (64 if bulk_a else 0))

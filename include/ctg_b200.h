@@ -254,6 +254,21 @@ int64_t ctgb_launch_count(void);
 /* ... of which wgmma launches whose A tiles are fetched by tensor-map TMA (cp.async.bulk.tensor). */
 int64_t ctgb_tensor_map_launches(void);
 
+/* The launch-time choices ctgb_contract_pair makes for a wgmma (complex64) descriptor whose A
+ * operand starts at device address a_addr, on a device with `sms` SMs and `smem_optin` bytes of
+ * opt-in shared memory per block.  Touches no device.  Writes n_out >= 9 words:
+ *   out[0] 1: B' resident (one slot per k-step, loaded once per CTA), 0: a B' ring
+ *   out[1] B' slots           out[2] A staging depth
+ *   out[3] CTAs (0: nothing to launch)
+ *   out[4] dynamic shared memory of one CTA, bytes
+ *   out[5] rank of the A tensor map (2..5), 0: no tensor map
+ *   out[6] 1: A fetched as contiguous runs by bulk copies (when out[5] is 0)
+ *   out[7] k-steps per register accumulation
+ *   out[8] accumulations (chunks) of the longest contracted range of one work item
+ * A descriptor the kernel does not take fails as ctgb_contract_pair would. */
+int ctgb_tc05_launch_config(const int64_t* words, uint64_t a_addr, int sms,
+                            uint64_t smem_optin, int64_t* out, int n_out);
+
 #ifdef __cplusplus
 }
 #endif

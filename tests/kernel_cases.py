@@ -59,9 +59,12 @@ ROW_VARIANTS = (L.VAR_ROW_128x8, L.VAR_ROW_256x4)
 SENTINEL_BITS = {np.dtype(np.float64): 0x7FF4C0FFEE5EA1ED, np.dtype(np.float32): 0x7FA5C0DE}
 C_ALIGN = 256  # bytes
 # per-element bound |got - ref| <= c * (|A| |B|)_ij (+ c |C0|_ij): c for the double and single types.
-# Largest ratio measured over the table on an H100 80GB HBM3 (400 W power limit): 6.0e-16 for the
-# double types (DMMA_128x64 complex128), 2.6e-7 for the single ones (SIMT_64x64 float32); c keeps a
-# margin above 15x.  A dropped k4 step or swapped output rows measured 2e-2 and more.
+# Largest ratios measured over the table on an H100 80GB HBM3 (400 W power limit): 6.0e-16 for the
+# double types (DMMA_128x64 complex128, a margin above 15x); for the single types 3.6e-7 with uniform
+# operands (TC05_128x64; SIMT_64x64 float32 2.6e-7), a margin above 10x, and 2.4e-6 in the wgmma kernel's
+# same-sign cases, where its truncating accumulation cannot cancel (seeded inputs, no atomics: the same
+# every run), a margin of 1.7x.  A dropped k4 step or swapped output rows measured 2e-2 and more; the
+# wgmma kernel without its lo correction terms 1.4e-5 and more.
 C_DOUBLE, C_SINGLE = 1e-14, 4e-6
 
 
@@ -89,7 +92,8 @@ class Case:
     offsets: tuple = (0, 0)         # element offsets of A and B in their buffers
     accumulate: bool = False
     force_splitk: int = 1           # None: the automatic choice
-    expect: tuple = ()              # ((predicate, value), ...) the plan must satisfy
+    expect: tuple = ()              # ((predicate, value), ...) the plan (and wgmma launch) must satisfy
+    dist: str = "uniform"           # operand values: "uniform" in [-1, 1], or "same_sign" (see _random)
 
     @property
     def id(self):
@@ -176,14 +180,52 @@ def plan_facts(plan):
         "full_tiles": full_tiles(L.W_PGM, MTa, MT) and full_tiles(L.W_PGN, NTa, NT),
         "zero_stride": 0 in op_strides,
         "steps_k": steps_k,
+        "m_tile": MTa,
         "n_tile": NTa,
         "k_tile": int(W[L.W_KTA]),
+        "nq": int(W[L.W_KTA]) // 4,            # wgmma k8 groups per k-step
+        "lbopad": int(W[L.W_LBOPAD]),
+        "run_a": int(W[L.W_RUNA]),
+        "bulk_flag": bool(flags & 64),
+        "tiles": (int(W[L.W_TILES_M]), int(W[L.W_TILES_N]), int(W[L.W_TILES_B])),
     }
+
+
+# the launch-time choices of the wgmma kernel (ctgb_tc05_launch_config) and what follows from them
+LAUNCH_KEYS = ("b_stat", "nb", "sa", "tm_rank", "bulk", "staging", "chunk_steps", "chunks", "one_item", "uneven")
+# an H100 SXM and an H100 PCIe: 132 and 114 SMs, 227 KB of opt-in shared memory per block on both
+H100_SMS = (132, 114)
+H100_SMEM_OPTIN = 232448
+
+
+def a_operand_addr(case, plan, base):
+    """Device address of the plan's A operand when the case's operand buffers start at ``base``
+    (a 256-byte aligned allocation): the streamed operand is B when the plan swaps them."""
+    which = 1 if plan.swapped else 0
+    return base + case.offsets[which] * np.dtype(case.dtype).itemsize
+
+
+def launch_facts(case, plan, a_addr, sms, smem_optin):
+    """The wgmma launch's choices for A at ``a_addr`` on a device with ``sms`` SMs."""
+    from cotengra_b200 import _lib
+
+    f = _lib.tc05_launch_config(plan.words, a_addr, sms, smem_optin)
+    W = plan.words
+    work = int(W[L.W_TILES_M]) * int(W[L.W_TILES_N]) * int(W[L.W_TILES_B]) * int(W[L.W_SPLITK])
+    f["staging"] = "tmap" if f["tm_rank"] else ("bulk" if f["bulk"] else "gather")
+    f["work"] = work
+    f["one_item"] = f["grid"] == work
+    f["uneven"] = work % f["grid"] != 0
+    return f
 
 
 def plan_mismatches(case, plan):
     facts = plan_facts(plan)
-    return {k: (v, facts[k]) for k, v in case.expect if facts[k] != v}
+    return {k: (v, facts[k]) for k, v in case.expect if k not in LAUNCH_KEYS and facts[k] != v}
+
+
+def launch_mismatches(case, facts):
+    return {k: (v, facts[k]) for k, v in case.expect if k in LAUNCH_KEYS and facts[k] != v}
 
 
 def store_mode(case, plan):
@@ -446,16 +488,256 @@ def stream_cases():
                  (L.VAR_TF32_32x32, C64)):
         add(v, d, "one_tile_splitk", "ab,bc->ac", ((31, 4219), (4219, 27)), force_splitk=None,
             expect={"splitk": 2 * SM_COUNT, "steps_k": 264})
-    # ---- wgmma complex64: guard bands and gapped C only (its modes: TC05_CASES, special values)
-    add(L.VAR_TC05_128x64, C64, "tc05_gapped_accumulate", "ab,bc->ac", ((256, 32), (32, 64)),
-        strides=((36, 1), None), out_strides=_gapped_c(64), offsets=(4, 0), accumulate=True)
-    add(L.VAR_TC05_128x32, C64, "tc05_dense_non_pow2", "ab,bc->ac", ((384, 48), (48, 32)))
-    add(L.VAR_TC05_128x16, C64, "tc05_splitk_dense", "ab,bc->ac", ((256, 64), (64, 16)), force_splitk=2,
-        expect={"splitk": 2})
     return out
 
 
-CASES = staged_cases() + stream_cases()
+# ---------------------------------------------------------------------------- wgmma (complex64)
+# Each family maps the N tile NT of a wgmma variant to the keyword arguments of one Case.  Its
+# expectations cover the plan (tile shape, k8 groups, flags) and the launch (ctgb_tc05_launch_config:
+# resident B' or ring, A staging, chunking), and hold on 132 and 114 SMs alike.  A's offset is even
+# (16-byte aligned tiles) except in the cases that exist for a misaligned A.
+
+# k-steps of B' that stay resident next to three A stages in 227 KB (32, 16 and 8 KB per k-step),
+# at most Tc05Cfg::NB_MAX = 8
+TC05_RESIDENT_STEPS = {64: 3, 32: 6, 16: 8}
+# A staging depth (16 KB stages) left beside that many resident k-steps
+_SA_AT_FIT = {64: 3, 32: 3, 16: 5}
+# NTa < NT with NTa % 4 != 0: the column quads of the last lanes straddle the tile's edge
+_NT_RAGGED = {64: 54, 32: 27, 16: 13}
+
+
+def _resident(NT, steps):
+    return {"b_stat": int(steps <= TC05_RESIDENT_STEPS[NT]), "nb": steps if steps <= TC05_RESIDENT_STEPS[NT] else 3}
+
+
+def tc_k4_m64(NT):
+    # ONE 4-wide k-step (nq 1) of a 64-row tile: consumer warpgroup 1 stores nothing.  Three work items,
+    # one per CTA; A's 256-element tile is one contiguous box dim: a rank-2 tensor map
+    return dict(eq="xak,kc->xac", shapes=((3, 64, 4), (4, NT)), strides=((300, 4, 1), None), offsets=(2, 0),
+                expect={"m_tile": 64, "k_tile": 4, "nq": 1, "steps_k": 1, "tiles": (3, 1, 1), "grid_pow2": False,
+                        "tm_rank": 2, "one_item": True, "chunks": 1, **_resident(NT, 1)})
+
+
+def tc_pow2_resident(NT):
+    # full 128 x NT x 16 tiles on a power-of-two grid (shift decode), two k-steps of resident B'
+    return _gemm(512, 2 * NT, 32, expect={"full_tiles": True, "grid_pow2": True, "m_pow2": True, "nq": 4,
+                                             "tiles": (4, 2, 1), "steps_k": 2, "tm_rank": 3, "lbopad": 1,
+                                             "one_item": True, "chunks": 1, **_resident(NT, 2)})
+
+
+def tc_idiv_ring(NT):
+    # three m tiles (idiv decode) and nine k-steps: more than fit, so B' streams through the ring
+    return _gemm(384, NT, 144, expect={"grid_pow2": False, "tiles": (3, 1, 1), "steps_k": 9, "chunk_steps": 9,
+                                          "chunks": 1, "tm_rank": 3, **_resident(NT, 9)})
+
+
+def tc_resident_at_fit(NT):
+    # the most k-steps whose B' stays resident next to three A stages: the most B' slots and barriers, and
+    # the least shared memory left for A
+    s = TC05_RESIDENT_STEPS[NT]
+    return _gemm(256, NT, 16 * s, expect={"steps_k": s, "b_stat": 1, "nb": s, "sa": _SA_AT_FIT[NT], "chunks": 1})
+
+
+def tc_ring_past_fit(NT):
+    # one k-step more: B' streams through the 3-slot ring
+    s = TC05_RESIDENT_STEPS[NT] + 1
+    return _gemm(256, NT, 16 * s, expect={"steps_k": s, "b_stat": 0, "nb": 3, "chunks": 1})
+
+
+def tc_accumulate(NT):
+    return _gemm(256, NT, 32, accumulate=True, expect={"accumulate": True, "chunks": 1, "steps_k": 2})
+
+
+def tc_two_chunks_fold(NT):
+    # 17 k-steps: two balanced chunks (9 + 8), the second folded into what the first stored (C starts NaN)
+    return _gemm(256, NT, 272, expect={"steps_k": 17, "chunk_steps": 9, "chunks": 2, "accumulate": False,
+                                          "b_stat": 0})
+
+
+def tc_chunks_accumulate(NT):
+    # 50 k-steps in four chunks (13, 13, 12, 12), every one added to C0
+    return _gemm(128, NT, 800, accumulate=True, expect={"steps_k": 50, "chunk_steps": 13, "chunks": 4,
+                                                           "accumulate": True})
+
+
+def tc_nq3_chunks(NT):
+    # 12-wide k-steps (6^n extents: nq 3): 25 steps in chunks of at most 36 k8 accumulations: 9, 8, 8
+    return _gemm(256, NT, 300, expect={"k_tile": 12, "nq": 3, "steps_k": 25, "chunk_steps": 9, "chunks": 3})
+
+
+def tc_nq2(NT):
+    return _gemm(256, NT, 40, expect={"k_tile": 8, "nq": 2, "steps_k": 5, "chunks": 1, **_resident(NT, 5)})
+
+
+def tc_splitk3_uneven(NT):
+    # 7 k-steps over three CTAs: ranges of 3, 3 and 1, added with atomics after the memset
+    return _gemm(256, NT, 112, force_splitk=3, expect={"splitk": 3, "steps_k": 7, "b_stat": 0, "chunks": 1})
+
+
+def tc_splitk3_chunked(NT):
+    # 50 k-steps over three CTAs: ranges of 17, 17 and 16, each in two chunks
+    return _gemm(128, NT, 800, force_splitk=3, expect={"splitk": 3, "steps_k": 50, "chunk_steps": 9, "chunks": 2})
+
+
+def tc_splitk_acc_gapped(NT):
+    return _gemm(256, NT, 112, force_splitk=2, accumulate=True, out_strides=_gapped_c(NT),
+                    expect={"splitk": 2, "accumulate": True, "b_stat": 0})
+
+
+def tc_ragged_tile(NT):
+    # 108 x NTa x 12 tiles (64 < MTa < 128, NTa % 4 != 0): the bond-6 PEPS shape of each N tile
+    R = _NT_RAGGED[NT]
+    return _gemm(216, 2 * R, 24, expect={"m_tile": 108, "n_tile": R, "k_tile": 12, "nq": 3, "tiles": (2, 2, 1),
+                                            "steps_k": 2, "full_tiles": False, **_resident(NT, 2)})
+
+
+def tc_gather_odd(NT):
+    # A rows 17 elements apart: runs of 16 at odd offsets -- no tensor map, no bulk copies
+    return _gemm(256, NT, 16, strides=((17, 1), None), offsets=(2, 0),
+                    expect={"bulk_flag": False, "staging": "gather", "tm_rank": 0, **_resident(NT, 1)})
+
+
+def tc_misaligned_a(NT):
+    # bulk runs in the descriptor, but A 8 bytes off 16-byte alignment: the launch gathers
+    return _gemm(256, NT, 32, offsets=(1, 0), expect={"bulk_flag": True, "staging": "gather", "tm_rank": 0})
+
+
+def tc_bulk_runs(NT):
+    # five box dims (k and four m dims that never coalesce): no tensor map; runs of 16 elements
+    return dict(eq="abcdk,kn->abcdn", shapes=((32, 2, 2, 2, 16), (16, NT)), strides=((160, 78, 38, 18, 1), None),
+                offsets=(4, 0), expect={"bulk_flag": True, "run_a": 16, "staging": "bulk", "tm_rank": 0,
+                                        "tiles": (2, 1, 1)})
+
+
+def tc_tmap4(NT):
+    # three box dims of A (k, then two m dims with gaps): a rank-4 tensor map
+    return dict(eq="abk,kc->abc", shapes=((32, 8, 16), (16, NT)), strides=((164, 20, 1), None), offsets=(2, 0),
+                expect={"tm_rank": 4, "tiles": (2, 1, 1)})
+
+
+def tc_tmap5(NT):
+    # four box dims: a rank-5 tensor map
+    return dict(eq="abck,kn->abcn", shapes=((16, 4, 4, 16), (16, NT)), strides=((310, 76, 18, 1), None),
+                offsets=(6, 0), expect={"tm_rank": 5, "tiles": (2, 1, 1)})
+
+
+def tc_swapped(NT):
+    # the larger operand second: the plan swaps them, so the launch streams B's buffer as A
+    return dict(eq="kc,ak->ac", shapes=((16, NT), (256, 16)), offsets=(0, 2), expect={"swapped": True})
+
+
+def tc_batched(NT):
+    # a batch grid of 3: B' changes between work items of a CTA, so it streams through the ring
+    return dict(eq="xab,xbc->xac", shapes=((3, 256, 32), (3, 32, NT)),
+                expect={"batch": True, "tiles": (2, 1, 3), "b_stat": 0, "nb": 3})
+
+
+def tc_permuted_gapped(NT):
+    # C transposed with gaps, B column-major with gaps (bprime_kernel reads past sentinels)
+    return dict(eq="ab,bc->ca", shapes=((256, 32), (32, NT)), strides=(None, (1, 34)), out_strides=(519, 2),
+                offsets=(0, 3), expect={"swapped": False})
+
+
+def tc_many_items_resident(NT):
+    # 512 work items over the CTAs, unevenly, with B' resident (one k-step)
+    return _gemm(65536, NT, 16, expect={"tiles": (512, 1, 1), "uneven": True, **_resident(NT, 1)})
+
+
+def tc_many_items_ring(NT):
+    # the same number of items in two batches: B' streamed
+    return dict(eq="xab,xbc->xac", shapes=((2, 32768, 16), (2, 16, NT)),
+                expect={"tiles": (256, 1, 2), "uneven": True, "b_stat": 0})
+
+
+def tc_same_sign_k256(NT):
+    # no cancellation: 16 k-steps = 64 truncating wgmma accumulations in one chunk
+    return _gemm(256, NT, 256, dist="same_sign", expect={"nq": 4, "steps_k": 16, "chunk_steps": 16, "chunks": 1})
+
+
+def tc_same_sign_k4096(NT):
+    # ... and 256 k-steps: 16 such chunks folded with round-to-nearest adds
+    return _gemm(128, NT, 4096, dist="same_sign", expect={"steps_k": 256, "chunk_steps": 16, "chunks": 16})
+
+
+TC05_FAMILIES = {
+    "k4_m64": tc_k4_m64,
+    "pow2_resident": tc_pow2_resident,
+    "idiv_ring": tc_idiv_ring,
+    "resident_at_fit": tc_resident_at_fit,
+    "ring_past_fit": tc_ring_past_fit,
+    "accumulate": tc_accumulate,
+    "two_chunks_fold": tc_two_chunks_fold,
+    "chunks_accumulate": tc_chunks_accumulate,
+    "nq3_chunks": tc_nq3_chunks,
+    "nq2": tc_nq2,
+    "splitk3_uneven": tc_splitk3_uneven,
+    "splitk3_chunked": tc_splitk3_chunked,
+    "splitk_acc_gapped": tc_splitk_acc_gapped,
+    "ragged_tile": tc_ragged_tile,
+    "gather_odd": tc_gather_odd,
+    "misaligned_a": tc_misaligned_a,
+    "bulk_runs": tc_bulk_runs,
+    "tmap4": tc_tmap4,
+    "tmap5": tc_tmap5,
+    "swapped": tc_swapped,
+    "batched": tc_batched,
+    "permuted_gapped": tc_permuted_gapped,
+    "many_items_resident": tc_many_items_resident,
+    "many_items_ring": tc_many_items_ring,
+    "same_sign_k256": tc_same_sign_k256,
+    "same_sign_k4096": tc_same_sign_k4096,
+}
+
+# The shapes the wgmma kernel's first mode tests used (name, eq, shapes, build_pair_desc kwargs, and the
+# (variant, split-K) the plan must take), each run with A aligned and with A 8 bytes further on.  Without
+# a forced variant or split the plan takes the automatic choice for 132 SMs.
+_T64, _T32, _T16 = L.VAR_TC05_128x64, L.VAR_TC05_128x32, L.VAR_TC05_128x16
+TC05_LEGACY = [
+    ("ring_b_long_k", "ab,bc->ac", ((1024, 256), (256, 64)), {"force_splitk": 1}, (_T64, 1)),  # 16 k-steps: a ring
+    ("m_fastest", "ba,bc->ac", ((64, 512), (64, 128)), {"force_splitk": 1}, (_T64, 1)),  # A k-major: runs of 128
+    ("batched", "xab,xbc->xac", ((3, 256, 32), (3, 32, 64)), {"variant": _T64}, (_T64, 1)),
+    ("gather_odd_strides", "abx,bcx->acx", ((256, 32, 3), (32, 32, 3)), {"variant": _T32}, (_T32, 1)),
+    ("split_k", "ab,bc->ac", ((128, 256), (256, 64)), {"force_splitk": 4}, (_T64, 4)),
+    ("accumulate", "ab,bc->ac", ((512, 64), (64, 64)), {"accumulate": True, "force_splitk": 1}, (_T64, 1)),
+    ("accumulate_split", "ab,bc->ac", ((512, 64), (64, 64)), {"accumulate": True, "force_splitk": 2}, (_T64, 2)),
+    ("non_pow2_grid", "ab,bc->ac", ((384, 48), (48, 32)), {"variant": _T32, "force_splitk": 1}, (_T32, 1)),
+    ("permuted_out", "aibj,ijc->cba", ((16, 4, 16, 8), (4, 8, 64)), {"variant": _T64}, (_T64, 1)),
+    ("wide_n", "ab,bc->ac", ((1024, 64), (64, 512)), {"force_splitk": 1}, (_T64, 1)),
+    ("narrow_n16", "ab,cb->ac", ((4096, 32), (16, 32)), {}, (_T16, 1)),
+    ("narrow_n16_batched", "xab,xbc->xca", ((2, 512, 64), (2, 64, 16)), {"variant": _T16}, (_T16, 4)),
+]
+
+def tc05_cases():
+    out = []
+    for v in L.TC05_VARIANTS:
+        NT = L.VARIANT_TILES[v][1]
+        for name, fam in TC05_FAMILIES.items():
+            out.append(_case(v, C64, name, fam(NT)))
+    # guard bands around a gapped A and C (accumulating), a dense non-power-of-two grid, dense split-K
+    out.append(_case(_T64, C64, "tc05_gapped_accumulate", _gemm(
+        256, 64, 32, strides=((36, 1), None), out_strides=_gapped_c(64), offsets=(4, 0), accumulate=True,
+        expect={"accumulate": True, "staging": "tmap", "b_stat": 1, "nb": 2})))
+    out.append(_case(_T32, C64, "tc05_dense_non_pow2", _gemm(
+        384, 32, 48, expect={"grid_pow2": False, "tiles": (3, 1, 1), "b_stat": 1, "nb": 3})))
+    out.append(_case(_T16, C64, "tc05_splitk_dense", _gemm(
+        256, 16, 64, force_splitk=2, expect={"splitk": 2, "b_stat": 0})))
+    # the bond-6 PEPS tile with same-sign operands: 18 k-steps of 12 in two chunks (9 + 9)
+    out.append(_case(_T64, C64, "same_sign_108x54x12", _gemm(
+        1296, 216, 216, dist="same_sign",
+        expect={"m_tile": 108, "n_tile": 54, "k_tile": 12, "steps_k": 18, "chunk_steps": 9, "chunks": 2})))
+    for name, eq, shapes, kw, (v, want_splitk) in TC05_LEGACY:
+        kw = dict(kw)
+        splitk = kw.pop("force_splitk", None)
+        kw.pop("variant", None)
+        exp = {"bulk_flag": name != "gather_odd_strides", "splitk": want_splitk}
+        for suffix, off, staging in (("", 0, None), ("_a_plus_8_bytes", 1, "gather")):
+            e = dict(exp, **({"staging": staging} if staging else {}))
+            out.append(_case(v, C64, f"legacy_{name}{suffix}", dict(eq=eq, shapes=shapes, offsets=(off, 0),
+                                                                    force_splitk=splitk, expect=e, **kw)))
+    return out
+
+
+CASES = staged_cases() + stream_cases() + tc05_cases()
 
 
 # ---------------------------------------------------------------------------- buffers
@@ -476,7 +758,15 @@ def sentinel_fill(n, dtype):
     return bits.view(rd).view(dtype)
 
 
-def _random(rng, shape, dtype):
+def _random(rng, shape, dtype, dist="uniform", which=0):
+    """Operand ``which`` (0: A, 1: B, 2: C0).  "same_sign": A real in [0.5, 1], B with real and
+    imaginary parts in [0.5, 1] -- every product of the contraction has positive real and imaginary
+    parts, so nothing cancels and a truncating accumulation shows its bias."""
+    if dist == "same_sign" and which < 2:
+        x = rng.uniform(0.5, 1.0, size=shape)
+        if which == 1:
+            x = x + 1j * rng.uniform(0.5, 1.0, size=shape)
+        return x.astype(dtype)
     x = rng.uniform(-1.0, 1.0, size=shape)
     if np.dtype(dtype).kind == "c":
         x = x + 1j * rng.uniform(-1.0, 1.0, size=shape)
@@ -498,11 +788,12 @@ def make_layout(case, seed=0):
     guard = max(32, C_ALIGN // dt.itemsize)
     bufs, offs, ops = [], [], []
     ta, tb, _ = case.terms()
-    for shape, strides, off in zip(case.shapes, case.strides, case.offsets):
+    for which, (shape, strides, off) in enumerate(zip(case.shapes, case.strides, case.offsets)):
         strides = L.row_major_strides(shape) if strides is None else strides
         reach = _reach(shape, strides)
         buf = sentinel_fill(off + int(reach.max()) + 1 + guard, dt)
-        buf[off + reach] = _random(rng, reach.shape, dt)  # repeated offsets (stride 0, diagonals): last write wins
+        # (repeated offsets -- stride 0, diagonals: the last write wins)
+        buf[off + reach] = _random(rng, reach.shape, dt, case.dist, which)
         bufs.append(buf)
         offs.append(off)
         ops.append(buf[off + reach])

@@ -8,6 +8,10 @@ element must lie within c * (|A| |B|)_ij (+ c |C0|_ij) of np.einsum in float64/c
 missing or doubled k-step, a row stored one row down or swapped real and imaginary halves fail
 that even where the normwise error is small.  The normwise bound (1e-12 double, 1e-5 single) is
 checked as well.  Set CTGB_ERROR_REPORT to collect the measured ratios.
+
+A wgmma (complex64) case also asserts the launch-time choices ctgb_tc05_launch_config reports for
+this device and the real A pointer (resident B' or ring, A staging, chunking), and that a tensor map
+was encoded exactly when one is predicted.
 """
 
 import json
@@ -19,6 +23,7 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
+from cotengra_b200 import lowering as L  # noqa: E402
 from tests import kernel_cases as KC  # noqa: E402
 from tests.helpers import rel_err  # noqa: E402
 
@@ -54,8 +59,20 @@ def test_kernel_path(cid):
     ptr = [d.data_ptr() + off * es for d, off in zip(dev, lay.offs)]
     assert ptr[2] % KC.C_ALIGN == 0
     pa, pb = (ptr[1], ptr[0]) if plan.swapped else (ptr[0], ptr[1])
+    wgmma = plan.variant in L.TC05_VARIANTS
+    if wgmma:
+        # the launch-time choices for this device and this A pointer, and the tensor-map launch counter
+        # moving exactly when a tensor map is predicted (an encode that fails shows here too)
+        info = _lib.device_info()
+        facts = KC.launch_facts(case, plan, pa, info["sm_count"], info["smem_optin"])
+        assert not KC.launch_mismatches(case, facts), KC.launch_mismatches(case, facts)
+        tmaps = _lib.tensor_map_launches()
     _lib.check(_lib.load().ctgb_contract_pair(plan.words.ctypes.data, pa, pb, ptr[2], 0))
     torch.cuda.synchronize()
+    if wgmma:
+        # (CTGB_NO_TENSOR_MAP, a measurement setting of the launcher, turns tensor maps off)
+        tmap = facts["tm_rank"] and "CTGB_NO_TENSOR_MAP" not in os.environ
+        assert _lib.tensor_map_launches() - tmaps == (1 if tmap else 0), facts
     for d, b in zip(dev[:2], lay.bufs[:2]):
         assert d.cpu().numpy().tobytes() == b.tobytes()  # operands untouched
     got, bad = KC.check_result(case, lay, dev[2].cpu().numpy())

@@ -155,68 +155,6 @@ def test_every_kernel_variant_ragged_gemm(variant, dtype):
             (m, n, k, variant, dtype)
 
 
-_T64, _T32, _T16 = L.VAR_TC05_128x64, L.VAR_TC05_128x32, L.VAR_TC05_128x16
-TC05_CASES = [
-    # (name, eq, shapes, build_pair_desc kwargs)
-    ("ring_b_long_k", "ab,bc->ac", [(1024, 256), (256, 64)], {"force_splitk": 1}),       # 16 k-steps > resident slots
-    ("m_fastest", "ba,bc->ac", [(64, 512), (64, 128)], {"force_splitk": 1}),             # A stored k-major: runs of 128
-    ("batched", "xab,xbc->xac", [(3, 256, 32), (3, 32, 64)], {"variant": _T64}),         # tiles_b = 3: B' ring
-    ("gather_odd_strides", "abx,bcx->acx", [(256, 32, 3), (32, 32, 3)], {"variant": _T32}),  # no runs: cp.async gather
-    ("split_k", "ab,bc->ac", [(128, 256), (256, 64)], {"force_splitk": 4}),              # atomics epilogue
-    ("accumulate", "ab,bc->ac", [(512, 64), (64, 64)], {"accumulate": True, "force_splitk": 1}),   # C += A B
-    ("accumulate_split", "ab,bc->ac", [(512, 64), (64, 64)], {"accumulate": True, "force_splitk": 2}),
-    ("non_pow2_grid", "ab,bc->ac", [(384, 48), (48, 32)], {"variant": _T32, "force_splitk": 1}),   # 3 tiles x 3 k-steps
-    ("permuted_out", "aibj,ijc->cba", [(16, 4, 16, 8), (4, 8, 64)], {"variant": _T64}),  # strided C rows and columns
-    ("wide_n", "ab,bc->ac", [(1024, 64), (64, 512)], {"force_splitk": 1}),               # 8 column tiles: resident B' per CTA
-    ("narrow_n16", "ab,cb->ac", [(4096, 32), (16, 32)], {}),                             # 128 x 16 tiles (UMMA N = 32)
-    ("narrow_n16_batched", "xab,xbc->xca", [(2, 512, 64), (2, 64, 16)], {"variant": _T16}),
-]
-
-
-@pytest.mark.parametrize("case", TC05_CASES, ids=[c[0] for c in TC05_CASES])
-@pytest.mark.parametrize("misalign", [False, True], ids=["aligned", "a_plus_8_bytes"])
-def test_tcgen05_kernel_modes(case, misalign):
-    """Every mode of the tcgen05 complex64 kernel (tc05_kernel.cuh): TMA-bulk vs cp.async
-    staging, resident vs ring B', split-K atomics, accumulate, non-power-of-two grids."""
-    import torch
-
-    from cotengra_b200 import _lib
-
-    name, eq, shapes, kw = case
-    lhs, out = eq.split("->")
-    ta_, tb_ = lhs.split(",")
-    a, b = make_arrays(shapes, "complex64", seed=len(name))
-    dims = L.classify_pair(ta_, a.shape, tb_, b.shape, out)
-    out_shape = tuple(dict(zip(ta_ + tb_, a.shape + b.shape))[ix] for ix in out)
-    n_out = math.prod(out_shape)
-    plan = L.build_pair_desc(dims, "complex64", c_dense_elems=n_out, sm_count=_lib.device_info()["sm_count"], **kw)
-    assert plan.variant in L.TC05_VARIANTS, (name, plan.variant)
-    bulk = bool(plan.words[L.W_FLAGS] & 64)
-    assert bulk == (name != "gather_odd_strides")
-    if "force_splitk" in kw:
-        assert plan.words[L.W_SPLITK] == kw["force_splitk"]
-
-    def dev(x, off):
-        # a device copy whose first element sits `off` elements into an allocation
-        buf = torch.empty(x.size + off, dtype=torch.complex64, device="cuda")
-        buf[off:].copy_(torch.from_numpy(np.ascontiguousarray(x).reshape(-1)))
-        return buf, buf[off:]
-
-    (keep_a, da), (keep_b, db) = dev(a, 1 if misalign else 0), dev(b, 0)
-    c0 = make_arrays([out_shape], "complex64", seed=77)[0]
-    dc = torch.from_numpy(np.ascontiguousarray(c0)).cuda()
-    pa, pb = (db, da) if plan.swapped else (da, db)
-    if plan.swapped and misalign:
-        pytest.skip("operands swapped: the streamed operand is not the misaligned one")
-    _lib.check(_lib.load().ctgb_contract_pair(plan.words.ctypes.data, pa.data_ptr(), pb.data_ptr(), dc.data_ptr(), 0))
-    torch.cuda.synchronize()
-    want = np.einsum(eq, a.astype(np.complex128), b.astype(np.complex128))
-    if kw.get("accumulate"):
-        want = want + c0
-    assert rel_err(dc.cpu().numpy().reshape(out_shape), want) < 1e-5, name
-    del keep_a, keep_b
-
-
 DSTREAM_CASES = [
     ("n16_k16", "ab,bc->ac", [(8192, 16), (16, 16)], {}),
     ("ragged_rows_cols", "xyzb,bc->zyxc", [(8, 27, 19, 7), (7, 11)], {}),   # 4104 rows (masked tail), odd N, K % 4 != 0

@@ -83,9 +83,9 @@ CASES = [
     (L.VAR_DOTSTREAM4, "mk,kn->mn", (3, 1 << 20), (1 << 20, 2), {}, ALL, "dot"),
     (L.VAR_DMMA_32x32, "mk,kn->mn", (20, 1 << 14), (1 << 14, 24), {}, ("complex128", "float64"), "split"),
     (L.VAR_ROWSTREAM_K, "ab,bc->ac", (4096, 40), (40, 7), {}, ("float64", "complex64", "float32"), "ragged_n"),
-    # the wgmma complex64 kernel: every N tile, every A staging mode (asserted), split-K, the non-power-of-two
-    # exact tiles, and shapes whose B' the launcher keeps resident (few k-steps, one batch) or streams
-    # through its ring (long k, batched) -- that choice is made inside the launcher and not asserted
+    # the wgmma complex64 kernel: every N tile, every A staging mode, split-K, the non-power-of-two exact
+    # tiles, and shapes whose B' the launcher keeps resident or streams through its ring (both asserted:
+    # _RESIDENT_B)
     (_T64, "ab,bc->ac", (512, 64), (64, 64), {"force_splitk": 1}, SINGLE[:1], "tmap,few_k"),
     (_T32, "ab,bc->ac", (512, 64), (64, 32), {"force_splitk": 1}, SINGLE[:1], "tmap,few_k"),
     (_T16, "ab,bc->ac", (512, 64), (64, 16), {"variant": _T16, "force_splitk": 1}, SINGLE[:1], "tmap,few_k"),
@@ -98,6 +98,9 @@ CASES = [
     (_T64, "ab,bc->ac", (1296, 216), (216, 216), {"force_splitk": 1}, SINGLE[:1], "tmap,exact108x54x12"),
     (_T64, "ab,bc->ac", (128, 256), (256, 64), {"force_splitk": 4}, SINGLE[:1], "tmap,split"),
 ]
+# wgmma rows whose B' stays resident: four k-steps fit next to three A stages for N tiles of 32 and 16,
+# not for 64 (three at most); long k, a batch or split-K always stream it through the ring
+_RESIDENT_B = {(_T32, "tmap,few_k"), (_T16, "tmap,few_k")}
 PARAMS = [pytest.param(c, dt, id=f"v{c[0]}-{dt}-{c[6]}-{'x'.join(map(str, c[2]))}")
           for c in CASES for dt in c[5]]
 
@@ -187,6 +190,11 @@ def _expect_variant(case, plan, mode):
         assert mode == want_mode, (note, mode)
         if "exact" in note:
             assert (int(plan.words[L.W_MTA]), int(plan.words[L.W_NTA]), int(plan.words[L.W_KTA])) == (108, 54, 12)
+        from cotengra_b200 import _lib
+
+        info = _lib.device_info()
+        launch = _lib.tc05_launch_config(plan.words, 0, info["sm_count"], info["smem_optin"])
+        assert launch["b_stat"] == ((v, note) in _RESIDENT_B), (note, launch)
 
 
 @pytest.mark.parametrize("case,dtype", PARAMS)
