@@ -38,10 +38,6 @@ EXPORTS = (
     "ctgb_plan_profile",
     "ctgb_plan_profile_read",
     "ctgb_probe_fp64_peaks",
-    "ctgb_vjp_create",
-    "ctgb_vjp_destroy",
-    "ctgb_vjp_workspace_bytes",
-    "ctgb_vjp_execute",
     "ctgb_tc05_launch_config",
 )
 TC05_LAUNCH_FIELDS = ("b_stat", "nb", "sa", "grid", "smem", "tm_rank", "bulk", "chunk_steps", "chunks")
@@ -65,7 +61,8 @@ class CtgbNode(C.Structure):
         ("a", C.c_int32),
         ("b", C.c_int32),
         ("c", C.c_int32),
-        ("invariant", C.c_int32),
+        ("phase", C.c_int32),
+        ("zero_fill", C.c_int32),
         ("is_root", C.c_int32),
         ("desc", C.POINTER(C.c_int64)),
     ]
@@ -87,36 +84,6 @@ class CtgbPlanDesc(C.Structure):
         ("workspace_bytes", C.c_int64),
         ("persistent_bytes", C.c_int64),
         ("strip_exponent", C.c_int32),
-    ]
-
-
-class CtgbVjpNode(C.Structure):
-    _fields_ = [
-        ("kind", C.c_int32),
-        ("a", C.c_int32),
-        ("b", C.c_int32),
-        ("c", C.c_int32),
-        ("phase", C.c_int32),
-        ("zero_fill", C.c_int32),
-        ("desc", C.POINTER(C.c_int64)),
-    ]
-
-
-class CtgbVjpDesc(C.Structure):
-    _fields_ = [
-        ("dtype", C.c_int32),
-        ("n_inputs", C.c_int32),
-        ("n_tensors", C.c_int32),
-        ("tensors", C.POINTER(CtgbTensor)),
-        ("n_nodes", C.c_int32),
-        ("nodes", C.POINTER(CtgbVjpNode)),
-        ("n_sliced", C.c_int32),
-        ("slice_radix", C.POINTER(C.c_int64)),
-        ("slice_project", C.POINTER(C.c_int64)),
-        ("slice_out_stride", C.POINTER(C.c_int64)),
-        ("out_elements", C.c_int64),
-        ("workspace_bytes", C.c_int64),
-        ("persistent_bytes", C.c_int64),
         ("cotangent_offset", C.c_int64),
     ]
 
@@ -159,8 +126,8 @@ def load():
     lib.ctgb_plan_destroy.argtypes = [C.c_void_p]
     lib.ctgb_plan_destroy.restype = None
     lib.ctgb_plan_execute.argtypes = [
-        C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p,
-        C.c_size_t, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
+        C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
+        C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
     ]
     lib.ctgb_plan_execute_host.argtypes = [
         C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_void_p,
@@ -170,18 +137,9 @@ def load():
     lib.ctgb_plan_profile.argtypes = [C.c_void_p, C.c_int]
     lib.ctgb_plan_profile_read.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_int]
     lib.ctgb_probe_fp64_peaks.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p]
-    lib.ctgb_vjp_create.argtypes = [C.POINTER(CtgbVjpDesc), C.POINTER(C.c_void_p)]
-    lib.ctgb_vjp_destroy.argtypes = [C.c_void_p]
-    lib.ctgb_vjp_destroy.restype = None
-    lib.ctgb_vjp_workspace_bytes.argtypes = [C.c_void_p]
-    lib.ctgb_vjp_workspace_bytes.restype = C.c_size_t
-    lib.ctgb_vjp_execute.argtypes = [
-        C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p,
-        C.c_size_t, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
-    ]
     lib.ctgb_tc05_launch_config.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_uint64,
                                             C.POINTER(C.c_int64), C.c_int]
-    if lib.ctgb_abi_version() != 1:
+    if lib.ctgb_abi_version() != 2:
         raise ImportError("libctgb200.so: ABI version mismatch")
     if lib.ctgb_desc_words() != lowering.DESC_WORDS:
         raise ImportError("libctgb200.so: pair descriptor layout mismatch")

@@ -673,7 +673,7 @@ int launch_node(int kind, const int64_t* h, const int64_t* d, const void* A, con
 
 }  // namespace
 
-// ================================================================== shared by plans and VJP plans
+// ================================================================== plans
 // A tensor slot (ctgb_tensor) as the library keeps it.
 struct ctgb_tensor_rec {
   int kind, input_index;
@@ -754,13 +754,16 @@ static int copy_tensors(const ctgb_tensor* ts, int n, int n_inputs, int n_sliced
   return CTGB_OK;
 }
 
-// ================================================================== plans
+// A forward plan runs phases 0 and 1.  A reverse-mode plan (cotengra_b200/vjp.py plans it) also runs
+// phases 2 and 3: it propagates H = conj(cotangent), for which the adjoint of a contraction needs no
+// conjugation, so every backward node is an ordinary pairwise or single-operand descriptor and only the
+// cotangent's copy and the finished input gradients are conjugated (complex dtypes).
 struct ctgb_plan {
   int dtype = 0;
   int n_inputs = 0;
   using Tensor = ctgb_tensor_rec;
   struct Node {
-    int kind, a, b, c, invariant, is_root;
+    int kind, a, b, c, phase, zero_fill, is_root;
     size_t desc_off;  // word offset into descs
     int64_t c_elems;  // dense elements of the result (strip_exponent)
     int measure_after = 0;  // strip_exponent: max|C| needs its own pass (split-K / block partial sums)
@@ -773,6 +776,10 @@ struct ctgb_plan {
   std::vector<int64_t> radix, project, out_stride;
   int64_t out_elements = 0, workspace_bytes = 0, persistent_bytes = 0;
   int strip_exponent = 0;
+  int root = -1;                    // the node that writes the output
+  bool backward = false;            // phase 2/3 nodes: needs a cotangent and the gradient buffers
+  int64_t cot_offset = -1;          // conjugated cotangent copy in the persistent arena
+  std::vector<int64_t> grad_elems;  // per input: elements of its gradient (0: not differentiated)
   int64_t launches_per_slice = 0;
   // strip_exponent scratch (device): [1] slice exponent, [2] invariant exponent
   double* d_scalars = nullptr;
@@ -895,8 +902,13 @@ int ctgb_reduce_single(const int64_t* desc, const void* X, void* out, void* stre
 
 int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
   if (!pd || !out) return fail(CTGB_E_VALUE, "null argument");
-  if (elem_size(pd->dtype) == 0) return fail(CTGB_E_VALUE, "bad dtype");
+  const size_t es = elem_size(pd->dtype);
+  if (es == 0) return fail(CTGB_E_VALUE, "bad dtype");
   ctgb_plan* p = new ctgb_plan();
+  auto refuse = [&](const char* msg) {
+    delete p;
+    return fail(CTGB_E_VALUE, msg);
+  };
   p->dtype = pd->dtype;
   p->n_inputs = pd->n_inputs;
   if (int rc = copy_tensors(pd->tensors, pd->n_tensors, pd->n_inputs, pd->n_sliced, p->tensors)) {
@@ -912,22 +924,20 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     q.a = n.a;
     q.b = n.b;
     q.c = n.c;
-    q.invariant = n.invariant;
+    q.phase = n.phase;
+    q.zero_fill = n.zero_fill;
     q.is_root = n.is_root;
     const int words = n.kind == 0 ? (int)DESC_WORDS : (int)SDESC_WORDS;
     const int64_t magic = n.kind == 0 ? DESC_MAGIC : SDESC_MAGIC;
-    if (!n.desc || n.desc[0] != magic) {
-      delete p;
-      return fail(CTGB_E_VALUE, "bad node descriptor");
-    }
+    if (n.kind < 0 || n.kind > 1 || !n.desc || n.desc[0] != magic) return refuse("bad node descriptor");
+    if (n.phase < 0 || n.phase > 3) return refuse("bad node phase");
     auto bad = [&](int t) { return t < 0 || t >= pd->n_tensors; };
-    if (bad(n.a) || bad(n.c) || (n.kind == 0 && bad(n.b))) {
-      delete p;
-      return fail(CTGB_E_VALUE, "node refers to a missing tensor");
-    }
+    if (bad(n.a) || bad(n.c) || (n.kind == 0 && bad(n.b))) return refuse("node refers to a missing tensor");
+    p->backward |= n.phase >= 2;
+    if (n.is_root) p->root = i;
     q.desc_off = p->descs.size();
     p->descs.insert(p->descs.end(), n.desc, n.desc + words);
-    q.c_elems = p->tensors[n.c].nbytes / (int64_t)elem_size(pd->dtype);
+    q.c_elems = p->tensors[n.c].nbytes / (int64_t)es;
     if (pd->strip_exponent && n.kind == 0) {
       const int64_t* w = n.desc;
       q.measure_after = w[W_SPLITK] > 1 || w[W_VARIANT] == VAR_DOTSTREAM || w[W_VARIANT] == VAR_DOTSTREAM4;
@@ -939,8 +949,23 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
                          tc05_chunk_steps((unsigned)((w[W_STEPS_K] + w[W_SPLITK] - 1) / w[W_SPLITK]),
                                           (unsigned)(w[W_KTA] >> 2)) < (unsigned)w[W_STEPS_K];
     }
-    if (!n.invariant) per_slice += 1 + q.measure_after + (pd->strip_exponent && n.kind == 0 ? 1 : 0);
+    if (n.phase == 1 || n.phase == 2) per_slice += 1 + q.measure_after + (pd->strip_exponent && n.kind == 0 ? 1 : 0);
   }
+  if (pd->strip_exponent && p->backward) return refuse("strip_exponent plans have no reverse mode");
+  // kind 3 (the output) belongs to forward plans, kinds 4-6 (cotangent, gradients, H accumulators) to
+  // reverse-mode ones: execute checks exactly the buffers the plan's kind needs
+  p->grad_elems.assign(pd->n_inputs, 0);
+  for (const auto& q : p->tensors) {
+    if (q.kind < 0 || q.kind > 6 || (q.kind == 3 && p->backward) || (q.kind >= 4 && !p->backward))
+      return refuse("bad tensor kind for the plan's phases");
+    if (q.kind == 5) p->grad_elems[q.input_index] = q.nbytes / (int64_t)es;
+  }
+  const bool cplx = pd->dtype == CTGB_C64 || pd->dtype == CTGB_C128;
+  if (cplx && p->backward && pd->cotangent_offset < 0)
+    return refuse("a complex reverse-mode plan needs room for the conjugated cotangent");
+  p->cot_offset = cplx ? pd->cotangent_offset : -1;
+  if (p->cot_offset >= 0 && p->cot_offset + pd->out_elements * (int64_t)es > pd->persistent_bytes)
+    return refuse("the conjugated cotangent does not fit the persistent arena");
   if (pd->strip_exponent) per_slice += 5;  // reset slots, sum of logs, rescale/add/commit
   p->launches_per_slice = per_slice;
   p->radix.assign(pd->slice_radix, pd->slice_radix + pd->n_sliced);
@@ -981,7 +1006,7 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
         w[W_SCALE_B] = (int64_t)(uintptr_t)(p->d_factors + n.b);
       }
       w[W_FACTOR_C] = n.measure_after ? 0 : (int64_t)(uintptr_t)(p->d_factors + n.c);
-      (n.invariant ? inv_slots : var_slots).push_back(n.c);
+      (n.phase == 0 ? inv_slots : var_slots).push_back(n.c);
     }
     p->n_var_slots = (int)var_slots.size();
     p->n_inv_slots = (int)inv_slots.size();
@@ -1069,67 +1094,77 @@ int ctgb_plan_set_chunk_desc(ctgb_plan* p, const int64_t* desc) {
   return CTGB_OK;
 }
 
-int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double* exponent_dev, void* workspace,
-                      size_t workspace_bytes, int64_t slice_begin, int64_t slice_step, int64_t slice_count,
-                      void* stream) {
+int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double* exponent_dev,
+                      const void* cotangent, void* const* grads, void* workspace, size_t workspace_bytes,
+                      int64_t slice_begin, int64_t slice_step, int64_t slice_count, void* stream) {
   if (!p) return fail(CTGB_E_VALUE, "null plan");
   if (workspace_bytes < (size_t)(p->workspace_bytes + p->persistent_bytes))
     return fail(CTGB_E_MEMORY, "workspace too small");
+  if (!inputs) return fail(CTGB_E_VALUE, "null inputs");
   if (p->strip_exponent && (!exponent_dev || p->chunk_desc.empty()))
     return fail(CTGB_E_VALUE, "strip_exponent needs an exponent buffer and a chunk descriptor");
+  if (p->strip_exponent && p->root < 0) return fail(CTGB_E_VALUE, "plan has no root node");
+  if ((p->backward || p->cot_offset >= 0) && !cotangent) return fail(CTGB_E_VALUE, "the plan needs a cotangent");
+  for (int i = 0; i < p->n_inputs; ++i)
+    if (p->grad_elems[i] > 0 && (!grads || !grads[i]))
+      return fail(CTGB_E_VALUE, "missing gradient buffer of a differentiated input");
   cudaStream_t st = (cudaStream_t)stream;
   const size_t es = elem_size(p->dtype);
   char* persistent = (char*)workspace;
   char* scratch = persistent + p->persistent_bytes;
-  const int ns = (int)p->radix.size();
-  std::vector<int64_t> digits(ns, 0);
+  std::vector<int64_t> digits(p->radix.size(), 0);
 
   double* d_slice_exp = p->d_scalars + 1;
   double* d_inv_exp = p->d_scalars + 2;
 
   ctgb_slice_mem mem;
   mem.inputs = inputs;
+  mem.grads = grads;
   mem.persistent = persistent;
   mem.scratch = scratch;
   mem.out = (char*)out;
+  mem.cot = (const char*)cotangent;
   mem.es = es;
   mem.digits = digits.data();
   auto resolve = [&](int t, int64_t out_off) -> char* { return resolve_tensor(p->tensors[t], mem, out_off); };
+  int rc;
 
-  auto run_nodes = [&](bool invariant_pass, int64_t out_off) -> int {
+  if (p->cot_offset >= 0) {
+    // H of the root = conj(cotangent): conjugate a copy, the caller's tensor stays as it is
+    char* copy = persistent + p->cot_offset;
+    CUDA_TRY(cudaMemcpyAsync(copy, cotangent, (size_t)p->out_elements * es, cudaMemcpyDeviceToDevice, st));
+    if ((rc = conj_inplace(p->dtype, copy, p->out_elements, st))) return rc;
+    mem.cot = copy;
+  }
+
+  auto run_phase = [&](int phase, int64_t out_off) -> int {
     for (size_t ni = 0; ni < p->nodes.size(); ++ni) {
       const auto& n = p->nodes[ni];
-      if ((n.invariant != 0) != invariant_pass) continue;
+      if (n.phase != phase) continue;
       if (p->profile) cudaEventRecord(p->ev0[ni], st);
       const int64_t* h = p->descs.data() + n.desc_off;
       const int64_t* d = p->d_descs + n.desc_off;
       char* A = resolve(n.a, out_off);
+      char* B = n.kind == 0 ? resolve(n.b, out_off) : nullptr;
       char* C = resolve(n.c, out_off);
-      int rc;
-      if (n.kind == 0) {
-        char* B = resolve(n.b, out_off);
-        if (n.prescale_b) {
-          // the whole underlying buffer of the small operand (a sliced input keeps its base
-          // offset into the copy), scaled by 1/(fA fB) read from the factor slots on the device
-          const ctgb_plan::Tensor& tb = p->tensors[n.b];
-          char* under = tb.kind == 0 ? (char*)inputs[tb.input_index] : (tb.kind == 1 ? scratch : persistent) + tb.offset;
-          rc = scale_copy(p->dtype, under, p->d_bscale, tb.nbytes / (int64_t)es, p->d_factors + n.a,
-                          p->d_factors + n.b, st);
-          if (rc) return rc;
-          B = p->d_bscale + (B - under);
-        }
-        rc = launch_node(0, h, d, A, B, C, st);
-      } else {
-        rc = launch_node(1, h, d, A, nullptr, C, st);
+      if (n.zero_fill) CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)p->tensors[n.c].nbytes, st));
+      if (n.prescale_b) {
+        // the whole underlying buffer of the small operand (a sliced input keeps its base
+        // offset into the copy), scaled by 1/(fA fB) read from the factor slots on the device
+        const ctgb_plan::Tensor& tb = p->tensors[n.b];
+        char* under = tb.kind == 0 ? (char*)inputs[tb.input_index] : (tb.kind == 1 ? scratch : persistent) + tb.offset;
+        if (int r = scale_copy(p->dtype, under, p->d_bscale, tb.nbytes / (int64_t)es, p->d_factors + n.a,
+                               p->d_factors + n.b, st))
+          return r;
+        B = p->d_bscale + (B - under);
       }
-      if (rc) return rc;
+      if (int r = launch_node(n.kind, h, d, A, B, C, st)) return r;
       // contract.py:816-829 strips after every *pairwise* node (single-operand preprocessing
       // steps `continue` before reaching it, :792-796).  The kernels do it in their epilogues
       // (scale by the operands' factors, record max|C|: gett_kernels.cuh StripCtx); only nodes
       // that add partial sums atomically need max|C| measured in a pass of its own.
-      if (p->strip_exponent && n.kind == 0 && n.measure_after) {
-        rc = absmax_into(p->dtype, C, n.c_elems, (unsigned long long*)(p->d_factors + n.c), st);
-        if (rc) return rc;
+      if (n.measure_after) {
+        if (int r = absmax_into(p->dtype, C, n.c_elems, (unsigned long long*)(p->d_factors + n.c), st)) return r;
       }
       if (p->profile) cudaEventRecord(p->ev1[ni], st);
     }
@@ -1137,22 +1172,20 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   };
 
   // slice-invariant subtrees: once per execute call, kept in the persistent arena
-  bool any_inv = false;
-  for (const auto& n : p->nodes) any_inv |= n.invariant != 0;
   if (p->strip_exponent && p->n_inv_slots > 0) {
     reset_slots_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists + p->n_var_slots, p->n_inv_slots);
     g_launches.fetch_add(1, std::memory_order_relaxed);
   }
-  if (any_inv) {
-    int rc = run_nodes(true, 0);
-    if (rc) return rc;
-  }
+  if ((rc = run_phase(0, 0))) return rc;
   if (p->strip_exponent) {
     // exponent of the slice-invariant part: sum of log10(factor) over the hoisted pairwise nodes
     sum_log_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists + p->n_var_slots, p->n_inv_slots, d_inv_exp,
                                       nullptr);
     g_launches.fetch_add(1, std::memory_order_relaxed);
   }
+  // H accumulators of slice-invariant tensors collect every slice of the call
+  for (const auto& q : p->tensors)
+    if (q.kind == 6) CUDA_TRY(cudaMemsetAsync(persistent + q.offset, 0, (size_t)q.nbytes, st));
 
   for (int64_t k = 0; k < slice_count; ++k) {
     const int64_t out_off = decode_slice(slice_begin + k * slice_step, p->radix, p->project, p->out_stride, digits);
@@ -1160,25 +1193,27 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
       reset_slots_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists, p->n_var_slots);
       g_launches.fetch_add(1, std::memory_order_relaxed);
     }
-    int rc = run_nodes(false, out_off);
-    if (rc) return rc;
+    if ((rc = run_phase(1, out_off))) return rc;
+    if ((rc = run_phase(2, out_off))) return rc;
     if (p->strip_exponent) {
       sum_log_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists, p->n_var_slots, d_slice_exp, d_inv_exp);
       g_launches.fetch_add(1, std::memory_order_relaxed);
       // the root wrote a dense mantissa into its workspace slot; fold it into the
       // output against the running exponent (core.py:163-170, 3856-3861)
-      const ctgb_plan::Node* root = nullptr;
-      for (const auto& n : p->nodes)
-        if (n.is_root) root = &n;
-      if (!root) return fail(CTGB_E_VALUE, "plan has no root node");
-      char* m = resolve(root->c, 0);
+      const ctgb_plan::Node& root = p->nodes[p->root];
+      char* m = resolve(root.c, 0);
       // (the stored root is the raw product: its own factor divides it here)
-      const double* froot = root->kind == 0 ? p->d_factors + root->c : nullptr;
+      const double* froot = root.kind == 0 ? p->d_factors + root.c : nullptr;
       rc = accum_stripped(p->dtype, p->d_chunk_desc, p->chunk_desc.data(), out, (char*)out + out_off * (int64_t)es,
                           p->out_elements, m, exponent_dev, d_slice_exp, froot, st);
       if (rc) return rc;
     }
   }
+  // the invariant subtrees are differentiated once, from the accumulated H
+  std::fill(digits.begin(), digits.end(), 0);
+  if ((rc = run_phase(3, 0))) return rc;
+  for (int i = 0; i < p->n_inputs; ++i)
+    if (p->grad_elems[i] > 0 && (rc = conj_inplace(p->dtype, grads[i], p->grad_elems[i], st))) return rc;
   return CTGB_OK;
 }
 
@@ -1237,8 +1272,8 @@ int ctgb_plan_execute_host(ctgb_plan* p, const void* const* host_inputs, const i
     const double ninf = -__builtin_huge_val();
     CUDA_TRY(cudaMemcpyAsync(d_exp, &ninf, sizeof(double), cudaMemcpyHostToDevice, st));
   }
-  int rc = ctgb_plan_execute(p, dev_inputs.data(), ws + out_off, d_exp, workspace, core, slice_begin, slice_step,
-                             slice_count, stream);
+  int rc = ctgb_plan_execute(p, dev_inputs.data(), ws + out_off, d_exp, nullptr, nullptr, workspace, core, slice_begin,
+                             slice_step, slice_count, stream);
   if (rc) return rc;
   CUDA_TRY(cudaMemcpyAsync(host_out, ws + out_off, (size_t)p->out_elements * es, cudaMemcpyDeviceToHost, st));
   if (p->strip_exponent && host_exponent)
@@ -1249,157 +1284,3 @@ int ctgb_plan_execute_host(ctgb_plan* p, const void* const* host_inputs, const i
 
 }  // extern "C"
 
-// ================================================================== VJP plans
-// Reverse mode through a tree (cotengra_b200/vjp.py plans it).  Every backward node is an ordinary
-// pairwise or single-operand descriptor: the plan propagates H = conj(cotangent), for which the
-// adjoint of a contraction needs no conjugation, so only the cotangent's copy and the finished input
-// gradients are conjugated (complex dtypes).
-struct ctgb_vjp {
-  int dtype = 0;
-  int n_inputs = 0;
-  std::vector<ctgb_tensor_rec> tensors;
-  struct Node {
-    int kind, a, b, c, phase, zero_fill;
-    size_t desc_off;
-  };
-  std::vector<Node> nodes;
-  std::vector<int64_t> descs;
-  int64_t* d_descs = nullptr;
-  std::vector<int64_t> radix, project, out_stride;
-  int64_t out_elements = 0, workspace_bytes = 0, persistent_bytes = 0, cot_offset = -1;
-  std::vector<int64_t> grad_elems;  // per input: elements of its gradient (0: not differentiated)
-};
-
-extern "C" {
-
-int ctgb_vjp_create(const ctgb_vjp_desc* vd, ctgb_vjp** out) {
-  if (!vd || !out) return fail(CTGB_E_VALUE, "null argument");
-  const size_t es = elem_size(vd->dtype);
-  if (es == 0) return fail(CTGB_E_VALUE, "bad dtype");
-  const bool cplx = vd->dtype == CTGB_C64 || vd->dtype == CTGB_C128;
-  if (cplx && (vd->cotangent_offset < 0 ||
-               vd->cotangent_offset + vd->out_elements * (int64_t)es > vd->persistent_bytes))
-    return fail(CTGB_E_VALUE, "a complex VJP plan needs room for the conjugated cotangent");
-  ctgb_vjp* v = new ctgb_vjp();
-  v->dtype = vd->dtype;
-  v->n_inputs = vd->n_inputs;
-  if (int rc = copy_tensors(vd->tensors, vd->n_tensors, vd->n_inputs, vd->n_sliced, v->tensors)) {
-    delete v;
-    return rc;
-  }
-  v->grad_elems.assign(vd->n_inputs, 0);
-  for (const auto& q : v->tensors) {
-    if (q.kind < 0 || q.kind > 6 || q.kind == 3) {
-      delete v;
-      return fail(CTGB_E_VALUE, "bad tensor kind for a VJP plan");
-    }
-    if (q.kind == 5) v->grad_elems[q.input_index] = q.nbytes / (int64_t)es;
-  }
-  v->nodes.resize(vd->n_nodes);
-  for (int i = 0; i < vd->n_nodes; ++i) {
-    const ctgb_vjp_node& n = vd->nodes[i];
-    auto& q = v->nodes[i];
-    q.kind = n.kind;
-    q.a = n.a;
-    q.b = n.b;
-    q.c = n.c;
-    q.phase = n.phase;
-    q.zero_fill = n.zero_fill;
-    const int words = n.kind == 0 ? (int)DESC_WORDS : (int)SDESC_WORDS;
-    const int64_t magic = n.kind == 0 ? DESC_MAGIC : SDESC_MAGIC;
-    auto bad = [&](int t) { return t < 0 || t >= vd->n_tensors; };
-    if (n.kind < 0 || n.kind > 1 || !n.desc || n.desc[0] != magic || n.phase < 0 || n.phase > 3 || bad(n.a) ||
-        bad(n.c) || (n.kind == 0 && bad(n.b))) {
-      delete v;
-      return fail(CTGB_E_VALUE, "bad VJP node");
-    }
-    q.desc_off = v->descs.size();
-    v->descs.insert(v->descs.end(), n.desc, n.desc + words);
-  }
-  v->radix.assign(vd->slice_radix, vd->slice_radix + vd->n_sliced);
-  v->project.assign(vd->slice_project, vd->slice_project + vd->n_sliced);
-  v->out_stride.assign(vd->slice_out_stride, vd->slice_out_stride + vd->n_sliced);
-  v->out_elements = vd->out_elements;
-  v->workspace_bytes = vd->workspace_bytes;
-  v->persistent_bytes = vd->persistent_bytes;
-  v->cot_offset = cplx ? vd->cotangent_offset : -1;
-  cudaError_t e = cudaMalloc((void**)&v->d_descs, v->descs.size() * sizeof(int64_t) + 8);
-  if (e == cudaSuccess)
-    e = cudaMemcpy(v->d_descs, v->descs.data(), v->descs.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    std::string msg = cudaGetErrorString(e);
-    ctgb_vjp_destroy(v);
-    return fail(CTGB_E_CUDA, "VJP plan upload: " + msg);
-  }
-  *out = v;
-  return CTGB_OK;
-}
-
-void ctgb_vjp_destroy(ctgb_vjp* v) {
-  if (!v) return;
-  if (v->d_descs) cudaFree(v->d_descs);
-  delete v;
-}
-
-size_t ctgb_vjp_workspace_bytes(const ctgb_vjp* v) {
-  return v ? (size_t)(v->workspace_bytes + v->persistent_bytes) : 0;
-}
-
-int ctgb_vjp_execute(ctgb_vjp* v, const void* const* inputs, const void* cotangent, void* const* grads,
-                     void* workspace, size_t workspace_bytes, int64_t slice_begin, int64_t slice_step,
-                     int64_t slice_count, void* stream) {
-  if (!v) return fail(CTGB_E_VALUE, "null VJP plan");
-  if (workspace_bytes < (size_t)(v->workspace_bytes + v->persistent_bytes))
-    return fail(CTGB_E_MEMORY, "workspace too small");
-  if (!inputs || !cotangent || !grads) return fail(CTGB_E_VALUE, "null argument");
-  for (int i = 0; i < v->n_inputs; ++i)
-    if (v->grad_elems[i] > 0 && !grads[i]) return fail(CTGB_E_VALUE, "missing gradient buffer of a differentiated input");
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t es = elem_size(v->dtype);
-  std::vector<int64_t> digits(v->radix.size(), 0);
-  ctgb_slice_mem mem;
-  mem.inputs = inputs;
-  mem.grads = grads;
-  mem.persistent = (char*)workspace;
-  mem.scratch = mem.persistent + v->persistent_bytes;
-  mem.cot = (const char*)cotangent;
-  mem.es = es;
-  mem.digits = digits.data();
-  int rc;
-  if (v->cot_offset >= 0) {
-    // H of the root = conj(cotangent): conjugate a copy, the caller's tensor stays as it is
-    char* copy = mem.persistent + v->cot_offset;
-    CUDA_TRY(cudaMemcpyAsync(copy, cotangent, (size_t)v->out_elements * es, cudaMemcpyDeviceToDevice, st));
-    if ((rc = conj_inplace(v->dtype, copy, v->out_elements, st))) return rc;
-    mem.cot = copy;
-  }
-  auto run_phase = [&](int phase, int64_t out_off) -> int {
-    for (const auto& n : v->nodes) {
-      if (n.phase != phase) continue;
-      char* A = resolve_tensor(v->tensors[n.a], mem, out_off);
-      char* B = n.kind == 0 ? resolve_tensor(v->tensors[n.b], mem, out_off) : nullptr;
-      char* C = resolve_tensor(v->tensors[n.c], mem, out_off);
-      if (n.zero_fill) CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)v->tensors[n.c].nbytes, st));
-      if (int r = launch_node(n.kind, v->descs.data() + n.desc_off, v->d_descs + n.desc_off, A, B, C, st)) return r;
-    }
-    return CTGB_OK;
-  };
-  // invariant forward: once per call into the persistent arena
-  if ((rc = run_phase(0, 0))) return rc;
-  // H accumulators of slice-invariant tensors collect every slice of the call
-  for (const auto& q : v->tensors)
-    if (q.kind == 6) CUDA_TRY(cudaMemsetAsync(mem.persistent + q.offset, 0, (size_t)q.nbytes, st));
-  for (int64_t k = 0; k < slice_count; ++k) {
-    const int64_t out_off = decode_slice(slice_begin + k * slice_step, v->radix, v->project, v->out_stride, digits);
-    if ((rc = run_phase(1, out_off))) return rc;
-    if ((rc = run_phase(2, out_off))) return rc;
-  }
-  // the invariant subtrees are differentiated once, from the accumulated H
-  std::fill(digits.begin(), digits.end(), 0);
-  if ((rc = run_phase(3, 0))) return rc;
-  for (int i = 0; i < v->n_inputs; ++i)
-    if (v->grad_elems[i] > 0 && (rc = conj_inplace(v->dtype, grads[i], v->grad_elems[i], st))) return rc;
-  return CTGB_OK;
-}
-
-}  // extern "C"

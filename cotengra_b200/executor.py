@@ -16,6 +16,12 @@ Planning is host-side integer work:
 * the root writes straight into the output view selected by the digits of
   sliced *output* indices (gather_slices' stack, core.py:3865-3876) and
   accumulates over inner sliced indices (core.py:3842-3844).
+
+Every node carries the phase it runs in: 0 (invariant forward, once per call)
+and 1 (variant forward, per slice) here; a reverse-mode plan (``vjp.py``) adds
+2 (variant backward) and 3 (invariant backward).  Both plan kinds are one
+``ctgb_plan`` type, laid out by ``layout`` and marshalled and uploaded by
+``_DevicePlan``.
 """
 
 from __future__ import annotations
@@ -41,6 +47,10 @@ from .lowering import (
 )
 
 ALIGN = 256
+# node phases and tensor kinds of a plan (include/ctg_b200.h)
+PHASE_INV_FWD, PHASE_VAR_FWD, PHASE_VAR_BWD, PHASE_INV_BWD = 0, 1, 2, 3
+LOOP_PHASES = (PHASE_VAR_FWD, PHASE_VAR_BWD)  # run once per slice
+K_INPUT, K_SCRATCH, K_PERSISTENT, K_OUTPUT, K_COT, K_GRAD, K_HACC = 0, 1, 2, 3, 4, 5, 6
 
 
 def _align(x):
@@ -111,28 +121,159 @@ def output_chunking(spec):
     return chunk_out, stepsize, spec.nslices // stepsize
 
 
-class _T:
-    """A tensor slot while planning."""
+class _Slot:
+    """A tensor slot while planning; ``kind`` is its ``ctgb_tensor`` kind."""
 
-    __slots__ = ("shape", "strides", "kind", "input_index", "variant", "slot",
-                 "nbytes", "offset", "producer", "last_use", "slice_pos", "slice_stride")
+    __slots__ = ("shape", "strides", "kind", "input_index", "slice_pos", "slice_stride", "nbytes",
+                 "offset", "variant", "first_use", "last_use")
 
-    def __init__(self, shape, strides, kind, variant):
+    def __init__(self, shape, strides, kind, nbytes, input_index=-1, slice_pos=(), slice_stride=(),
+                 variant=False):
         self.shape = tuple(int(d) for d in shape)
-        self.strides = list(strides)
+        self.strides = [int(s) for s in strides]
         self.kind = kind
-        self.variant = variant
-        self.input_index = -1
-        self.slot = -1
-        self.nbytes = 0
+        self.nbytes = int(nbytes)
+        self.input_index = input_index
+        self.slice_pos = list(slice_pos)
+        self.slice_stride = list(slice_stride)
         self.offset = 0
-        self.producer = -1
+        self.variant = variant  # (forward planning) a sliced input lies below it
+        self.first_use = None
         self.last_use = -1
-        self.slice_pos = []
-        self.slice_stride = []
 
 
-class ExecPlan:
+def layout(sched, reserve=0):
+    """Offsets of the scratch and persistent slots of the node schedule ``sched`` (the order the
+    library runs the nodes in, phase by phase) by liveness: a slot is allocated where it is first
+    written and released after its last read.  Persistent values read inside the slice loop
+    (phases 1 and 2) live to its end; H accumulators live from the ``None`` entry of ``sched``,
+    where the slice loop starts and they are zeroed.  ``reserve`` bytes (the conjugated cotangent
+    copy) are taken from the persistent arena first.
+    Returns ``(workspace_bytes, persistent_bytes, reserve_offset)``, the offset -1 without reserve."""
+    zero_pos = sched.index(None) if None in sched else 0
+    end_loop = max((pos for pos, nd in enumerate(sched) if nd is not None and nd["phase"] in LOOP_PHASES),
+                   default=zero_pos)
+    for pos, nd in enumerate(sched):
+        if nd is None:
+            continue
+        c = nd["c"]
+        if c.first_use is None:
+            c.first_use = zero_pos if c.kind == K_HACC else pos
+        for s in (nd["a"], nd["b"]):
+            if s is None:
+                continue
+            s.last_use = max(s.last_use, pos)
+            if s.kind == K_PERSISTENT and nd["phase"] in LOOP_PHASES:
+                s.last_use = max(s.last_use, end_loop)
+    persistent, scratch = _Arena(), _Arena()
+    reserved = persistent.alloc(reserve) if reserve else -1
+    arena = {K_SCRATCH: scratch, K_PERSISTENT: persistent, K_HACC: persistent}
+    allocs, releases = {}, {}
+    for t in _slots(sched):
+        if t.kind in arena:
+            t.last_use = max(t.last_use, t.first_use)
+            allocs.setdefault(t.first_use, []).append(t)
+            releases.setdefault(t.last_use, []).append(t)
+    for pos in range(len(sched)):
+        for t in allocs.get(pos, ()):
+            t.offset = arena[t.kind].alloc(t.nbytes)
+        for t in releases.get(pos, ()):
+            arena[t.kind].release(t.offset, t.nbytes)
+    return _align(scratch.peak), _align(persistent.peak), reserved
+
+
+def _slots(sched):
+    """The slots of a schedule in order of first appearance."""
+    return list(dict.fromkeys(t for nd in sched if nd is not None for t in (nd["a"], nd["b"], nd["c"])
+                              if t is not None))
+
+
+class _DevicePlan:
+    """A schedule as the library runs it: its ``ctgb_plan_desc``, upload and release.  Subclasses
+    set ``dtype``, ``inputs``, ``sliced``, ``slice_out_stride``, ``out_elements``, the arena sizes
+    and ``tensors``/``nodes`` before calling ``_marshal``."""
+
+    handle = None
+    strip_exponent = False
+    cotangent_offset = -1
+
+    def _marshal(self):
+        keep = self._keep = []
+        slot = {id(t): i for i, t in enumerate(self.tensors)}
+        ct = (_lib.CtgbTensor * max(len(self.tensors), 1))()
+        for i, t in enumerate(self.tensors):
+            ct[i].kind = t.kind
+            ct[i].input_index = t.input_index
+            ct[i].offset = t.offset
+            ct[i].nbytes = t.nbytes
+            ct[i].n_sliced = len(t.slice_pos)
+            if t.slice_pos:
+                pos = (C.c_int32 * len(t.slice_pos))(*t.slice_pos)
+                st = (C.c_int64 * len(t.slice_stride))(*t.slice_stride)
+                keep += [pos, st]
+                ct[i].slice_pos = C.cast(pos, C.POINTER(C.c_int32))
+                ct[i].slice_stride = C.cast(st, C.POINTER(C.c_int64))
+        cn = (_lib.CtgbNode * max(len(self.nodes), 1))()
+        for i, nd in enumerate(self.nodes):
+            words = np.ascontiguousarray(nd["words"], dtype=np.int64)
+            keep.append(words)
+            cn[i].kind = nd["kind"]
+            cn[i].a = slot[id(nd["a"])]
+            cn[i].b = slot[id(nd["b"])] if nd["b"] is not None else -1
+            cn[i].c = slot[id(nd["c"])]
+            cn[i].phase = nd["phase"]
+            cn[i].zero_fill = int(nd.get("zero_fill", False))
+            cn[i].is_root = int(nd.get("root", False))
+            cn[i].desc = words.ctypes.data_as(C.POINTER(C.c_int64))
+        ns = len(self.sliced)
+        radix = (C.c_int64 * max(ns, 1))(*[s for _i, s, _p in self.sliced])
+        proj = (C.c_int64 * max(ns, 1))(*[(-1 if p is None else p) for _i, _s, p in self.sliced])
+        ostr = (C.c_int64 * max(ns, 1))(*self.slice_out_stride)
+        keep += [ct, cn, radix, proj, ostr]
+        pd = self._pd = _lib.CtgbPlanDesc()
+        pd.dtype = DTYPE_CODES[self.dtype]
+        pd.n_inputs = len(self.inputs)
+        pd.n_tensors = len(self.tensors)
+        pd.tensors = C.cast(ct, C.POINTER(_lib.CtgbTensor))
+        pd.n_nodes = len(self.nodes)
+        pd.nodes = C.cast(cn, C.POINTER(_lib.CtgbNode))
+        pd.n_sliced = ns
+        pd.slice_radix = C.cast(radix, C.POINTER(C.c_int64))
+        pd.slice_project = C.cast(proj, C.POINTER(C.c_int64))
+        pd.slice_out_stride = C.cast(ostr, C.POINTER(C.c_int64))
+        pd.out_elements = self.out_elements
+        pd.workspace_bytes = self.workspace_bytes
+        pd.persistent_bytes = self.persistent_bytes
+        pd.strip_exponent = int(self.strip_exponent)
+        pd.cotangent_offset = self.cotangent_offset
+        self.total_bytes = self.workspace_bytes + self.persistent_bytes
+
+    def create(self):
+        """Upload the plan to the current CUDA device."""
+        if self.handle is not None:
+            return self
+        lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(lib.ctgb_plan_create(C.byref(self._pd), C.byref(h)))
+        self.handle = h
+        if self.strip_exponent:
+            w = self._chunk_words
+            _lib.check(lib.ctgb_plan_set_chunk_desc(h, w.ctypes.data_as(C.c_void_p)))
+        return self
+
+    def destroy(self):
+        if self.handle is not None:
+            _lib.load().ctgb_plan_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
+class ExecPlan(_DevicePlan):
     """Compile ``contractions`` (reference IR) for fixed input shapes / dtype.
 
     Parameters
@@ -155,14 +296,12 @@ class ExecPlan:
         self.size_dict = dict(size_dict)
         self.sliced = [(i, int(s), None if p is None else int(p)) for i, s, p in sliced]
         self.strip_exponent = bool(strip_exponent)
-        self.handle = None
         if sm_count is None:
             try:
                 sm_count = _lib.device_info()["sm_count"]
             except Exception:
                 sm_count = 132  # H100 SXM
         self.sm_count = sm_count
-        self._keep = []
         self._build(hoist, allow_dmma, variant)
 
     # ------------------------------------------------------------------ build
@@ -185,10 +324,10 @@ class ExecPlan:
         root_term = tuple(ix for ix in self.output if ix not in sliced_pos)
         root_strides = [s for ix, s in zip(self.output, out_full_strides) if ix not in sliced_pos]
         self.root_shape = tuple(self.size_dict[ix] for ix in root_term)
-        slice_out_stride = [0] * len(self.sliced)
+        self.slice_out_stride = [0] * len(self.sliced)
         for ix, s in zip(self.output, out_full_strides):
             if ix in sliced_pos and self.sliced[sliced_pos[ix]][2] is None:
-                slice_out_stride[sliced_pos[ix]] += s
+                self.slice_out_stride[sliced_pos[ix]] += s
 
         # network inputs as strided views of the unsliced arrays
         cur = {}
@@ -198,15 +337,10 @@ class ExecPlan:
             fs = row_major_strides(full_shape)
             self.input_nbytes.append(math.prod(full_shape) * self.esize)
             keep = [k for k, ix in enumerate(term) if ix not in sliced_pos]
-            t = _T([full_shape[k] for k in keep], [fs[k] for k in keep], 0,
-                   variant=any(ix in sliced_pos for ix in term))
-            t.input_index = i
-            t.nbytes = self.input_nbytes[-1]  # the whole (unsliced) array: strip_exponent copies it scaled
-            for k, ix in enumerate(term):
-                if ix in sliced_pos:
-                    t.slice_pos.append(sliced_pos[ix])
-                    t.slice_stride.append(fs[k])
-            cur[i] = t
+            cut = [k for k, ix in enumerate(term) if ix in sliced_pos]
+            # (nbytes: the whole unsliced array, which strip_exponent copies scaled)
+            cur[i] = _Slot([full_shape[k] for k in keep], [fs[k] for k in keep], K_INPUT, self.input_nbytes[-1],
+                           i, [sliced_pos[term[k]] for k in cut], [fs[k] for k in cut], variant=bool(cut))
         self.sliced_shapes = [cur[i].shape for i in range(len(self.inputs))]
 
         tensors = list(cur.values())
@@ -231,7 +365,8 @@ class ExecPlan:
                 # slice sums, split-K atomics and plain stores share one path
                 acc = is_root and not self.strip_exponent
                 words = build_single_desc(odims, sdims, self.dtype, accumulate=acc)
-                dst = _T(oshape, row_major_strides(oshape), 1, src.variant)
+                dst = _Slot(oshape, row_major_strides(oshape), K_SCRATCH, max(math.prod(oshape), 1) * self.esize,
+                            variant=src.variant)
                 nodes.append(dict(kind=1, a=src, b=None, c=dst, words=words, root=is_root))
                 tensors.append(dst)
                 cur[p] = dst
@@ -257,7 +392,8 @@ class ExecPlan:
             dense = 0 if (is_root and not self.strip_exponent) else math.prod(dims.out_shape)
             plan = build_pair_desc(dims, self.dtype, accumulate=acc, sm_count=self.sm_count,
                                    allow_dmma=allow_dmma, c_dense_elems=dense, variant=variant)
-            dst = _T(dims.out_shape, row_major_strides(dims.out_shape), 1, A.variant or Bt.variant)
+            dst = _Slot(dims.out_shape, row_major_strides(dims.out_shape), K_SCRATCH,
+                        max(math.prod(dims.out_shape), 1) * self.esize, variant=A.variant or Bt.variant)
             a, b = (Bt, A) if plan.swapped else (A, Bt)
             nodes.append(dict(kind=0, a=a, b=b, c=dst, words=plan.words, root=is_root, plan=plan,
                               sizes=plan.sizes, dims=dims, acc=acc, dense=dense))
@@ -266,49 +402,22 @@ class ExecPlan:
 
         if not nodes:
             raise ValueError("empty contraction program")
-        root_node = nodes[-1]
         if not self.strip_exponent:
-            root_node["c"].kind = 3  # writes the output accumulator directly
-        # invariance
+            nodes[-1]["c"].kind = K_OUTPUT  # the root writes the output accumulator directly
+        # invariance: hoisted results live in the persistent arena
         for nd in nodes:
             srcs = [nd["a"]] + ([nd["b"]] if nd["b"] is not None else [])
             nd["invariant"] = bool(hoist and not nd["root"] and not any(s.variant for s in srcs))
-            if not nd["invariant"]:
+            nd["phase"] = PHASE_INV_FWD if nd["invariant"] else PHASE_VAR_FWD
+            if nd["invariant"]:
+                nd["c"].kind = K_PERSISTENT
+            else:
                 nd["c"].variant = True
         # schedule: invariant pass then variant pass (the C side runs them so)
         order = [nd for nd in nodes if nd["invariant"]] + [nd for nd in nodes if not nd["invariant"]]
         for pos, nd in enumerate(order):
             nd["pos"] = pos
-            nd["c"].producer = pos
-            for s in (nd["a"], nd["b"]):
-                if s is not None:
-                    s.last_use = max(s.last_use, pos)
-        # persistent tensors read by the variant pass must survive every slice
-        for nd in order:
-            if not nd["invariant"]:
-                for s in (nd["a"], nd["b"]):
-                    if s is not None and s.kind == 1 and s.producer >= 0 and order[s.producer]["invariant"]:
-                        s.last_use = 1 << 60
-        persistent, scratch = _Arena(), _Arena()
-        for pos, nd in enumerate(order):
-            c = nd["c"]
-            arena = persistent if nd["invariant"] else scratch
-            if c.kind == 1:
-                c.nbytes = max(math.prod(c.shape), 1) * self.esize
-                c.offset = arena.alloc(c.nbytes)
-                if nd["invariant"]:
-                    c.kind = 2
-            elif c.kind == 3:
-                c.nbytes = max(math.prod(c.shape), 1) * self.esize
-            for s in (nd["a"], nd["b"]):
-                if s is None or s.last_use != pos:
-                    continue
-                if s.kind == 1:
-                    scratch.release(s.offset, s.nbytes)
-                elif s.kind == 2:
-                    persistent.release(s.offset, s.nbytes)
-        self.workspace_bytes = _align(scratch.peak)
-        self.persistent_bytes = _align(persistent.peak)
+        self.workspace_bytes, self.persistent_bytes, _ = layout(order)
         self.nodes = nodes
         self.n_variant_nodes = sum(1 for nd in nodes if not nd["invariant"])
 
@@ -328,62 +437,14 @@ class ExecPlan:
                 self.macs_per_slice += macs
                 self.elements_per_slice += el
 
-        # ---- marshal for the C-ABI
-        for i, t in enumerate(tensors):
-            t.slot = i
-        n_t = len(tensors)
-        ct = (_lib.CtgbTensor * n_t)()
-        for i, t in enumerate(tensors):
-            ct[i].kind = t.kind
-            ct[i].input_index = t.input_index
-            ct[i].offset = t.offset
-            ct[i].nbytes = t.nbytes
-            ct[i].n_sliced = len(t.slice_pos)
-            if t.slice_pos:
-                pos = (C.c_int32 * len(t.slice_pos))(*t.slice_pos)
-                st = (C.c_int64 * len(t.slice_stride))(*t.slice_stride)
-                self._keep += [pos, st]
-                ct[i].slice_pos = C.cast(pos, C.POINTER(C.c_int32))
-                ct[i].slice_stride = C.cast(st, C.POINTER(C.c_int64))
-        cn = (_lib.CtgbNode * len(nodes))()
-        for i, nd in enumerate(nodes):
-            words = np.ascontiguousarray(nd["words"], dtype=np.int64)
-            self._keep.append(words)
-            cn[i].kind = nd["kind"]
-            cn[i].a = nd["a"].slot
-            cn[i].b = nd["b"].slot if nd["b"] is not None else -1
-            cn[i].c = nd["c"].slot
-            cn[i].invariant = int(nd["invariant"])
-            cn[i].is_root = int(nd["root"])
-            cn[i].desc = words.ctypes.data_as(C.POINTER(C.c_int64))
-        ns = len(self.sliced)
-        radix = (C.c_int64 * max(ns, 1))(*[s for _i, s, _p in self.sliced])
-        proj = (C.c_int64 * max(ns, 1))(*[(-1 if p is None else p) for _i, _s, p in self.sliced])
-        ostr = (C.c_int64 * max(ns, 1))(*slice_out_stride)
-        pd = _lib.CtgbPlanDesc()
-        pd.dtype = DTYPE_CODES[self.dtype]
-        pd.n_inputs = len(self.inputs)
-        pd.n_tensors = n_t
-        pd.tensors = C.cast(ct, C.POINTER(_lib.CtgbTensor))
-        pd.n_nodes = len(nodes)
-        pd.nodes = C.cast(cn, C.POINTER(_lib.CtgbNode))
-        pd.n_sliced = ns
-        pd.slice_radix = C.cast(radix, C.POINTER(C.c_int64))
-        pd.slice_project = C.cast(proj, C.POINTER(C.c_int64))
-        pd.slice_out_stride = C.cast(ostr, C.POINTER(C.c_int64))
-        pd.out_elements = self.out_elements
-        pd.workspace_bytes = self.workspace_bytes
-        pd.persistent_bytes = self.persistent_bytes
-        pd.strip_exponent = int(self.strip_exponent)
-        self._keep += [ct, cn, radix, proj, ostr]
-        self._pd = pd
+        self.tensors = tensors
+        self._marshal()
         if self.strip_exponent:
             # dense root result -> its chunk of the (strided) output
             rs = self.root_shape
             dense = row_major_strides(rs)
             odims = [[e, sx, so] for e, sx, so in zip(rs, dense, root_strides) if e != 1]
             self._chunk_words = build_single_desc(odims, [], self.dtype)
-        self.total_bytes = self.workspace_bytes + self.persistent_bytes
 
     def _check_root_shape(self, shape):
         if tuple(shape) != tuple(self.root_shape):
@@ -393,19 +454,6 @@ class ExecPlan:
             )
 
     # ------------------------------------------------------------------ device side
-    def create(self):
-        """Upload the plan to the current CUDA device."""
-        if self.handle is not None:
-            return self
-        lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(lib.ctgb_plan_create(C.byref(self._pd), C.byref(h)))
-        self.handle = h
-        if self.strip_exponent:
-            w = self._chunk_words
-            _lib.check(lib.ctgb_plan_set_chunk_desc(h, w.ctypes.data_as(C.c_void_p)))
-        return self
-
     def host_staging_bytes(self):
         extra = _align(self.total_bytes) - self.total_bytes
         for n in self.input_nbytes:
@@ -415,7 +463,7 @@ class ExecPlan:
     def execute(self, input_ptrs, out_ptr, exp_ptr, ws_ptr, ws_bytes, begin, step, count, stream=0):
         lib = _lib.load()
         arr = (C.c_void_p * len(input_ptrs))(*input_ptrs)
-        _lib.check(lib.ctgb_plan_execute(self.handle, arr, out_ptr, exp_ptr, ws_ptr, ws_bytes,
+        _lib.check(lib.ctgb_plan_execute(self.handle, arr, out_ptr, exp_ptr, None, None, ws_ptr, ws_bytes,
                                          int(begin), int(step), int(count), stream))
 
     def execute_host(self, host_arrays, host_out, ws_ptr, ws_bytes, begin, step, count, stream=0):
@@ -448,14 +496,3 @@ class ExecPlan:
         pre, after = (C.c_int32 * n)(), (C.c_int32 * n)()
         _lib.check(_lib.load().ctgb_plan_strip_modes(self.handle, pre, after, n))
         return [(int(a), int(b)) for a, b in zip(pre, after)]
-
-    def destroy(self):
-        if self.handle is not None:
-            _lib.load().ctgb_plan_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.destroy()
-        except Exception:
-            pass

@@ -1,5 +1,6 @@
 """Reverse mode through the tree executor: the vector-Jacobian product of a whole sliced tree
-compiled into one ``ctgb_vjp`` whose slice loop runs in C++/CUDA.
+compiled into one ``ctgb_plan`` (the forward plan's type, with backward phases) whose slice
+loop runs in C++/CUDA.
 
 The plan propagates the *conjugated* cotangent ``H = conj(g)``.  For a pairwise node
 ``p = contract(l, r)`` torch's convention ``g_l = g_p . conj(r)^T`` becomes
@@ -13,7 +14,7 @@ descriptor -- a sum becomes a stride-0 read, a transpose strides, a diagonal a w
 summed strides.  Conjugation happens only on a copy of the incoming cotangent and on the
 finished input gradients (complex dtypes).
 
-Schedule (``ctgb_vjp_execute`` runs the phases in this order):
+Schedule (``ctgb_plan_execute`` runs the phases in this order; a forward plan has 0 and 1 only):
 
     0  invariant forward   once per call, into the persistent arena (as ``ExecPlan`` hoists)
        -- the H accumulators of slice-invariant tensors are zeroed --
@@ -25,8 +26,9 @@ Schedule (``ctgb_vjp_execute`` runs the phases in this order):
 
 Only nodes on a path from the root to an input in ``wrt`` are differentiated, and a forward
 node runs only if some backward step reads its value.  Intermediates live until their last
-backward use; both arenas are laid out by liveness over the whole schedule.  The per-slice
-arena keeps every intermediate the backward needs (no recomputation).
+backward use; both arenas are laid out by liveness over the whole schedule (``executor.layout``,
+as for forward plans).  The per-slice arena keeps every intermediate the backward needs (no
+recomputation).
 """
 
 from __future__ import annotations
@@ -34,12 +36,25 @@ from __future__ import annotations
 import ctypes as C
 import math
 
-import numpy as np
-
 from . import _lib
-from .executor import ExecPlan, _align, _Arena
+from .executor import (
+    K_COT,
+    K_GRAD,
+    K_HACC,
+    K_INPUT,
+    K_PERSISTENT,
+    K_SCRATCH,
+    PHASE_INV_BWD,
+    PHASE_INV_FWD,
+    PHASE_VAR_BWD,
+    PHASE_VAR_FWD,
+    ExecPlan,
+    _DevicePlan,
+    _Slot,
+    _slots,
+    layout,
+)
 from .lowering import (
-    DTYPE_CODES,
     VAR_TF32_32x32,
     PairDims,
     build_pair_desc,
@@ -48,11 +63,6 @@ from .lowering import (
     split_equation,
     tensordot_terms,
 )
-
-PHASE_INV_FWD, PHASE_VAR_FWD, PHASE_VAR_BWD, PHASE_INV_BWD = 0, 1, 2, 3
-# tensor kinds of a VJP plan (include/ctg_b200.h)
-K_INPUT, K_SCRATCH, K_PERSISTENT, K_COT, K_GRAD, K_HACC = 0, 1, 2, 4, 5, 6
-
 
 def choose_vjp_variant(dtype, B, M, N, K):
     """``VAR_TF32_32x32`` for the single-precision backward nodes with a small result over a long
@@ -64,26 +74,6 @@ def choose_vjp_variant(dtype, B, M, N, K):
     if M <= 4 and N <= 4 and K >= 1 << 20:
         return None  # DOTSTREAM4
     return VAR_TF32_32x32
-
-
-class _V:
-    """A tensor slot of the VJP schedule."""
-
-    __slots__ = ("shape", "strides", "kind", "input_index", "slice_pos", "slice_stride", "nbytes",
-                 "offset", "first", "last", "slot")
-
-    def __init__(self, shape, strides, kind, nbytes, input_index=-1, slice_pos=(), slice_stride=()):
-        self.shape = tuple(int(d) for d in shape)
-        self.strides = [int(s) for s in strides]
-        self.kind = kind
-        self.nbytes = int(nbytes)
-        self.input_index = input_index
-        self.slice_pos = list(slice_pos)
-        self.slice_stride = list(slice_stride)
-        self.offset = 0
-        self.first = None
-        self.last = -1
-        self.slot = -1
 
 
 def _axes(term, shape, strides):
@@ -152,7 +142,7 @@ def vjp_single_dims(h, t):
     return [[et[ix], sh.get(ix, 0), stt[ix]] for ix in order]
 
 
-class VjpPlan:
+class VjpPlan(_DevicePlan):
     """Compile the VJP of ``contractions`` (the executed IR, stem fusion included) for fixed
     input shapes and dtype.  Same arguments as ``ExecPlan`` plus ``wrt``, the inputs that need a
     gradient (default: all).  ``variant`` forces the kernel of every backward pairwise node."""
@@ -168,13 +158,12 @@ class VjpPlan:
         self.dtype, self.esize, self.sm_count = fwd.dtype, fwd.esize, fwd.sm_count
         self.inputs, self.output, self.sliced = fwd.inputs, fwd.output, fwd.sliced
         self.nslices, self.out_shape, self.out_elements = fwd.nslices, fwd.out_shape, fwd.out_elements
+        self.slice_out_stride = fwd.slice_out_stride
         n_in = len(self.inputs)
         wrt = set(range(n_in)) if wrt is None else {int(i) for i in wrt}
         if any(i < 0 or i >= n_in for i in wrt):
             raise ValueError(f"wrt {sorted(wrt)} names inputs outside 0..{n_in - 1}")
         self.wrt = tuple(sorted(wrt))
-        self.handle = None
-        self._keep = []
         self._build(tuple(contractions), allow_dmma, variant)
 
     # ------------------------------------------------------------------ build
@@ -223,33 +212,33 @@ class VjpPlan:
         vals = {}
         for t in (t for opl, _ in ops for t, _ in opl):
             if t.kind == 0 and id(t) not in vals:
-                vals[id(t)] = _V(t.shape, t.strides, K_INPUT, fwd.input_nbytes[t.input_index], t.input_index,
-                                 t.slice_pos, t.slice_stride)
+                vals[id(t)] = _Slot(t.shape, t.strides, K_INPUT, fwd.input_nbytes[t.input_index], t.input_index,
+                                    t.slice_pos, t.slice_stride)
         for i, nd in enumerate(nodes):
             if runs[i]:
                 c = nd["c"]
                 kind = K_PERSISTENT if nd["invariant"] else K_SCRATCH
-                vals[id(c)] = _V(c.shape, row_major_strides(c.shape), kind, max(math.prod(c.shape), 1) * es)
+                vals[id(c)] = _Slot(c.shape, row_major_strides(c.shape), kind, max(math.prod(c.shape), 1) * es)
 
         # H of the root: the (conjugated) cotangent at the slice's output view
         sliced_inds = {s[0] for s in self.sliced}
         full_strides = row_major_strides(self.out_shape)
         root_strides = [s for ix, s in zip(self.output, full_strides) if ix not in sliced_inds]
         root = nodes[-1]
-        hs = {id(root["c"]): _V(root["c"].shape, root_strides, K_COT, self.out_elements * es)}
+        hs = {id(root["c"]): _Slot(root["c"].shape, root_strides, K_COT, self.out_elements * es)}
         producer_invariant = {id(nd["c"]): bool(nd["invariant"]) for nd in nodes}
 
         def h_of(t, consumer_invariant):
             v = hs.get(id(t))
             if v is None:
                 if t.kind == 0:
-                    v = _V(t.shape, t.strides, K_GRAD, fwd.input_nbytes[t.input_index], t.input_index,
-                           t.slice_pos, t.slice_stride)
+                    v = _Slot(t.shape, t.strides, K_GRAD, fwd.input_nbytes[t.input_index], t.input_index,
+                              t.slice_pos, t.slice_stride)
                 else:
                     # H of an invariant tensor read by the slice loop collects every slice
                     hoisted = producer_invariant[id(t)] and not consumer_invariant
                     kind = K_HACC if hoisted else K_SCRATCH
-                    v = _V(t.shape, row_major_strides(t.shape), kind, max(math.prod(t.shape), 1) * es)
+                    v = _Slot(t.shape, row_major_strides(t.shape), kind, max(math.prod(t.shape), 1) * es)
                 hs[id(t)] = v
             return v
 
@@ -320,101 +309,16 @@ class VjpPlan:
         self.nodes = [nd for nd in sched if nd is not None]
         self.n_backward_nodes = len(bwd_nodes[PHASE_VAR_BWD]) + len(bwd_nodes[PHASE_INV_BWD])
         self.differentiated = sorted({nd["fwd_index"] for nd in self.nodes if nd["phase"] >= PHASE_VAR_BWD})
-        self._layout(sched)
+        self.tensors = _slots(sched)
+        # the conjugated cotangent copy comes first in the persistent arena
+        cot_bytes = self.out_elements * self.esize if self.dtype.startswith("complex") else 0
+        self.workspace_bytes, self.persistent_bytes, self.cotangent_offset = layout(sched, cot_bytes)
         self._marshal()
 
-    def _layout(self, sched):
-        """Offsets in the two arenas by liveness over the whole forward + backward schedule."""
-        zero_pos = sched.index(None)
-        end_loop = zero_pos
-        for pos, nd in enumerate(sched):
-            if nd is not None and nd["phase"] in (PHASE_VAR_FWD, PHASE_VAR_BWD):
-                end_loop = pos
-        tensors = []
-        for pos, nd in enumerate(sched):
-            if nd is None:
-                continue
-            for t in (nd["a"], nd["b"], nd["c"]):
-                if t is not None and t.slot < 0:
-                    t.slot = len(tensors)
-                    tensors.append(t)
-            c = nd["c"]
-            if c.first is None:
-                c.first = zero_pos if c.kind == K_HACC else pos
-            for s in (nd["a"], nd["b"]):
-                if s is None:
-                    continue
-                s.last = max(s.last, pos)
-                # persistent values read inside the slice loop must survive every slice
-                if s.kind == K_PERSISTENT and nd["phase"] in (PHASE_VAR_FWD, PHASE_VAR_BWD):
-                    s.last = max(s.last, end_loop)
-        self.tensors = tensors
-        persistent, scratch = _Arena(), _Arena()
-        self.cotangent_offset = -1
-        if self.dtype.startswith("complex"):
-            self.cotangent_offset = persistent.alloc(self.out_elements * self.esize)
-        arena = {K_SCRATCH: scratch, K_PERSISTENT: persistent, K_HACC: persistent}
-        placed = [t for t in tensors if t.kind in arena]
-        for t in placed:
-            t.last = max(t.last, t.first)
-        for pos in range(len(sched)):
-            for t in placed:
-                if t.first == pos:
-                    t.offset = arena[t.kind].alloc(t.nbytes)
-            for t in placed:
-                if t.last == pos:
-                    arena[t.kind].release(t.offset, t.nbytes)
-        self.workspace_bytes = _align(scratch.peak)
-        self.persistent_bytes = _align(persistent.peak)
-        self.total_bytes = self.workspace_bytes + self.persistent_bytes
-
-    def _marshal(self):
-        n_t = len(self.tensors)
-        ct = (_lib.CtgbTensor * max(n_t, 1))()
-        for i, t in enumerate(self.tensors):
-            ct[i].kind = t.kind
-            ct[i].input_index = t.input_index
-            ct[i].offset = t.offset
-            ct[i].nbytes = t.nbytes
-            ct[i].n_sliced = len(t.slice_pos)
-            if t.slice_pos:
-                pos = (C.c_int32 * len(t.slice_pos))(*t.slice_pos)
-                st = (C.c_int64 * len(t.slice_stride))(*t.slice_stride)
-                self._keep += [pos, st]
-                ct[i].slice_pos = C.cast(pos, C.POINTER(C.c_int32))
-                ct[i].slice_stride = C.cast(st, C.POINTER(C.c_int64))
-        cn = (_lib.CtgbVjpNode * max(len(self.nodes), 1))()
-        for i, nd in enumerate(self.nodes):
-            words = np.ascontiguousarray(nd["words"], dtype=np.int64)
-            self._keep.append(words)
-            cn[i].kind = nd["kind"]
-            cn[i].a = nd["a"].slot
-            cn[i].b = nd["b"].slot if nd["b"] is not None else -1
-            cn[i].c = nd["c"].slot
-            cn[i].phase = nd["phase"]
-            cn[i].zero_fill = int(nd["zero_fill"])
-            cn[i].desc = words.ctypes.data_as(C.POINTER(C.c_int64))
-        ns = len(self.sliced)
-        radix = (C.c_int64 * max(ns, 1))(*[s for _i, s, _p in self.sliced])
-        proj = (C.c_int64 * max(ns, 1))(*[(-1 if p is None else p) for _i, _s, p in self.sliced])
-        ostr = (C.c_int64 * max(ns, 1))(*[int(self.fwd._pd.slice_out_stride[j]) for j in range(ns)])
-        vd = _lib.CtgbVjpDesc()
-        vd.dtype = DTYPE_CODES[self.dtype]
-        vd.n_inputs = len(self.inputs)
-        vd.n_tensors = n_t
-        vd.tensors = C.cast(ct, C.POINTER(_lib.CtgbTensor))
-        vd.n_nodes = len(self.nodes)
-        vd.nodes = C.cast(cn, C.POINTER(_lib.CtgbVjpNode))
-        vd.n_sliced = ns
-        vd.slice_radix = C.cast(radix, C.POINTER(C.c_int64))
-        vd.slice_project = C.cast(proj, C.POINTER(C.c_int64))
-        vd.slice_out_stride = C.cast(ostr, C.POINTER(C.c_int64))
-        vd.out_elements = self.out_elements
-        vd.workspace_bytes = self.workspace_bytes
-        vd.persistent_bytes = self.persistent_bytes
-        vd.cotangent_offset = self.cotangent_offset
-        self._keep += [ct, cn, radix, proj, ostr]
-        self._vd = vd
+    @property
+    def _vd(self):
+        """The plan's ``ctgb_plan_desc`` (``_pd``) under the name VJP emulation code reads it by."""
+        return self._pd
 
     # ------------------------------------------------------------------ work
     def vjp_macs(self, count):
@@ -427,30 +331,9 @@ class VjpPlan:
         return [int(nd["words"][32]) for nd in self.nodes if nd["kind"] == 0 and nd["phase"] in phases]
 
     # ------------------------------------------------------------------ device side
-    def create(self):
-        """Upload the plan to the current CUDA device."""
-        if self.handle is not None:
-            return self
-        lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(lib.ctgb_vjp_create(C.byref(self._vd), C.byref(h)))
-        self.handle = h
-        return self
-
     def execute(self, input_ptrs, cot_ptr, grad_ptrs, ws_ptr, ws_bytes, begin, step, count, stream=0):
         lib = _lib.load()
         arr = (C.c_void_p * len(input_ptrs))(*input_ptrs)
         grads = (C.c_void_p * len(grad_ptrs))(*grad_ptrs)
-        _lib.check(lib.ctgb_vjp_execute(self.handle, arr, cot_ptr, grads, ws_ptr, ws_bytes, int(begin),
-                                        int(step), int(count), stream))
-
-    def destroy(self):
-        if self.handle is not None:
-            _lib.load().ctgb_vjp_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.destroy()
-        except Exception:
-            pass
+        _lib.check(lib.ctgb_plan_execute(self.handle, arr, None, None, cot_ptr, grads, ws_ptr, ws_bytes, int(begin),
+                                         int(step), int(count), stream))

@@ -47,7 +47,7 @@
 extern "C" {
 #endif
 
-#define CTGB_ABI_VERSION 1
+#define CTGB_ABI_VERSION 2
 
 /* element types (output dtype == input dtype, no casting on the path:
  * cotengra/contract.py has none either) */
@@ -93,11 +93,18 @@ int ctgb_reduce_single(const int64_t* desc, const void* X, void* out,
 
 typedef struct ctgb_plan ctgb_plan;
 
-/* A tensor slot of the plan.  kind: 0 = network input `input_index` (device
- * pointer supplied at execute time; for sliced inputs the per-slice element
- * offset is sum(digit[slice_pos[j]] * slice_stride[j])), 1 = per-slice
- * workspace at byte offset `offset`, 2 = persistent (slice-invariant)
- * workspace at byte offset `offset`, 3 = the output accumulator. */
+/* A tensor slot of the plan.  kind:
+ *   0 = network input `input_index` (device pointer supplied at execute time;
+ *       for sliced inputs the per-slice element offset is
+ *       sum(digit[slice_pos[j]] * slice_stride[j])),
+ *   1 = per-slice workspace at byte offset `offset`,
+ *   2 = persistent (slice-invariant) workspace at byte offset `offset`,
+ *   3 = the output accumulator (at the slice's output view, slice_out_stride),
+ *   4 = the cotangent's view of the slice (element offset as kind 3),
+ *   5 = the gradient of network input `input_index` (slice offset as kind 0),
+ *   6 = a persistent accumulator at byte offset `offset` of the persistent
+ *       arena, zeroed before the slice loop (H of a slice-invariant tensor).
+ * Kinds 4-6 belong to reverse-mode plans, kind 3 to forward ones. */
 typedef struct {
   int32_t kind;
   int32_t input_index;
@@ -108,12 +115,17 @@ typedef struct {
   const int64_t* slice_stride;
 } ctgb_tensor;
 
-/* A node of the linear program (cotengra/contract.py:573-651 IR, lowered). */
+/* A node of the linear program (cotengra/contract.py:573-651 IR, lowered).
+ * A forward plan has phases 0 and 1 only.  A reverse-mode plan propagates
+ * H = conj(cotangent) from the root to the inputs through phases 2 and 3; every
+ * backward step is an ordinary pairwise or single-operand descriptor. */
 typedef struct {
-  int32_t kind;       /* 0 = pairwise (desc = pair words), 1 = single-operand */
-  int32_t a, b, c;    /* tensor slots (b unused for kind 1)                   */
-  int32_t invariant;  /* 1: no sliced input below it -> run once per execute  */
-  int32_t is_root;    /* 1: writes the output (accumulated over slices)       */
+  int32_t kind;       /* 0 = pairwise (desc = pair words), 1 = single-operand   */
+  int32_t a, b, c;    /* tensor slots (b unused for kind 1)                     */
+  int32_t phase;      /* 0 invariant forward (once), 1 variant forward, 2 variant
+                         backward (per slice), 3 invariant backward (once, last) */
+  int32_t zero_fill;  /* 1: zero tensor c (nbytes) before the launch           */
+  int32_t is_root;    /* 1: writes the output (accumulated over slices)         */
   const int64_t* desc;
 } ctgb_node;
 
@@ -134,12 +146,16 @@ typedef struct {
    * digits of sliced indices that are also OUTPUT indices (gather_slices'
    * stack, core.py:3865-3876); 0 stride for inner sliced indices. */
   const int64_t* slice_out_stride;
-  int64_t out_elements;       /* elements of the full output tensor          */
+  int64_t out_elements;       /* elements of the full output (or cotangent)  */
   int64_t workspace_bytes;    /* per-slice arena                              */
-  int64_t persistent_bytes;   /* slice-invariant arena                        */
-  int32_t strip_exponent;     /* contract.py:816-829 semantics                */
+  int64_t persistent_bytes;   /* arena kept over the whole call               */
+  int32_t strip_exponent;     /* contract.py:816-829 semantics; forward only  */
+  int64_t cotangent_offset;   /* complex reverse-mode plans: byte offset of the
+                                 conjugated cotangent copy in the persistent
+                                 arena; -1 = no copy                          */
 } ctgb_plan_desc;
 
+/* Refuses strip_exponent together with phase 2/3 nodes (CTGB_E_VALUE). */
 int ctgb_plan_create(const ctgb_plan_desc* desc, ctgb_plan** plan);
 /* strip_exponent only: the single-operand descriptor (ctgb_single_desc_words()
  * words) that maps the dense root result of one slice onto its chunk of the
@@ -155,22 +171,38 @@ int64_t ctgb_plan_launches_per_slice(const ctgb_plan* plan);
  * launch (split-K, dot-type, KRED and chunked wgmma nodes). */
 int ctgb_plan_strip_modes(const ctgb_plan* plan, int32_t* prescale_b, int32_t* measure_after, int n);
 
-/* Contract slices slice_begin, slice_begin + slice_step, ... (slice_count of
- * them) and ACCUMULATE their contributions into `out` (device, out_elements of
- * the plan dtype; the caller zeroes it before the first call).  `inputs` is a
- * host array of n_inputs DEVICE pointers to the unsliced, C-contiguous input
- * arrays.  `workspace` must hold ctgb_plan_workspace_bytes() bytes.  With
- * strip_exponent the mantissa is accumulated against the running base-10
+/* Run slices slice_begin, slice_begin + slice_step, ... (slice_count of them).
+ * `inputs` is a host array of n_inputs DEVICE pointers to the unsliced,
+ * C-contiguous input arrays.  `workspace` must hold ctgb_plan_workspace_bytes()
+ * bytes.  A smaller one fails with CTGB_E_MEMORY, and a missing buffer the plan
+ * needs with CTGB_E_VALUE, before any launch.
+ *
+ * A forward plan ACCUMULATES the slices' contributions into `out` (device,
+ * out_elements of the plan dtype; the caller zeroes it before the first call).
+ * With strip_exponent the mantissa is accumulated against the running base-10
  * exponent stored in exponent_dev[0] (device double; core.py:163-170).
- * Asynchronous on `stream`. */
+ * `cotangent` and `grads` may be null.
+ *
+ * A reverse-mode plan forms the input gradients of the sum of the slices for
+ * the output cotangent `cotangent` (device, out_elements).  `grads` is a host
+ * array of n_inputs device pointers, null for inputs that are not
+ * differentiated; the caller zeroes the buffers (the final conjugation of
+ * complex gradients acts on the whole buffer), and on return they hold the
+ * finished gradients in torch's convention (grad_x = sum over outputs of
+ * grad_out * conj(d out / d x)).  `out` and `exponent_dev` may be null.
+ *
+ * Order: conjugated cotangent copy; phase 0; H accumulators zeroed; per slice
+ * phases 1 and 2 (and the stripped accumulation); phase 3; conjugated
+ * gradients.  Asynchronous on `stream`. */
 int ctgb_plan_execute(ctgb_plan* plan, const void* const* inputs, void* out,
-                      double* exponent_dev, void* workspace,
+                      double* exponent_dev, const void* cotangent,
+                      void* const* grads, void* workspace,
                       size_t workspace_bytes, int64_t slice_begin,
                       int64_t slice_step, int64_t slice_count, void* stream);
 
-/* Same job with HOST buffers: copies the inputs host->device, runs the slices,
- * copies the accumulated output (and exponent) back, synchronises.  This is the
- * end-to-end call bench.py times as `e2e`.  `workspace` stays a device buffer
+/* Same job for a forward plan with HOST buffers: copies the inputs
+ * host->device, runs the slices, copies the accumulated output (and exponent)
+ * back, synchronises.  This is the end-to-end call bench.py times as `e2e`.  `workspace` stays a device buffer
  * (it is scratch); input staging memory is taken from its tail. */
 int ctgb_plan_execute_host(ctgb_plan* plan, const void* const* host_inputs,
                            const int64_t* input_nbytes, void* host_out,
@@ -191,62 +223,6 @@ int ctgb_plan_profile_read(ctgb_plan* plan, float* ms, int n_nodes);
  * denominators bench.py uses for the fp64 roofline (MEASURED_PEAKS.json holds
  * only HBM and bf16 numbers). */
 int ctgb_probe_fp64_peaks(double* dmma_tflops, double* dfma_tflops, void* stream);
-
-/* ---- reverse mode (vector-Jacobian products) ----------------------------- */
-
-typedef struct ctgb_vjp ctgb_vjp;
-
-/* A VJP plan propagates H = conj(cotangent) from the root to the inputs; every
- * backward step is an ordinary pairwise or single-operand descriptor.  Its
- * tensor slots are ctgb_tensor records with kinds 0-2 as in plans plus
- *   4 = the cotangent's view of the slice (element offset as the root's output
- *       view, slice_out_stride),
- *   5 = the gradient of network input `input_index` (slice offset as kind 0),
- *   6 = a persistent accumulator at byte offset `offset` of the persistent
- *       arena, zeroed before the slice loop (H of a slice-invariant tensor). */
-typedef struct {
-  int32_t kind;       /* 0 = pairwise, 1 = single-operand                       */
-  int32_t a, b, c;    /* tensor slots (b unused for kind 1)                     */
-  int32_t phase;      /* 0 invariant forward (once), 1 variant forward, 2 variant
-                         backward (per slice), 3 invariant backward (once, last) */
-  int32_t zero_fill;  /* 1: zero tensor c (nbytes) before the launch           */
-  const int64_t* desc;
-} ctgb_vjp_node;
-
-typedef struct {
-  int32_t dtype;
-  int32_t n_inputs;
-  int32_t n_tensors;
-  const ctgb_tensor* tensors;
-  int32_t n_nodes;
-  const ctgb_vjp_node* nodes;
-  int32_t n_sliced;
-  const int64_t* slice_radix;
-  const int64_t* slice_project;
-  const int64_t* slice_out_stride;
-  int64_t out_elements;       /* elements of the full output (the cotangent) */
-  int64_t workspace_bytes;    /* per-slice arena                              */
-  int64_t persistent_bytes;   /* arena kept over the whole call               */
-  int64_t cotangent_offset;   /* complex dtypes: byte offset of the conjugated
-                                 cotangent copy in the persistent arena        */
-} ctgb_vjp_desc;
-
-int ctgb_vjp_create(const ctgb_vjp_desc* desc, ctgb_vjp** vjp);
-void ctgb_vjp_destroy(ctgb_vjp* vjp);
-size_t ctgb_vjp_workspace_bytes(const ctgb_vjp* vjp);
-/* The input gradients of the sum of slices slice_begin, slice_begin +
- * slice_step, ... (slice_count of them) for the output cotangent `cotangent`
- * (device, out_elements).  `grads` is a host array of n_inputs device
- * pointers, null for inputs that are not differentiated; the caller zeroes the
- * buffers (the final conjugation of complex gradients acts on the whole
- * buffer), and on return they hold the finished gradients in torch's
- * convention (grad_x = sum over outputs of grad_out * conj(d out / d x)).  A workspace smaller than ctgb_vjp_workspace_bytes()
- * fails with CTGB_E_MEMORY before any launch.  Asynchronous on `stream`. */
-int ctgb_vjp_execute(ctgb_vjp* vjp, const void* const* inputs,
-                     const void* cotangent, void* const* grads,
-                     void* workspace, size_t workspace_bytes,
-                     int64_t slice_begin, int64_t slice_step,
-                     int64_t slice_count, void* stream);
 
 /* Number of kernels this library has launched since load (bench.py's
  * `gpu_launches`). */

@@ -13,6 +13,7 @@ import math
 
 import numpy as np
 
+from cotengra_b200 import executor as X
 from cotengra_b200 import lowering as L
 
 
@@ -159,38 +160,55 @@ def emulate_single(W, X, out):
         out[oo] = out[oo] + acc if accumulate else acc
 
 
-def emulate_plan(plan, arrays, slice_ids=None):
-    """Run a ``cotengra_b200.executor.ExecPlan`` on the CPU the way
-    ``ctgb_plan_execute`` does (invariant pass, slice digits, input offsets,
-    arenas, root accumulation).  strip_exponent is emulated per node."""
+def emulate_plan(plan, arrays, cotangent=None, slice_ids=None, grads=None):
+    """Run an ``ExecPlan`` or, given the output ``cotangent``, a ``VjpPlan`` on the CPU the way
+    ``ctgb_plan_execute`` does: the conjugated cotangent copy, phase 0, the zeroed H accumulators,
+    per slice phases 1 and 2, phase 3 and the conjugated gradients; slice digits, input, output,
+    cotangent and gradient views, zero fills, and strip_exponent per node.  The arenas are exactly
+    the reported bytes and filled with NaN, as uninitialised device memory may be: an access
+    outside them raises and a read of memory nothing wrote spoils the result.  Returns the output
+    of the slices ``slice_ids`` (default all), with its exponent under strip_exponent, or their
+    gradients (``None`` outside ``plan.wrt``)."""
     dt = np.dtype(plan.dtype)
     es = plan.esize
-    persistent = np.zeros(plan.persistent_bytes // es + 1, dtype=dt)
-    scratch = np.zeros(plan.workspace_bytes // es + 1, dtype=dt)
+    assert plan.workspace_bytes % es == 0 and plan.persistent_bytes % es == 0
+    persistent = np.full(plan.persistent_bytes // es, np.nan, dtype=dt)
+    scratch = np.full(plan.workspace_bytes // es, np.nan, dtype=dt)
     out = np.zeros(max(plan.out_elements, 1), dtype=dt)
     flats = [np.ascontiguousarray(a, dtype=dt).reshape(-1) for a in arrays]
+    if cotangent is not None:
+        if grads is None:
+            grads = [np.zeros(a.size, dtype=dt) if i in plan.wrt else None for i, a in enumerate(flats)]
+        cot = np.ascontiguousarray(cotangent, dtype=dt).reshape(-1)
+        if plan.cotangent_offset >= 0:
+            o = plan.cotangent_offset // es
+            persistent[o:o + cot.size] = np.conj(cot)
+            cot = persistent[o:o + cot.size]
     ns = len(plan.sliced)
     radix = [s for _i, s, _p in plan.sliced]
     proj = [p for _i, _s, p in plan.sliced]
-    out_stride = [int(plan._pd.slice_out_stride[j]) for j in range(ns)]
     E = -math.inf
 
     def view(t, digits, out_off):
-        if t.kind == 0:
+        if t.kind in (X.K_INPUT, X.K_GRAD):
             off = sum(digits[p] * s for p, s in zip(t.slice_pos, t.slice_stride))
-            return flats[t.input_index][off:]
-        if t.kind == 1:
+            return (flats if t.kind == X.K_INPUT else grads)[t.input_index][off:]
+        if t.kind in (X.K_SCRATCH, X.K_PERSISTENT, X.K_HACC):
             assert t.offset % es == 0
-            return scratch[t.offset // es:]
-        if t.kind == 2:
-            assert t.offset % es == 0
-            return persistent[t.offset // es:]
+            return (scratch if t.kind == X.K_SCRATCH else persistent)[t.offset // es:]
+        if t.kind == X.K_COT:
+            return cot[out_off:]
+        assert t.kind == X.K_OUTPUT
         return out[out_off:]
 
-    def run(nodes, digits, out_off, exp):
-        for nd in nodes:
-            a = view(nd["a"], digits, out_off)
+    def run(phase, digits, out_off, exp=0.0):
+        for nd in plan.nodes:
+            if nd["phase"] != phase:
+                continue
             c = view(nd["c"], digits, out_off)
+            if nd.get("zero_fill"):
+                c[: nd["c"].nbytes // es] = 0
+            a = view(nd["a"], digits, out_off)
             if nd["kind"] == 0:
                 emulate_pair(nd["words"], a, view(nd["b"], digits, out_off), c)
                 if plan.strip_exponent:
@@ -204,14 +222,15 @@ def emulate_plan(plan, arrays, slice_ids=None):
                 emulate_single(nd["words"], a, c)
         return exp
 
-    inv = [nd for nd in plan.nodes if nd["invariant"]]
-    var = [nd for nd in plan.nodes if not nd["invariant"]]
-    inv_exp = run(inv, [0] * ns, 0, 0.0)
-    ids = range(plan.nslices) if slice_ids is None else slice_ids
+    zero = [0] * ns
+    inv_exp = run(X.PHASE_INV_FWD, zero, 0)
+    for t in plan.tensors:
+        if t.kind == X.K_HACC:
+            persistent[t.offset // es: (t.offset + t.nbytes) // es] = 0
     strides = [1] * ns
     for j in range(ns - 2, -1, -1):
         strides[j] = strides[j + 1] * radix[j + 1]
-    for i in ids:
+    for i in range(plan.nslices) if slice_ids is None else slice_ids:
         digits, rem = [0] * ns, i
         for j in range(ns):
             if proj[j] is not None:
@@ -219,8 +238,9 @@ def emulate_plan(plan, arrays, slice_ids=None):
             else:
                 digits[j] = rem // strides[j]
                 rem %= strides[j]
-        out_off = sum(d * s for d, s in zip(digits, out_stride))
-        exp = run(var, digits, out_off, inv_exp)
+        out_off = sum(d * s for d, s in zip(digits, plan.slice_out_stride))
+        exp = run(X.PHASE_VAR_FWD, digits, out_off, inv_exp)
+        run(X.PHASE_VAR_BWD, digits, out_off)
         if plan.strip_exponent:
             root = plan.nodes[-1]
             m = view(root["c"], digits, 0)
@@ -231,6 +251,17 @@ def emulate_plan(plan, arrays, slice_ids=None):
             chunk = out[out_off:]
             emulate_single_scaled(plan._chunk_words, m, chunk, sn)
             E = e
+    run(X.PHASE_INV_BWD, zero, 0)
+    if cotangent is not None:
+        res = []
+        for i, g in enumerate(grads):
+            if g is None or i not in plan.wrt:
+                res.append(None)
+                continue
+            if dt.kind == "c":
+                g[:] = np.conj(g)
+            res.append(g.reshape(np.shape(arrays[i])))
+        return res
     res = out[: plan.out_elements].reshape(plan.out_shape)
     return (res, E) if plan.strip_exponent else res
 

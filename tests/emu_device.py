@@ -5,8 +5,9 @@ reference but no GPU.
 
 Everything above the C-ABI call is the product: argument handling, classification, lowering
 to descriptors, plan building (arenas, slice offsets, hoisting, stem fusion).  Only the last
-step -- ``ctgb_contract_pair`` / ``ctgb_reduce_single`` / ``ctgb_plan_execute`` -- is replaced
-by ``tests/desc_emulator.py``, which walks the very descriptors the kernels would receive.
+step -- ``ctgb_contract_pair`` / ``ctgb_reduce_single`` / ``ctgb_plan_execute`` of forward and
+reverse-mode plans -- is replaced by ``tests/desc_emulator.py``, which walks the very descriptors
+the kernels would receive.
 Host tensors (torch CPU) stand in for device memory.  NOT a fallback: it lives under
 ``tests/``, is never imported by ``cotengra_b200`` and is installed by monkeypatching only.
 """
@@ -39,7 +40,7 @@ class FakeLib:
     launches = 0
 
     def ctgb_abi_version(self):
-        return 1
+        return 2
 
     def ctgb_desc_words(self):
         return L.DESC_WORDS
@@ -132,7 +133,7 @@ def install(monkeypatch):
     ``monkeypatch`` fixture)."""
     import torch
 
-    from cotengra_b200 import _lib, contract, executor
+    from cotengra_b200 import _lib, contract, executor, vjp
 
     fake_torch = _FakeTorch()
     fake_lib = FakeLib()
@@ -183,8 +184,25 @@ def install(monkeypatch):
         host_out[...] = np.asarray(res).reshape(host_out.shape)
         return 0.0
 
-    monkeypatch.setattr(executor.ExecPlan, "create", create)
+    def execute_vjp(self, input_ptrs, cot_ptr, grad_ptrs, ws_ptr, ws_bytes, begin, step, count, stream=0):
+        if ws_bytes < self.total_bytes:
+            raise MemoryError("workspace too small")
+        dt = np.dtype(self.dtype)
+        arrays, grads = [], []
+        for i, (ptr, term) in enumerate(zip(input_ptrs, self.inputs)):
+            shape = tuple(self.fwd.size_dict[ix] for ix in term)
+            arrays.append(_view(ptr, dt, math.prod(shape)).reshape(shape))
+            gp = grad_ptrs[i]
+            grads.append(None if gp is None else _view(gp, dt, math.prod(shape)))
+        cot = _view(cot_ptr, dt, max(self.out_elements, 1))[: self.out_elements]
+        ids = range(int(begin), int(begin) + int(step) * int(count), int(step))
+        emu.emulate_plan(self, arrays, cot.copy(), slice_ids=ids, grads=grads)
+        # phases 0 and 3 run once, phases 1 and 2 once per slice
+        FakeLib.launches += sum(1 if nd["phase"] in (0, 3) else len(ids) for nd in self.nodes)
+
+    monkeypatch.setattr(executor._DevicePlan, "create", create)
+    monkeypatch.setattr(executor._DevicePlan, "destroy", lambda self: None)
     monkeypatch.setattr(executor.ExecPlan, "execute", execute)
     monkeypatch.setattr(executor.ExecPlan, "execute_host", execute_host)
-    monkeypatch.setattr(executor.ExecPlan, "destroy", lambda self: None)
+    monkeypatch.setattr(vjp.VjpPlan, "execute", execute_vjp)
     return fake_lib

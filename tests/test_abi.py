@@ -29,7 +29,7 @@ def test_library_exports_header_symbols():
 
 def test_layout_constants_agree():
     lib = _lib.load()
-    assert lib.ctgb_abi_version() == 1
+    assert lib.ctgb_abi_version() == 2
     assert lib.ctgb_desc_words() == lowering.DESC_WORDS
     assert lib.ctgb_single_desc_words() == lowering.SDESC_WORDS
 

@@ -1,4 +1,4 @@
-"""Reverse mode on the device: ``ctgb_vjp_execute`` against the torch-CPU gradient oracle
+"""Reverse mode on the device: ``ctgb_plan_execute`` of VJP plans against the torch-CPU gradient oracle
 (``oracle/grad_oracle.py``), kernel-family coverage of the backward nodes, the autograd paths of
 the public interface, and the workspace check."""
 

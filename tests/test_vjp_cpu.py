@@ -1,5 +1,5 @@
 """Reverse mode (``cotengra_b200/vjp.py``) on the CPU: the VJP plans' descriptors walked by the
-descriptor emulator (``tests/emu_vjp.py``) against the torch-CPU gradient oracle
+descriptor emulator (``tests/desc_emulator.py``) against the torch-CPU gradient oracle
 (``oracle/grad_oracle.py``), finite differences, planner properties, and the autograd paths of
 the public interface with the device launch emulated."""
 
@@ -16,8 +16,8 @@ import cotengra_b200 as cb
 from cotengra_b200 import VjpPlan
 from cotengra_b200.fusion import fuse_stems
 from oracle import grad_oracle as go
-from tests import emu_device, emu_vjp
-from tests.emu_vjp import emulate_vjp
+from tests import emu_device
+from tests.desc_emulator import emulate_plan
 from tests.helpers import load_json, make_arrays, tree_spec
 
 TREES = load_json("trees.json")
@@ -71,23 +71,23 @@ def test_gradients_match_oracle(rec):
         want = go.tree_gradients(spec.inputs, spec.output, spec.sliced, ir, arrays, cot, wrt=wrt)
         w = set(range(n)) if wrt is None else set(wrt)
         plan = base if wrt is None else _plan(spec, dt, wrt=wrt)
-        _check(emulate_vjp(plan, arrays, cot), want, w, 1e-10)
+        _check(emulate_plan(plan, arrays, cot), want, w, 1e-10)
         if wrt is None:
             # hoisting off, and stem fusion forced on (the fused program is differentiated as it runs)
-            _check(emulate_vjp(_plan(spec, dt, hoist=False), arrays, cot), want, w, 1e-10)
+            _check(emulate_plan(_plan(spec, dt, hoist=False), arrays, cot), want, w, 1e-10)
             fused, _info = fuse_stems(spec, dt, min_big=2, ratio=1.0, min_gain=-1.0, model=_bytes_only)
             fplan = VjpPlan(fused.contractions(), spec.inputs, spec.output, spec.size_dict, spec.sliced,
                             dtype=dt, sm_count=8)
-            _check(emulate_vjp(fplan, arrays, cot), want, w, 1e-10)
+            _check(emulate_plan(fplan, arrays, cot), want, w, 1e-10)
     if base.nslices > 1:
         # a slice range split into two calls adds up to the full call
         h = base.nslices // 2
-        g1 = emulate_vjp(base, arrays, cot, slice_ids=range(0, h))
-        g2 = emulate_vjp(base, arrays, cot, slice_ids=range(h, base.nslices))
+        g1 = emulate_plan(base, arrays, cot, slice_ids=range(0, h))
+        g2 = emulate_plan(base, arrays, cot, slice_ids=range(h, base.nslices))
         want1 = go.tree_gradients(spec.inputs, spec.output, spec.sliced, ir, arrays, cot,
                                   slice_ids=range(0, h))
         _check(g1, want1, set(range(n)), 1e-10)
-        full = emulate_vjp(base, arrays, cot)
+        full = emulate_plan(base, arrays, cot)
         for a, b, c in zip(g1, g2, full):
             assert nrel(a + b, c) < 1e-12
 
@@ -104,8 +104,7 @@ def test_central_differences(name):
     plan = _plan(spec, "float64")
     fwd = plan.fwd
     cot = make_arrays([plan.out_shape], "float64", seed=3)[0]
-    grads = emulate_vjp(plan, arrays, cot)
-    from tests.desc_emulator import emulate_plan
+    grads = emulate_plan(plan, arrays, cot)
 
     def loss(xs):
         return float(np.sum(cot * emulate_plan(fwd, xs)))
@@ -135,7 +134,7 @@ def test_complex_tree_against_torch_autograd_directly():
     ts = [torch.tensor(a, requires_grad=True) for a in arrays]
     out = torch.einsum(eq, *ts)
     want = torch.autograd.grad(out, ts, grad_outputs=torch.tensor(cot).reshape(out.shape))
-    for g, w in zip(emulate_vjp(plan, arrays, cot), want):
+    for g, w in zip(emulate_plan(plan, arrays, cot), want):
         assert nrel(g, w.numpy()) < 1e-12
 
 
@@ -160,7 +159,7 @@ def test_pruned_subtrees_emit_no_backward_nodes():
     assert one.vjp_macs(1) < full.vjp_macs(1)
     arrays = make_arrays(spec.shapes(), rec["dtype"], seed=rec["seed"])
     cot = make_arrays([one.out_shape], rec["dtype"], seed=2)[0]
-    g = emulate_vjp(one, arrays, cot)
+    g = emulate_plan(one, arrays, cot)
     assert g[0] is not None and all(x is None for x in g[1:])
 
 
@@ -197,7 +196,7 @@ def test_tf32_32x32_selected_for_small_single_precision_results_only():
 
 
 def _emulated_executor(monkeypatch, name, **kw):
-    emu_vjp.install(monkeypatch)
+    emu_device.install(monkeypatch)
     rec = next(r for r in TREES if r["name"] == name)
     spec = tree_spec(rec)
     return rec, spec, cb.TreeExecutor(spec, dtype=rec["dtype"], **kw)
@@ -281,7 +280,7 @@ def ctg(monkeypatch):
         for mod in list(sys.modules.values()):
             if getattr(mod, "__name__", "").startswith("cotengra.") and getattr(mod, "do", None) is np_do:
                 monkeypatch.setattr(mod, "do", do)
-        emu_vjp.install(monkeypatch)
+        emu_device.install(monkeypatch)
         yield cotengra
     finally:
         del sys.path[:2]
