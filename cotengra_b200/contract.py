@@ -179,10 +179,13 @@ class TreeExecutor:
     ``TreeSpec.from_cotengra``).  The slice loop, the node loop, the slice
     accumulation and (optionally) exponent stripping all run inside
     ``ctgb_plan_execute``.
+
+    ``vjp_max_bytes`` bounds the workspace of its reverse-mode plans (``vjp_plan``, ``vjp``), which
+    then recompute per-slice forward values instead of keeping them (``VjpPlan(max_bytes=...)``).
     """
 
     def __init__(self, tree, dtype="complex128", strip_exponent=False, device=None,
-                 contractions=None, fuse=True, **plan_opts):
+                 contractions=None, fuse=True, vjp_max_bytes=None, **plan_opts):
         self.spec = tree if isinstance(tree, TreeSpec) else TreeSpec.from_cotengra(tree)
         # stem fusion (fusion.py): an execution-plan transformation of the tree cotengra found --
         # big stem tensors absorb pre-contracted groups of small tensors in one pass.  ``spec``
@@ -209,6 +212,7 @@ class TreeExecutor:
         self._ref_work = None
         self._ir, self._plan_opts = ir, plan_opts
         self._vjp_plans, self._vjp_ws = {}, None
+        self.vjp_max_bytes = vjp_max_bytes
 
     @property
     def reference_work(self):
@@ -282,33 +286,37 @@ class TreeExecutor:
         return ptrs, keep
 
     # ------------------------------------------------------------------ gradients
-    def vjp_plan(self, wrt=None):
-        """The (cached) ``VjpPlan`` of the executed program for the inputs ``wrt`` (default all)."""
+    def vjp_plan(self, wrt=None, max_bytes=None):
+        """The (cached) ``VjpPlan`` of the executed program for the inputs ``wrt`` (default all),
+        within ``max_bytes`` of workspace (default: the executor's ``vjp_max_bytes``)."""
         from .vjp import VjpPlan
 
         n = len(self.spec.inputs)
-        key = tuple(range(n)) if wrt is None else tuple(sorted({int(i) for i in wrt}))
+        wrt = tuple(range(n)) if wrt is None else tuple(sorted({int(i) for i in wrt}))
+        max_bytes = self.vjp_max_bytes if max_bytes is None else max_bytes
+        key = wrt if max_bytes is None else (wrt, max_bytes)
         plan = self._vjp_plans.get(key)
         if plan is None:
             torch = _torch()
             with torch.cuda.device(self.device):
                 plan = VjpPlan(self._ir, self.spec.inputs, self.spec.output, self.spec.size_dict,
-                               self.spec.sliced, dtype=self.dtype, wrt=key,
-                               strip_exponent=self.strip_exponent, **self._plan_opts).create()
+                               self.spec.sliced, dtype=self.dtype, wrt=wrt,
+                               strip_exponent=self.strip_exponent, max_bytes=max_bytes,
+                               **self._plan_opts).create()
             self._vjp_plans[key] = plan
         return plan
 
-    def vjp(self, tensors, cotangent, begin=0, step=1, count=None, wrt=None):
+    def vjp(self, tensors, cotangent, begin=0, step=1, count=None, wrt=None, max_bytes=None):
         """Gradients of the sum of slices ``begin, begin+step, ...`` (``count`` of them) for the
         output cotangent ``cotangent`` (the full output's shape): a list with one tensor per input,
         ``None`` for inputs outside ``wrt`` (default: all).  Complex gradients follow torch's
         convention.  Asynchronous on the current stream.  Gradients are linear in the cotangent and
         additive over slices, so one call per rank over ``rank_slices(...)`` followed by an
-        all-reduce gives the gradient of the whole tree."""
+        all-reduce gives the gradient of the whole tree.  ``max_bytes`` as for ``vjp_plan``."""
         torch = _torch()
         self._check_inputs(tensors)
         begin, step, count = self._check_slice_range(begin, step, count)
-        plan = self.vjp_plan(wrt)
+        plan = self.vjp_plan(wrt, max_bytes)
         tdt = getattr(torch, _NP2T[self.dtype])
         with torch.cuda.device(self.device):
             ptrs, _keep = self._input_ptrs(tensors)
@@ -411,18 +419,20 @@ class TreeExecutor:
 
 
 def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=None,
-                  slice_ids=None, **plan_opts):
+                  slice_ids=None, vjp_max_bytes=None, **plan_opts):
     """``tree.contract(arrays)`` (cotengra/core.py:3943): takes the *unsliced*
     arrays, handles slicing, contraction and gathering, returns the output in
     ``tree.output`` order -- or ``(mantissa, exponent)`` with ``strip_exponent``.
-    numpy in -> numpy out; torch CUDA in -> torch CUDA out."""
+    numpy in -> numpy out; torch CUDA in -> torch CUDA out.  ``vjp_max_bytes`` bounds the
+    workspace of the backward pass (``TreeExecutor``); by default an executor's own bound."""
     torch = _torch()
     if isinstance(tree, TreeExecutor):
         ex = tree
     else:
         if dtype is None:
             dtype = dtype_name(arrays[0].dtype)
-        ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, **plan_opts)
+        ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, vjp_max_bytes=vjp_max_bytes,
+                          **plan_opts)
     all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
     begin, step, count = (0, 1, None) if slice_ids is None else slice_ids
     if all_numpy:
@@ -434,7 +444,8 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
     tensors = [_to_device(a, ex.device)[0] for a in arrays]
     if _records_grad(torch, arrays, ex.strip_exponent):
         return _differentiable(torch, lambda ts: ex.contract_device(ts, begin, step, count),
-                               lambda ts, g, wrt: ex.vjp(ts, g, begin, step, count, wrt=wrt), tensors)
+                               lambda ts, g, wrt: ex.vjp(ts, g, begin, step, count, wrt=wrt,
+                                                         max_bytes=vjp_max_bytes), tensors)
     res = ex.contract_device(tensors, begin, step, count)
     if ex.strip_exponent:
         m, e = res
@@ -636,11 +647,12 @@ class B200Contractor:
     """
 
     __slots__ = ("contractions", "strip_exponent", "check_zero", "implementation", "backend",
-                 "progbar", "_plans", "__weakref__")
+                 "progbar", "vjp_max_bytes", "_plans", "__weakref__")
 
     def __init__(self, contractions, strip_exponent=False, check_zero=False,
-                 implementation="b200", backend=None, progbar=False):
+                 implementation="b200", backend=None, progbar=False, vjp_max_bytes=None):
         self.contractions = tuple(contractions)
+        self.vjp_max_bytes = vjp_max_bytes  # workspace bound of the backward pass (VjpPlan max_bytes)
         self.strip_exponent = strip_exponent
         self.check_zero = check_zero
         self.implementation = implementation
@@ -662,7 +674,7 @@ class B200Contractor:
             n_in = len(shapes)
             inputs = [tuple((i, k) for k in range(len(s))) for i, s in enumerate(shapes)]
             size_dict = {(i, k): d for i, s in enumerate(shapes) for k, d in enumerate(s)}
-            ex = _FlatExecutor(self.contractions, inputs, size_dict, dtype, strip)
+            ex = _FlatExecutor(self.contractions, inputs, size_dict, dtype, strip, self.vjp_max_bytes)
             self._plans[key] = ex
         return ex
 
@@ -699,7 +711,7 @@ class _FlatExecutor:
     """ExecPlan over explicit per-call arrays (no tree-level slicing): the output
     term is whatever the program produces."""
 
-    def __init__(self, contractions, inputs, size_dict, dtype, strip):
+    def __init__(self, contractions, inputs, size_dict, dtype, strip, vjp_max_bytes=None):
         torch = _torch()
         out_shape = _program_output_shape(contractions, [tuple(size_dict[ix] for ix in t) for t in inputs])
         output = tuple(("o", k) for k in range(len(out_shape)))
@@ -713,6 +725,7 @@ class _FlatExecutor:
         self.tdt = getattr(torch, _NP2T[self.plan.dtype])
         self._program = (contractions, inputs, output, sd)
         self._vjp_plans = {}
+        self.vjp_max_bytes = vjp_max_bytes
 
     def run(self, tensors):
         torch = _torch()
@@ -733,7 +746,8 @@ class _FlatExecutor:
         with torch.cuda.device(self.device):
             plan = self._vjp_plans.get(key)
             if plan is None:
-                plan = self._vjp_plans[key] = VjpPlan(*self._program, (), dtype=self.plan.dtype, wrt=key).create()
+                plan = self._vjp_plans[key] = VjpPlan(*self._program, (), dtype=self.plan.dtype, wrt=key,
+                                                              max_bytes=self.vjp_max_bytes).create()
             cot = cotangent.to(device=self.device, dtype=self.tdt).contiguous()
             grads = [torch.zeros(tuple(t.shape), dtype=self.tdt, device=self.device) if i in plan.wrt else None
                      for i, t in enumerate(tensors)]
@@ -772,19 +786,22 @@ def _program_output_shape(contractions, shapes):
     return shp
 
 
-def make_contractor(tree, strip_exponent=False, check_zero=False, **_ignored):
+def make_contractor(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, **_ignored):
     """``cotengra.contract.make_contractor`` for ``implementation="b200"``
     (contract.py:925-1006): the per-slice callable for ``tree``."""
-    return B200Contractor.from_tree(tree, strip_exponent=strip_exponent, check_zero=check_zero)
+    return B200Contractor.from_tree(tree, strip_exponent=strip_exponent, check_zero=check_zero,
+                                    vjp_max_bytes=vjp_max_bytes)
 
 
-def install(tree, strip_exponent=False, check_zero=False):
+def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None):
     """Route ``tree.contract(...)`` / ``tree.contract_slice(...)`` of a live
     cotengra tree through this package's contractor by seeding its contractor cache
     (core.py:3699-3711).  Key order: ``(autojit, order, prefer_einsum,
     strip_exponent, check_zero, implementation, progbar)``.  Call after the tree
-    is final: slicing/reconfiguration clears the cache (core.py:2040, 2087)."""
-    fn = make_contractor(tree, strip_exponent=strip_exponent, check_zero=check_zero)
+    is final: slicing/reconfiguration clears the cache (core.py:2040, 2087).  ``vjp_max_bytes``
+    bounds the workspace of the backward pass of ``tree.contract`` on torch tensors."""
+    fn = make_contractor(tree, strip_exponent=strip_exponent, check_zero=check_zero,
+                         vjp_max_bytes=vjp_max_bytes)
     key = (False, None, False, bool(strip_exponent), check_zero, None, False)
     tree.contraction_cores[key] = fn
     return fn

@@ -148,8 +148,11 @@ def layout(sched, reserve=0):
     written and released after its last read.  Persistent values read inside the slice loop
     (phases 1 and 2) live to its end; H accumulators live from the ``None`` entry of ``sched``,
     where the slice loop starts and they are zeroed.  ``reserve`` bytes (the conjugated cotangent
-    copy) are taken from the persistent arena first.
+    copy) are taken from the persistent arena first.  The liveness fields of the slots are reset on
+    entry, so a planner may lay out candidate schedules that share slots one after another.
     Returns ``(workspace_bytes, persistent_bytes, reserve_offset)``, the offset -1 without reserve."""
+    for t in _slots(sched):
+        t.first_use, t.last_use, t.offset = None, -1, 0
     zero_pos = sched.index(None) if None in sched else 0
     end_loop = max((pos for pos, nd in enumerate(sched) if nd is not None and nd["phase"] in LOOP_PHASES),
                    default=zero_pos)

@@ -27,14 +27,22 @@ Schedule (``ctgb_plan_execute`` runs the phases in this order; a forward plan ha
 Only nodes on a path from the root to an input in ``wrt`` are differentiated, and a forward
 node runs only if some backward step reads its value.  Intermediates live until their last
 backward use; both arenas are laid out by liveness over the whole schedule (``executor.layout``,
-as for forward plans).  The per-slice arena keeps every intermediate the backward needs (no
-recomputation).
+as for forward plans).  Without a budget the per-slice arena keeps every intermediate the backward
+needs.
+
+Under a workspace budget (``max_bytes``) some per-slice forward values are dropped after phase 1
+and recomputed in phase 2: a recomputation is a copy of the forward node's record (same
+descriptor) with phase 2 and a fresh scratch slot, emitted right before the first phase-2 node
+that reads the value and kept until its last read.  A dropped value whose operands were dropped
+recomputes them first, from the nearest kept values.  Which values to drop is a greedy search on
+the arena size ``executor.layout`` reports (see ``VjpPlan._fit``).
 """
 
 from __future__ import annotations
 
 import ctypes as C
 import math
+import numbers
 
 from . import _lib
 from .executor import (
@@ -54,6 +62,7 @@ from .executor import (
     _slots,
     layout,
 )
+from .fusion import node_time
 from .lowering import (
     VAR_TF32_32x32,
     PairDims,
@@ -145,11 +154,20 @@ def vjp_single_dims(h, t):
 class VjpPlan(_DevicePlan):
     """Compile the VJP of ``contractions`` (the executed IR, stem fusion included) for fixed
     input shapes and dtype.  Same arguments as ``ExecPlan`` plus ``wrt``, the inputs that need a
-    gradient (default: all).  ``variant`` forces the kernel of every backward pairwise node."""
+    gradient (default: all).  ``variant`` forces the kernel of every backward pairwise node.
+
+    ``max_bytes`` bounds ``workspace_bytes + persistent_bytes`` by recomputing per-slice forward
+    values in phase 2.  ``None``, or a budget at or above the plan's own size, gives the plan
+    without recomputation.  A budget below the smallest the planner reaches raises
+    ``MemoryError``.  ``recompute_macs`` are the MACs of the phase-2 forward nodes of one slice;
+    ``min_bytes`` is the smallest budget the planner reached (``total_bytes`` without a budget)."""
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  wrt=None, strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None):
+                 variant=None, max_bytes=None):
+        if max_bytes is not None and (isinstance(max_bytes, bool) or not isinstance(max_bytes, numbers.Integral)
+                                      or max_bytes <= 0):
+            raise ValueError(f"max_bytes must be a positive integer, got {max_bytes!r}")
         if strip_exponent:
             raise NotImplementedError("gradients of strip_exponent results are not supported")
         fwd = ExecPlan(contractions, inputs, output, size_dict, sliced, dtype=dtype, hoist=hoist,
@@ -164,10 +182,10 @@ class VjpPlan(_DevicePlan):
         if any(i < 0 or i >= n_in for i in wrt):
             raise ValueError(f"wrt {sorted(wrt)} names inputs outside 0..{n_in - 1}")
         self.wrt = tuple(sorted(wrt))
-        self._build(tuple(contractions), allow_dmma, variant)
+        self._build(tuple(contractions), allow_dmma, variant, None if max_bytes is None else int(max_bytes))
 
     # ------------------------------------------------------------------ build
-    def _build(self, contractions, allow_dmma, variant):
+    def _build(self, contractions, allow_dmma, variant, max_bytes):
         fwd, es, dtype = self.fwd, self.esize, self.dtype
         nodes = fwd.nodes
         # local index terms of every node: [(operand, term)], output term
@@ -306,14 +324,108 @@ class VjpPlan(_DevicePlan):
 
         sched = (fwd_nodes[PHASE_INV_FWD] + [None] + fwd_nodes[PHASE_VAR_FWD] + bwd_nodes[PHASE_VAR_BWD]
                  + bwd_nodes[PHASE_INV_BWD])
-        self.nodes = [nd for nd in sched if nd is not None]
         self.n_backward_nodes = len(bwd_nodes[PHASE_VAR_BWD]) + len(bwd_nodes[PHASE_INV_BWD])
-        self.differentiated = sorted({nd["fwd_index"] for nd in self.nodes if nd["phase"] >= PHASE_VAR_BWD})
-        self.tensors = _slots(sched)
+        self.differentiated = sorted({nd["fwd_index"] for nd in sched if nd is not None and nd["phase"] >= PHASE_VAR_BWD})
         # the conjugated cotangent copy comes first in the persistent arena
         cot_bytes = self.out_elements * self.esize if self.dtype.startswith("complex") else 0
-        self.workspace_bytes, self.persistent_bytes, self.cotangent_offset = layout(sched, cot_bytes)
+        sizes = layout(sched, cot_bytes)
+        self.recompute_macs = 0
+        self.min_bytes = sizes[0] + sizes[1]
+        if max_bytes is not None and sizes[0] + sizes[1] > max_bytes:
+            sched, sizes = self._fit(fwd_nodes, bwd_nodes, cot_bytes, sizes, max_bytes)
+        self.nodes = [nd for nd in sched if nd is not None]
+        self.tensors = _slots(sched)
+        self.workspace_bytes, self.persistent_bytes, self.cotangent_offset = sizes
         self._marshal()
+
+    # ------------------------------------------------------------------ recomputation
+    def _fit(self, fwd_nodes, bwd_nodes, cot_bytes, sizes, max_bytes):
+        """The schedule with recomputation that fits ``max_bytes`` at the least estimated recompute
+        time the greedy search finds, and its ``layout``.
+
+        The candidates are the per-slice values a phase-2 node reads that take at least 1/1024 of
+        the unbudgeted arena (the stem tensors; smaller values stay kept).  Starting from every
+        candidate kept, each step drops the candidate with the largest arena reduction per second of
+        added recompute time (``fusion.node_time``), or, where no single drop lowers the arena, the
+        largest reduction of the bytes x schedule positions held.  The search runs until no
+        candidate is left or no drop helps, so ``min_bytes`` is the smallest arena along its path;
+        the plan is the first state of the path within the budget."""
+        var_fwd, var_bwd = fwd_nodes[PHASE_VAR_FWD], bwd_nodes[PHASE_VAR_BWD]
+        producer = {id(rec["c"]): rec for rec in var_fwd}
+        saved = {}
+        for nd in var_bwd:
+            for s in (nd["a"], nd["b"]):
+                if s is not None and id(s) in producer:
+                    saved[id(s)] = s
+        cost = {}
+        for rec in var_fwd:
+            elems = sum(math.prod(s.shape) for s in (rec["a"], rec["b"], rec["c"]) if s is not None)
+            Bn, M, N, K = rec["plan"].sizes if rec["kind"] == 0 else (1, math.prod(rec["c"].shape), 1, 1)
+            cost[id(rec["c"])] = (node_time(self.dtype, Bn, M, N, K, elems), Bn * M * N * K if rec["kind"] == 0 else 0)
+        head, tail = fwd_nodes[PHASE_INV_FWD] + [None], bwd_nodes[PHASE_INV_BWD]
+
+        def schedule(dropped):
+            # phase 1 forms the kept values and what they are formed from
+            kept = saved.keys() - dropped
+            want, run1 = set(kept), []
+            for rec in reversed(var_fwd):
+                if id(rec["c"]) in want:
+                    run1.append(rec)
+                    want.update(id(s) for s in (rec["a"], rec["b"]) if s is not None)
+            run1.reverse()
+            # phase 2 recomputes every other per-slice value where it is first read again
+            mat, run2, t_rec = {}, [], [0.0, 0]
+
+            def get(s):
+                if s is None or id(s) not in producer or id(s) in kept:
+                    return s
+                r = mat.get(id(s))
+                if r is None:
+                    rec = producer[id(s)]
+                    a, b = get(rec["a"]), get(rec["b"])
+                    r = mat[id(s)] = _Slot(s.shape, s.strides, K_SCRATCH, s.nbytes)
+                    run2.append(dict(rec, a=a, b=b, c=r, phase=PHASE_VAR_BWD, recompute=True))
+                    t_rec[0] += cost[id(s)][0]
+                    t_rec[1] += cost[id(s)][1]
+                return r
+
+            for nd in var_bwd:
+                a, b = get(nd["a"]), get(nd["b"])
+                run2.append(nd if a is nd["a"] and b is nd["b"] else dict(nd, a=a, b=b))
+            sched = head + run1 + run2 + tail
+            ws, ps, off = layout(sched, cot_bytes)
+            held = sum(t.nbytes * (t.last_use - t.first_use + 1) for t in _slots(sched) if t.kind == K_SCRATCH)
+            return sched, (ws, ps, off), ws + ps, t_rec[0], held, t_rec[1]
+
+        total0 = sizes[0] + sizes[1]
+        cands = [k for k, s in saved.items() if s.nbytes * 1024 >= total0]
+        dropped = frozenset()
+        state = (total0, 0.0, sum(t.nbytes * (t.last_use - t.first_use + 1)
+                                  for t in _slots(head + var_fwd + var_bwd + tail) if t.kind == K_SCRATCH))
+        path = [(total0, dropped)]
+        while cands:
+            best = None
+            for k in cands:
+                _s, _z, total, t, held, _m = schedule(dropped | {k})
+                dt = max(t - state[1], 0.0) + 1e-6
+                key = (total < state[0], (state[0] - total) / dt if total < state[0] else (state[2] - held) / dt)
+                if best is None or key > best[0]:
+                    best = (key, k, (total, t, held))
+            if not best[0][0] and best[2][2] >= state[2]:
+                break  # no drop lowers the arena or the bytes held
+            dropped = dropped | {best[1]}
+            cands.remove(best[1])
+            state = best[2]
+            path.append((state[0], dropped))
+        self.min_bytes = min(total for total, _d in path)
+        fits = [d for total, d in path if total <= max_bytes]
+        if not fits:
+            err = MemoryError(f"the VJP plan needs at least {self.min_bytes} bytes with recomputation "
+                              f"(min_bytes), {total0} without; the budget is {max_bytes}")
+            err.min_bytes, err.total_bytes = self.min_bytes, total0
+            raise err
+        sched, sizes, _total, _t, _held, self.recompute_macs = schedule(fits[0])
+        return sched, sizes
 
     @property
     def _vd(self):

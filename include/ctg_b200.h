@@ -118,7 +118,10 @@ typedef struct {
 /* A node of the linear program (cotengra/contract.py:573-651 IR, lowered).
  * A forward plan has phases 0 and 1 only.  A reverse-mode plan propagates
  * H = conj(cotangent) from the root to the inputs through phases 2 and 3; every
- * backward step is an ordinary pairwise or single-operand descriptor. */
+ * backward step is an ordinary pairwise or single-operand descriptor.  Phase 2
+ * may also hold forward nodes: a plan under a workspace budget recomputes
+ * per-slice values there, right before the backward steps that read them.
+ * Each phase runs its nodes in list order, so this needs nothing new here. */
 typedef struct {
   int32_t kind;       /* 0 = pairwise (desc = pair words), 1 = single-operand   */
   int32_t a, b, c;    /* tensor slots (b unused for kind 1)                     */
