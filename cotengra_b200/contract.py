@@ -33,6 +33,7 @@ from .executor import ExecPlan, output_chunking
 from .lowering import (
     build_pair_desc,
     build_single_desc,
+    check_precision,
     check_tensordot_shapes,
     classify_pair,
     classify_single,
@@ -90,10 +91,10 @@ def _common_dtype(*ts):
 
 
 @functools.lru_cache(4096)
-def _pair_words(term_a, shape_a, term_b, shape_b, out, dtype, sm_count):
+def _pair_words(term_a, shape_a, term_b, shape_b, out, dtype, sm_count, precision="3xtf32"):
     dims = classify_pair(term_a, shape_a, term_b, shape_b, out)
     plan = build_pair_desc(dims, dtype, sm_count=sm_count,
-                           c_dense_elems=math.prod(dims.out_shape))
+                           c_dense_elems=math.prod(dims.out_shape), precision=precision)
     return plan, dims.out_shape
 
 
@@ -107,13 +108,13 @@ def _sm_count():
     return _lib.device_info()["sm_count"]
 
 
-def _run_pair(term_a, a, term_b, b, out):
+def _run_pair(term_a, a, term_b, b, out, precision="3xtf32"):
     torch = _torch()
     ta, na = _to_device(a)
     tb, nb = _to_device(b, ta.device)
     dtype = _common_dtype(ta, tb)
     plan, oshape = _pair_words(tuple(term_a), tuple(ta.shape), tuple(term_b), tuple(tb.shape),
-                               tuple(out), dtype, _sm_count())
+                               tuple(out), dtype, _sm_count(), precision)
     c = torch.empty(oshape, dtype=ta.dtype, device=ta.device)
     if c.numel():
         pa, pb = (tb, ta) if plan.swapped else (ta, tb)
@@ -123,10 +124,11 @@ def _run_pair(term_a, a, term_b, b, out):
     return _from_device(c, na and nb)
 
 
-def _run_single(term, x, out):
+def _run_single(term, x, out, precision="3xtf32"):
     torch = _torch()
     tx, nx = _to_device(x)
     dtype = dtype_name(tx.dtype)
+    check_precision(precision, dtype)  # (a single-operand node has no tensor-core work to change)
     words, oshape = _single_words(tuple(term), tuple(tx.shape), tuple(out), dtype)
     c = torch.empty(oshape, dtype=tx.dtype, device=tx.device)
     if c.numel():
@@ -136,20 +138,23 @@ def _run_single(term, x, out):
     return _from_device(c, nx)
 
 
-def einsum(eq, a, b=None, *, backend=None):
-    """Single or pairwise einsum (cotengra/contract.py:414-459), one kernel."""
+def einsum(eq, a, b=None, *, backend=None, precision="3xtf32"):
+    """Single or pairwise einsum (cotengra/contract.py:414-459), one kernel.  ``precision="tf32"``
+    runs float32 / complex64 tensor-core work in one tf32 pass (``lowering.PRECISIONS``)."""
+    check_precision(precision)
     terms, out = split_equation(eq)
     if b is None:
         if len(terms) != 1:
             raise ValueError(f"equation {eq!r} needs {len(terms)} operands, got 1")
-        return _run_single(terms[0], a, out)
+        return _run_single(terms[0], a, out, precision)
     if len(terms) != 2:
         raise ValueError(f"equation {eq!r} needs {len(terms)} operands, got 2")
-    return _run_pair(terms[0], a, terms[1], b, out)
+    return _run_pair(terms[0], a, terms[1], b, out, precision)
 
 
-def tensordot(a, b, axes=2, *, backend=None):
-    """Tensordot (cotengra/contract.py:521-570), one kernel."""
+def tensordot(a, b, axes=2, *, backend=None, precision="3xtf32"):
+    """Tensordot (cotengra/contract.py:521-570), one kernel; ``precision`` as for ``einsum``."""
+    check_precision(precision)
     na, nb = len(a.shape), len(b.shape)
     try:
         axes = tuple(map(int, axes[0])), tuple(map(int, axes[1]))
@@ -158,13 +163,15 @@ def tensordot(a, b, axes=2, *, backend=None):
         axes = tuple(range(na - n, na)), tuple(range(n))
     check_tensordot_shapes(axes, tuple(a.shape), tuple(b.shape))
     ta, tb, to = tensordot_terms(axes, na, nb)
-    return _run_pair(ta, a, tb, b, to)
+    return _run_pair(ta, a, tb, b, to, precision)
 
 
-def implementation():
+def implementation(precision="3xtf32"):
     """The ``(einsum, tensordot)`` pair for cotengra's ``implementation=`` kwarg
-    or ``set_default_implementation`` (contract.py:13-31, 775-776)."""
-    return (einsum, tensordot)
+    or ``set_default_implementation`` (contract.py:13-31, 775-776), bound to ``precision``."""
+    if check_precision(precision) == "3xtf32":
+        return (einsum, tensordot)
+    return (functools.partial(einsum, precision=precision), functools.partial(tensordot, precision=precision))
 
 
 # ---------------------------------------------------------------------------
@@ -182,10 +189,14 @@ class TreeExecutor:
 
     ``vjp_max_bytes`` bounds the workspace of its reverse-mode plans (``vjp_plan``, ``vjp``), which
     then recompute per-slice forward values instead of keeping them (``VjpPlan(max_bytes=...)``).
+
+    ``precision`` is the compute mode of the float32 / complex64 tensor-core nodes of every plan it
+    builds (forward, output chunks, reverse mode): ``"3xtf32"`` (default) or ``"tf32"``.
     """
 
     def __init__(self, tree, dtype="complex128", strip_exponent=False, device=None,
-                 contractions=None, fuse=True, vjp_max_bytes=None, **plan_opts):
+                 contractions=None, fuse=True, vjp_max_bytes=None, precision="3xtf32", **plan_opts):
+        check_precision(precision, dtype)
         self.spec = tree if isinstance(tree, TreeSpec) else TreeSpec.from_cotengra(tree)
         # stem fusion (fusion.py): an execution-plan transformation of the tree cotengra found --
         # big stem tensors absorb pre-contracted groups of small tensors in one pass.  ``spec``
@@ -205,8 +216,9 @@ class TreeExecutor:
         with torch.cuda.device(self.device):
             self.plan = ExecPlan(ir, self.spec.inputs, self.spec.output, self.spec.size_dict,
                                  self.spec.sliced, dtype=dtype, strip_exponent=strip_exponent,
-                                 **plan_opts).create()
+                                 precision=precision, **plan_opts).create()
         self.dtype = self.plan.dtype
+        self.precision = precision
         self.strip_exponent = bool(strip_exponent)
         self._ws = None
         self._ref_work = None
@@ -302,7 +314,7 @@ class TreeExecutor:
                 plan = VjpPlan(self._ir, self.spec.inputs, self.spec.output, self.spec.size_dict,
                                self.spec.sliced, dtype=self.dtype, wrt=wrt,
                                strip_exponent=self.strip_exponent, max_bytes=max_bytes,
-                               **self._plan_opts).create()
+                               precision=self.precision, **self._plan_opts).create()
             self._vjp_plans[key] = plan
         return plan
 
@@ -378,7 +390,7 @@ class TreeExecutor:
             with torch.cuda.device(self.device):
                 self._chunk = ExecPlan(spec.contractions(), spec.inputs, chunk_out, spec.size_dict,
                                        spec.sliced, dtype=self.dtype,
-                                       strip_exponent=self.strip_exponent).create()
+                                       strip_exponent=self.strip_exponent, precision=self.precision).create()
         return self._chunk
 
     def gen_output_chunks(self, arrays, with_key=False):
@@ -419,12 +431,13 @@ class TreeExecutor:
 
 
 def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=None,
-                  slice_ids=None, vjp_max_bytes=None, **plan_opts):
+                  slice_ids=None, vjp_max_bytes=None, precision="3xtf32", **plan_opts):
     """``tree.contract(arrays)`` (cotengra/core.py:3943): takes the *unsliced*
     arrays, handles slicing, contraction and gathering, returns the output in
     ``tree.output`` order -- or ``(mantissa, exponent)`` with ``strip_exponent``.
     numpy in -> numpy out; torch CUDA in -> torch CUDA out.  ``vjp_max_bytes`` bounds the
-    workspace of the backward pass (``TreeExecutor``); by default an executor's own bound."""
+    workspace of the backward pass (``TreeExecutor``); by default an executor's own bound.
+    ``precision`` as for ``TreeExecutor`` (an executor passed in keeps its own)."""
     torch = _torch()
     if isinstance(tree, TreeExecutor):
         ex = tree
@@ -432,7 +445,7 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
         if dtype is None:
             dtype = dtype_name(arrays[0].dtype)
         ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, vjp_max_bytes=vjp_max_bytes,
-                          **plan_opts)
+                          precision=precision, **plan_opts)
     all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
     begin, step, count = (0, 1, None) if slice_ids is None else slice_ids
     if all_numpy:
@@ -495,7 +508,8 @@ def _differentiable(torch, run, vjp, tensors):
     return _GRAD_FN.apply(run, vjp, *tensors)
 
 
-def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=None, **plan_opts):
+def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=None, precision="3xtf32",
+                      **plan_opts):
     """``tree.gen_output_chunks(arrays, with_key=...)`` (cotengra/core.py:3884-3941) on the
     GPU executor; see ``TreeExecutor.gen_output_chunks``."""
     if isinstance(tree, TreeExecutor):
@@ -503,12 +517,12 @@ def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=
     else:
         if dtype is None:
             dtype = dtype_name(arrays[0].dtype)
-        ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, **plan_opts)
+        ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, precision=precision, **plan_opts)
     yield from ex.gen_output_chunks(arrays, with_key=with_key)
 
 
 def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warmup=True,
-              executor=None, **plan_opts):
+              executor=None, precision="3xtf32", **plan_opts):
     """``tree.benchmark(dtype, max_time, min_reps, max_reps, warmup)`` (cotengra/core.py:
     4092-4164) on the GPU executor, same protocol and same keys: random inputs, ``warmup``
     untimed slices, then single slices ``i % nslices`` (each one synchronised, as the
@@ -520,7 +534,7 @@ def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warm
     import time
 
     torch = _torch()
-    ex = executor if executor is not None else TreeExecutor(tree, dtype=dtype, **plan_opts)
+    ex = executor if executor is not None else TreeExecutor(tree, dtype=dtype, precision=precision, **plan_opts)
     tdt = getattr(torch, _NP2T[ex.dtype])
     gen = torch.Generator(device=ex.device)
     gen.manual_seed(0)
@@ -573,7 +587,7 @@ def _combine_stripped(m1, e1, m2, e2):
 
 
 def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=False, dtype=None,
-                          executor=None, on_block=None, **plan_opts):
+                          executor=None, on_block=None, precision="3xtf32", **plan_opts):
     """``tree.contract(arrays)`` for runs too long to lose (SURVEY 8f-4, partial-sum
     checkpointing; the reference has no equivalent -- ``tree.contract`` restarts at
     slice 0): the slices are contracted in blocks of ``every``, and after each block
@@ -584,20 +598,25 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     different tree or different inputs is refused (``ValueError``), never silently
     overwritten.  Slices are independent, so the result equals the uninterrupted
     run up to floating-point summation order.  numpy inputs and outputs (host path).
-    ``on_block(next_slice, nslices)`` is called after every saved block."""
+    ``on_block(next_slice, nslices)`` is called after every saved block.  A file written
+    under the other ``precision`` is refused too: the two modes give different sums."""
     import hashlib
     import os
 
     if executor is None:
         if dtype is None:
             dtype = dtype_name(arrays[0].dtype)
-        executor = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, **plan_opts)
+        executor = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, precision=precision,
+                                **plan_opts)
     ex = executor
     spec = ex.spec
     host = [np.asarray(a, dtype=ex.dtype, order="C") for a in arrays]
     h = hashlib.sha256()
     h.update(spec.to_json().encode())
     h.update(f"|{ex.dtype}|{int(bool(ex.strip_exponent))}|".encode())
+    precision = getattr(ex, "precision", "3xtf32")
+    if precision != "3xtf32":  # (the default mode hashes as before: existing checkpoints resume)
+        h.update(f"precision={precision}|".encode())
     for a in host:
         h.update(str(a.shape).encode())
         h.update(a.tobytes())
@@ -609,7 +628,7 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     if os.path.exists(checkpoint):
         with np.load(checkpoint, allow_pickle=False) as z:
             if str(z["tag"]) != tag:
-                raise ValueError(f"{checkpoint} belongs to a different tree, dtype or set of input values")
+                raise ValueError(f"{checkpoint} belongs to a different tree, dtype, precision or set of input values")
             done, total, exponent = int(z["next_slice"]), z["partial"], float(z["exponent"])
     while done < nslices:
         count = min(every, nslices - done)
@@ -647,11 +666,13 @@ class B200Contractor:
     """
 
     __slots__ = ("contractions", "strip_exponent", "check_zero", "implementation", "backend",
-                 "progbar", "vjp_max_bytes", "_plans", "__weakref__")
+                 "progbar", "vjp_max_bytes", "precision", "_plans", "__weakref__")
 
     def __init__(self, contractions, strip_exponent=False, check_zero=False,
-                 implementation="b200", backend=None, progbar=False, vjp_max_bytes=None):
+                 implementation="b200", backend=None, progbar=False, vjp_max_bytes=None, precision="3xtf32"):
         self.contractions = tuple(contractions)
+        # compute mode of the float32 / complex64 tensor-core nodes (TreeExecutor); checked per dtype at call
+        self.precision = check_precision(precision)
         self.vjp_max_bytes = vjp_max_bytes  # workspace bound of the backward pass (VjpPlan max_bytes)
         self.strip_exponent = strip_exponent
         self.check_zero = check_zero
@@ -674,7 +695,8 @@ class B200Contractor:
             n_in = len(shapes)
             inputs = [tuple((i, k) for k in range(len(s))) for i, s in enumerate(shapes)]
             size_dict = {(i, k): d for i, s in enumerate(shapes) for k, d in enumerate(s)}
-            ex = _FlatExecutor(self.contractions, inputs, size_dict, dtype, strip, self.vjp_max_bytes)
+            ex = _FlatExecutor(self.contractions, inputs, size_dict, dtype, strip, self.vjp_max_bytes,
+                               self.precision)
             self._plans[key] = ex
         return ex
 
@@ -711,7 +733,7 @@ class _FlatExecutor:
     """ExecPlan over explicit per-call arrays (no tree-level slicing): the output
     term is whatever the program produces."""
 
-    def __init__(self, contractions, inputs, size_dict, dtype, strip, vjp_max_bytes=None):
+    def __init__(self, contractions, inputs, size_dict, dtype, strip, vjp_max_bytes=None, precision="3xtf32"):
         torch = _torch()
         out_shape = _program_output_shape(contractions, [tuple(size_dict[ix] for ix in t) for t in inputs])
         output = tuple(("o", k) for k in range(len(out_shape)))
@@ -719,7 +741,7 @@ class _FlatExecutor:
         sd.update({("o", k): d for k, d in enumerate(out_shape)})
         self.device = torch.device("cuda", torch.cuda.current_device())
         self.plan = ExecPlan(contractions, inputs, output, sd, (), dtype=dtype,
-                             strip_exponent=strip).create()
+                             strip_exponent=strip, precision=precision).create()
         self.strip = strip
         self.ws = torch.empty(max(self.plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
         self.tdt = getattr(torch, _NP2T[self.plan.dtype])
@@ -747,7 +769,8 @@ class _FlatExecutor:
             plan = self._vjp_plans.get(key)
             if plan is None:
                 plan = self._vjp_plans[key] = VjpPlan(*self._program, (), dtype=self.plan.dtype, wrt=key,
-                                                              max_bytes=self.vjp_max_bytes).create()
+                                                              max_bytes=self.vjp_max_bytes,
+                                                              precision=self.plan.precision).create()
             cot = cotangent.to(device=self.device, dtype=self.tdt).contiguous()
             grads = [torch.zeros(tuple(t.shape), dtype=self.tdt, device=self.device) if i in plan.wrt else None
                      for i, t in enumerate(tensors)]
@@ -786,22 +809,24 @@ def _program_output_shape(contractions, shapes):
     return shp
 
 
-def make_contractor(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, **_ignored):
+def make_contractor(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, precision="3xtf32",
+                    **_ignored):
     """``cotengra.contract.make_contractor`` for ``implementation="b200"``
     (contract.py:925-1006): the per-slice callable for ``tree``."""
     return B200Contractor.from_tree(tree, strip_exponent=strip_exponent, check_zero=check_zero,
-                                    vjp_max_bytes=vjp_max_bytes)
+                                    vjp_max_bytes=vjp_max_bytes, precision=precision)
 
 
-def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None):
+def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, precision="3xtf32"):
     """Route ``tree.contract(...)`` / ``tree.contract_slice(...)`` of a live
     cotengra tree through this package's contractor by seeding its contractor cache
     (core.py:3699-3711).  Key order: ``(autojit, order, prefer_einsum,
     strip_exponent, check_zero, implementation, progbar)``.  Call after the tree
     is final: slicing/reconfiguration clears the cache (core.py:2040, 2087).  ``vjp_max_bytes``
-    bounds the workspace of the backward pass of ``tree.contract`` on torch tensors."""
+    bounds the workspace of the backward pass of ``tree.contract`` on torch tensors; ``precision``
+    is the compute mode of its float32 / complex64 tensor-core nodes (``TreeExecutor``)."""
     fn = make_contractor(tree, strip_exponent=strip_exponent, check_zero=check_zero,
-                         vjp_max_bytes=vjp_max_bytes)
+                         vjp_max_bytes=vjp_max_bytes, precision=precision)
     key = (False, None, False, bool(strip_exponent), check_zero, None, False)
     tree.contraction_cores[key] = fn
     return fn
@@ -813,7 +838,7 @@ def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None):
 
 
 def contract_distributed(tree, arrays, root=None, group=None, strip_exponent=False,
-                         dtype=None, executor=None, **plan_opts):
+                         dtype=None, executor=None, precision="3xtf32", **plan_opts):
     """``tree.contract_mpi(arrays, comm, root)`` (cotengra/core.py:4032-4090)
     over ``torch.distributed`` (NCCL on NVLink): rank ``r`` of ``W`` contracts
     slices ``r, r+W, ...`` (core.py:4070), sums them locally on its GPU, then a
@@ -840,7 +865,8 @@ def contract_distributed(tree, arrays, root=None, group=None, strip_exponent=Fal
     if executor is None:
         if dtype is None:
             dtype = dtype_name(arrays[0].dtype)
-        executor = TreeExecutor(spec, dtype=dtype, strip_exponent=strip_exponent, **plan_opts)
+        executor = TreeExecutor(spec, dtype=dtype, strip_exponent=strip_exponent, precision=precision,
+                                **plan_opts)
     all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
     tensors = [_to_device(a, executor.device)[0] for a in arrays]
     begin, step, count = rank_slices(rank, world, spec.nslices)

@@ -393,9 +393,10 @@ struct Tc05Launch {
   unsigned chunks = 0;   // accumulations of the longest contracted range of a work item
 };
 
-template <int NT>
+// (ONE: the one-pass kernel, whose B' k-steps and A' images are half the size)
+template <int NT, bool ONE>
 int tc05_launch_config(const int64_t* h, uint64_t a_addr, int sms, uint64_t smem_optin, Tc05Launch& lc) {
-  using Cfg = Tc05Cfg<NT>;
+  using Cfg = Tc05Cfg<NT, ONE>;
   lc = Tc05Launch();
   auto exact = [&](int pg, int full, int text) { return h[pg] < 0 || (h[full] % h[text]) == 0; };
   // every tile has the same shape: the full 128 x NT x 16, or exact divisors of the index extents
@@ -446,19 +447,19 @@ int tc05_launch_config(const int64_t* h, uint64_t a_addr, int sms, uint64_t smem
 }
 
 // complex64 on wgmma: prepare B' (hi/lo, tile order) once, then the warp-specialised kernel
-template <int NT>
+template <int NT, bool ONE>
 int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
-  using Cfg = Tc05Cfg<NT>;
+  using Cfg = Tc05Cfg<NT, ONE>;
   DevInfo& di = devinfo();
   if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
   Tc05Launch lc;
-  if (int rc = tc05_launch_config<NT>(h, (uint64_t)(uintptr_t)A, di.sms, di.smem_optin, lc)) return rc;
+  if (int rc = tc05_launch_config<NT, ONE>(h, (uint64_t)(uintptr_t)A, di.sms, di.smem_optin, lc)) return rc;
   if (lc.grid == 0) return CTGB_OK;
   static thread_local int attr_dev = -1;
   int dev;
   cudaGetDevice(&dev);
   if (attr_dev != dev) {
-    CUDA_TRY(cudaFuncSetAttribute(tc05_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CUDA_TRY(cudaFuncSetAttribute(tc05_kernel<NT, ONE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)di.smem_optin - 1024));
     attr_dev = dev;
   }
@@ -470,7 +471,7 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   const unsigned long long total = tiles * Cfg::TILE_FLOATS;
   unsigned long long blocks = (total + 255) / 256;
   if (blocks > (unsigned long long)di.sms * 8) blocks = (unsigned long long)di.sms * 8;
-  bprime_kernel<NT><<<(unsigned)blocks, 256, 0, st>>>(d, (const float2*)B, Bp);
+  bprime_kernel<NT, ONE><<<(unsigned)blocks, 256, 0, st>>>(d, (const float2*)B, Bp);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   if (h[W_SPLITK] > 1 && !(h[W_FLAGS] & 1)) {
     if (h[W_CELEMS] <= 0) {
@@ -485,9 +486,9 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   static const bool tm_off = getenv("CTGB_NO_TENSOR_MAP") != nullptr;
   const int tm_rank = tm_off ? 0 : tc05_make_tensor_map(h, A, &tm);
   if (tm_rank) g_tmap_launches.fetch_add(1, std::memory_order_relaxed);
-  tc05_kernel<NT><<<(unsigned)lc.grid, Cfg::THREADS, lc.smem, st>>>(d, (const float2*)A, Bp, (float2*)C,
-                                                                    (unsigned)lc.sa, (unsigned)lc.nb, lc.b_stat, tm,
-                                                                    tm_rank);
+  tc05_kernel<NT, ONE><<<(unsigned)lc.grid, Cfg::THREADS, lc.smem, st>>>(d, (const float2*)A, Bp, (float2*)C,
+                                                                         (unsigned)lc.sa, (unsigned)lc.nb, lc.b_stat,
+                                                                         tm, tm_rank);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
   cudaFreeAsync(Bp, st);
@@ -495,17 +496,21 @@ int launch_tc05(const int64_t* h, const int64_t* d, const void* A, const void* B
   return CTGB_OK;
 }
 
+// flags bit7: float32 / complex64 tensor-core variants run one tf32 pass instead of three
+constexpr int64_t FLAG_TF32_ONE_PASS = 128;
+
 template <typename T>
 int launch_gett_typed(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
   const int variant = (int)h[W_VARIANT];
+  const bool one = (h[W_FLAGS] & FLAG_TF32_ONE_PASS) != 0;
   if (variant == VAR_ROWSTREAM) return launch_rowstream<T>(h, d, A, B, C, st);
   if (variant == VAR_ROWSTREAM_K) return launch_rowstream_longk<T>(h, d, A, B, C, st);
   if (variant == VAR_DMMASTREAM) return launch_dmmastream(h, d, A, B, C, st);
   if (variant == VAR_DOTSTREAM || variant == VAR_DOTSTREAM4) return launch_dotstream<T>(h, d, A, B, C, st);
   if constexpr (std::is_same<T, float2>::value) {
-    if (variant == VAR_TC05_128x64) return launch_tc05<64>(h, d, A, B, C, st);
-    if (variant == VAR_TC05_128x32) return launch_tc05<32>(h, d, A, B, C, st);
-    if (variant == VAR_TC05_128x16) return launch_tc05<16>(h, d, A, B, C, st);
+    if (variant == VAR_TC05_128x64) return one ? launch_tc05<64, true>(h, d, A, B, C, st) : launch_tc05<64, false>(h, d, A, B, C, st);
+    if (variant == VAR_TC05_128x32) return one ? launch_tc05<32, true>(h, d, A, B, C, st) : launch_tc05<32, false>(h, d, A, B, C, st);
+    if (variant == VAR_TC05_128x16) return one ? launch_tc05<16, true>(h, d, A, B, C, st) : launch_tc05<16, false>(h, d, A, B, C, st);
   }
   switch (variant) {
     case VAR_SIMT_64x64: return launch_gett_policy<T, SimtPolicy<T, 64, 64, 8, 3>>(h, d, A, B, C, st);
@@ -534,14 +539,18 @@ int launch_gett_typed(const int64_t* h, const int64_t* d, const void* A, const v
     }
   }
   if constexpr (std::is_same<T, float>::value || std::is_same<T, float2>::value) {
-    // single precision on the tensor pipe: 3xTF32 mma.sync, same tile shapes
+    // single precision on the tensor pipe: 3xTF32 mma.sync (one pass with flags bit7), same tile shapes
     switch (variant) {
-      case VAR_DMMA_128x64: return launch_gett_policy<T, Tf32Policy<T, 4, 2, 2, 4, 16, 3>>(h, d, A, B, C, st);
-      case VAR_DMMA_64x128: return launch_gett_policy<T, Tf32Policy<T, 2, 4, 2, 4, 16, 3>>(h, d, A, B, C, st);
-      case VAR_DMMA_256x32: return launch_gett_policy<T, Tf32Policy<T, 8, 1, 2, 4, 8, 3>>(h, d, A, B, C, st);
-      case VAR_DMMA_256x16: return launch_gett_policy<T, Tf32Policy<T, 8, 1, 2, 2, 8, 3>>(h, d, A, B, C, st);
+#define CTGB_TF32(...)                                                                             \
+  return one ? launch_gett_policy<T, Tf32Policy<T, __VA_ARGS__, true>>(h, d, A, B, C, st)           \
+             : launch_gett_policy<T, Tf32Policy<T, __VA_ARGS__>>(h, d, A, B, C, st)
+      case VAR_DMMA_128x64: CTGB_TF32(4, 2, 2, 4, 16, 3);
+      case VAR_DMMA_64x128: CTGB_TF32(2, 4, 2, 4, 16, 3);
+      case VAR_DMMA_256x32: CTGB_TF32(8, 1, 2, 4, 8, 3);
+      case VAR_DMMA_256x16: CTGB_TF32(8, 1, 2, 2, 8, 3);
       // DMMA_32x32's geometry: one 32 x 32 tile, four warps, the contracted range split over the SMs
-      case VAR_TF32_32x32: return launch_gett_policy<T, Tf32Policy<T, 2, 2, 1, 2, 16, 4>>(h, d, A, B, C, st);
+      case VAR_TF32_32x32: CTGB_TF32(2, 2, 1, 2, 16, 4);
+#undef CTGB_TF32
       default: break;
     }
   }
@@ -819,10 +828,20 @@ int ctgb_tc05_launch_config(const int64_t* words, uint64_t a_addr, int sms, uint
   if (sms < 1) return fail(CTGB_E_VALUE, "sms must be positive");
   Tc05Launch lc;
   int rc;
+  const bool one = (words[W_FLAGS] & FLAG_TF32_ONE_PASS) != 0;
   switch (words[W_VARIANT]) {
-    case VAR_TC05_128x64: rc = tc05_launch_config<64>(words, a_addr, sms, smem_optin, lc); break;
-    case VAR_TC05_128x32: rc = tc05_launch_config<32>(words, a_addr, sms, smem_optin, lc); break;
-    case VAR_TC05_128x16: rc = tc05_launch_config<16>(words, a_addr, sms, smem_optin, lc); break;
+    case VAR_TC05_128x64:
+      rc = one ? tc05_launch_config<64, true>(words, a_addr, sms, smem_optin, lc)
+               : tc05_launch_config<64, false>(words, a_addr, sms, smem_optin, lc);
+      break;
+    case VAR_TC05_128x32:
+      rc = one ? tc05_launch_config<32, true>(words, a_addr, sms, smem_optin, lc)
+               : tc05_launch_config<32, false>(words, a_addr, sms, smem_optin, lc);
+      break;
+    case VAR_TC05_128x16:
+      rc = one ? tc05_launch_config<16, true>(words, a_addr, sms, smem_optin, lc)
+               : tc05_launch_config<16, false>(words, a_addr, sms, smem_optin, lc);
+      break;
     default: return fail(CTGB_E_VALUE, "not a wgmma descriptor");
   }
   if (rc) return rc;

@@ -37,7 +37,10 @@ enum : int {
   W_PGK = 25, W_KFULL = 26, W_KTEXT = 27, W_KW = 28,
   W_NLDA = 29, W_NLDB = 30,
   W_FLAGS = 31,        // bit0: accumulate into C; bit1: column pairs adjacent+aligned in C;
-                       // bit2: tile-grid extents are powers of two; bit3: all m dims are powers of two
+                       // bit2: tile-grid extents are powers of two; bit3: all m dims are powers of two;
+                       // bit4/5: column quads/pairs of 8-byte elements adjacent+aligned in C;
+                       // bit6: wgmma A tile made of contiguous runs; bit7: float32/complex64
+                       // tensor-core variants run ONE round-to-nearest tf32 pass (precision="tf32")
   W_VARIANT = 32,      // kernel variant chosen by the host
   W_CELEMS = 33,       // elements of a dense C (memset before split-K atomics); 0: strided C
   W_RUNA = 34,         // wgmma: elements of the contiguous runs the A tile is made of (flags bit6)

@@ -7,7 +7,8 @@
 //   B'[2n][2k] = Br   B'[2n][2k+1] = -Bi   B'[2n+1][2k] = Bi   B'[2n+1][2k+1] = Br
 // so that C' is C's own interleaved image.  fp32 accuracy comes from the 3xTF32
 // split  D = A'hi*B'hi + (A'lo*B'hi + A'hi*B'lo)  (hi = rn_tf32(x), lo = rn_tf32(x - hi); the tensor
-// core itself would only truncate, which biases a deep tree).
+// core itself would only truncate, which biases a deep tree).  The opt-in one-pass mode (descriptor
+// flags bit7) keeps D = A'hi*B'hi: the same round-to-nearest hi, no lo images.
 //
 // B' (hi and lo, already in shared-memory tile order: wgmma's K-major no-swizzle
 // core-matrix layout [chunk = k'/4][row][k'%4]) is prepared once per launch by
@@ -38,21 +39,26 @@ __device__ __forceinline__ float half_up_tf32(float x) { return __uint_as_float(
 __device__ __forceinline__ float round_tf32(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-// The split for every input: a finite x whose rounding would carry into the exponent is truncated (lo stays
+// hi for every input: a finite x whose rounding would carry into the exponent is truncated (lo stays
 // finite and exact), inf stays inf, a NaN gets its quiet bit set (the MMA reads only the top 10 mantissa
-// bits, so 0x7F800001 would otherwise be read as inf).  lo of an inf or NaN is whatever the add makes of
-// x - hi: the product is non-finite either way.
-__device__ __forceinline__ void tc05_split(float x, float& hi, float& lo) {
+// bits, so 0x7F800001 would otherwise be read as inf).  The one-pass mode's operand is this hi alone.
+__device__ __forceinline__ float tc05_hi(float x) {
   const unsigned u = __float_as_uint(x), a = u & 0x7FFFFFFFu;
   unsigned h = (u + 0x1000u) & 0xFFFFE000u;
   if (a >= 0x7F7FF000u) h = a > 0x7F800000u ? (u | 0x00400000u) : a == 0x7F800000u ? u : (u & 0xFFFFE000u);
-  hi = __uint_as_float(h);
+  return __uint_as_float(h);
+}
+// The split for every input.  lo of an inf or NaN is whatever the add makes of x - hi: the product is
+// non-finite either way.
+__device__ __forceinline__ void tc05_split(float x, float& hi, float& lo) {
+  hi = tc05_hi(x);
   lo = half_up_tf32(x - hi);
 }
 
 // B -> B'hi / B'lo in shared-memory tile order:
 //   Bp[((ib*tiles_n + in)*steps_k + step)][chunk 0..7][row 0..4NT-1: hi rows, then lo rows][4 floats]
-template <int NT>
+// ONE (a single tf32 pass): B'hi alone, rows 0..2NT-1 of every chunk.
+template <int NT, bool ONE = false>
 __global__ void __launch_bounds__(256) bprime_kernel(const int64_t* __restrict__ D, const float2* __restrict__ B,
                                                      float* __restrict__ Bp) {
   constexpr int TILE = 8 * (2 * NT) * 4;
@@ -97,6 +103,10 @@ __global__ void __launch_bounds__(256) bprime_kernel(const int64_t* __restrict__
     }
     const float2 b = B[off];
     const float v = (q == p) ? b.x : (q == 0 ? -b.y : b.y);
+    if constexpr (ONE) {
+      Bp[(idx / TILE) * TILE + ((unsigned long long)chunk * (2 * NT) + row) * 4 + j] = tc05_hi(v);
+      continue;
+    }
     // stacked along N: chunk c holds 4NT rows -- rows [0, 2NT) are B'hi, rows [2NT, 4NT) are B'lo --
     // so that one wgmma of N = 4NT multiplies A'hi with both and one of N = 2NT takes B'hi alone
     const unsigned long long base = (idx / TILE) * (2ull * TILE) + ((unsigned long long)chunk * (4 * NT)) * 4 + j;

@@ -9,6 +9,8 @@
 // Instruction: mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32.
 // Complex products are four real products per fragment pair:
 //     Cr += Ar*Br - Ai*Bi ;  Ci += Ar*Bi + Ai*Br      -> 12 MMAs.
+// ONE_PASS (descriptor flags bit7, opt-in): a*b ~= a_hi*b_hi, one MMA per product (4 per complex
+// fragment pair), with the same round-to-nearest a_hi and the same per-k8 folding.
 #pragma once
 
 __device__ __forceinline__ unsigned to_tf32(float x) {
@@ -16,12 +18,22 @@ __device__ __forceinline__ unsigned to_tf32(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
   return r;
 }
-__device__ __forceinline__ void split_tf32(float x, unsigned& hi, unsigned& lo) {
-  hi = to_tf32(x);
-  // a finite x within half a tf32 ulp of FLT_MAX rounds to inf (and hi + lo = inf - inf): truncate it
-  // instead; inf and NaN inputs pass through
+// a finite x within half a tf32 ulp of FLT_MAX rounds to inf (and hi + lo = inf - inf): truncate it
+// instead; inf and NaN inputs pass through
+__device__ __forceinline__ unsigned hi_tf32(float x) {
+  unsigned hi = to_tf32(x);
   if ((hi & 0x7FFFFFFFu) == 0x7F800000u && (__float_as_uint(x) & 0x7FFFFFFFu) != 0x7F800000u)
     hi = __float_as_uint(x) & 0xFFFFE000u;
+  return hi;
+}
+// the one-pass operand: no lo term carries a NaN into the product, and cvt.rna turns a NaN whose payload
+// lies in the low 13 bits (0x7F800001) into inf, so a NaN gets its quiet bit set instead
+__device__ __forceinline__ unsigned one_pass_tf32(float x) {
+  const unsigned u = __float_as_uint(x);
+  return (u & 0x7FFFFFFFu) > 0x7F800000u ? (u | 0x00400000u) : hi_tf32(x);
+}
+__device__ __forceinline__ void split_tf32(float x, unsigned& hi, unsigned& lo) {
+  hi = hi_tf32(x);
   lo = to_tf32(x - __uint_as_float(hi));
 }
 __device__ __forceinline__ void mma_tf32(float (&c)[4], const unsigned (&a)[4], const unsigned (&b)[2]) {
@@ -38,7 +50,7 @@ __device__ __forceinline__ void mma_3xtf32(float (&c)[4], const unsigned (&ah)[4
   mma_tf32(c, ah, bh);
 }
 
-template <typename T, int WARPS_M, int WARPS_N, int FM, int FN, int KT_, int STAGES_>
+template <typename T, int WARPS_M, int WARPS_N, int FM, int FN, int KT_, int STAGES_, bool ONE_PASS = false>
 struct Tf32Policy {
   // T is float (real) or float2 (complex)
   static constexpr bool CPLX = sizeof(T) == 8;
@@ -73,6 +85,16 @@ struct Tf32Policy {
   __device__ static __forceinline__ float re_of(float2 v) { return v.x; }
   __device__ static __forceinline__ float im_of(float v) { return 0.f; }
   __device__ static __forceinline__ float im_of(float2 v) { return v.y; }
+  // operand conversion and product of the mode (lo is left unset, and never read, in one pass)
+  __device__ static __forceinline__ void split(float x, unsigned& hi, unsigned& lo) {
+    if constexpr (ONE_PASS) hi = one_pass_tf32(x);
+    else split_tf32(x, hi, lo);
+  }
+  __device__ static __forceinline__ void mma(float (&c)[4], const unsigned (&ah)[4], const unsigned (&al)[4],
+                                             const unsigned (&bh)[2], const unsigned (&bl)[2]) {
+    if constexpr (ONE_PASS) mma_tf32(c, ah, bh);
+    else mma_3xtf32(c, ah, al, bh, bl);
+  }
 
   __device__ static __forceinline__ void compute(const T* __restrict__ sA, const T* __restrict__ sB, Acc& acc,
                                                  int kvalid, int ncols) {
@@ -91,8 +113,8 @@ struct Tf32Policy {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const T v = pb[((2 * k8 + h) * NT + j * 8) * 4];
-          split_tf32(re_of(v), brh[j][h], brl[j][h]);
-          if constexpr (CPLX) split_tf32(im_of(v), bih[j][h], bil[j][h]);
+          split(re_of(v), brh[j][h], brl[j][h]);
+          if constexpr (CPLX) split(im_of(v), bih[j][h], bil[j][h]);
         }
 #pragma unroll
       for (int i = 0; i < FM; ++i) {
@@ -101,11 +123,11 @@ struct Tf32Policy {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const T v = pa[((2 * k8 + (e >> 1)) * MT + i * 16 + (e & 1) * 8) * 4];
-          split_tf32(re_of(v), arh[e], arl[e]);
+          split(re_of(v), arh[e], arl[e]);
           if constexpr (CPLX) {
-            split_tf32(im_of(v), aih[e], ail[e]);
+            split(im_of(v), aih[e], ail[e]);
             nih[e] = aih[e] ^ 0x80000000u;  // -Ai
-            nil[e] = ail[e] ^ 0x80000000u;
+            if constexpr (!ONE_PASS) nil[e] = ail[e] ^ 0x80000000u;
           }
         }
 #pragma unroll
@@ -116,12 +138,12 @@ struct Tf32Policy {
           // folded into the running sum with a round-to-nearest FADD
           // (Ootomo & Yokota's error-corrected scheme).
           float tr[4] = {0.f, 0.f, 0.f, 0.f};
-          mma_3xtf32(tr, arh, arl, brh[j], brl[j]);
+          mma(tr, arh, arl, brh[j], brl[j]);
           if constexpr (CPLX) {
             float ti[4] = {0.f, 0.f, 0.f, 0.f};
-            mma_3xtf32(ti, arh, arl, bih[j], bil[j]);
-            mma_3xtf32(tr, nih, nil, bih[j], bil[j]);
-            mma_3xtf32(ti, aih, ail, brh[j], brl[j]);
+            mma(ti, arh, arl, bih[j], bil[j]);
+            mma(tr, nih, nil, bih[j], bil[j]);
+            mma(ti, aih, ail, brh[j], brl[j]);
 #pragma unroll
             for (int e = 0; e < 4; ++e) acc.im[i][j][e] += ti[e];
           }

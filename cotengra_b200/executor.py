@@ -37,6 +37,7 @@ from .lowering import (
     DTYPE_SIZES,
     build_pair_desc,
     build_single_desc,
+    check_precision,
     check_tensordot_shapes,
     classify_pair,
     classify_single,
@@ -286,12 +287,15 @@ class ExecPlan(_DevicePlan):
     output : the full output term.
     size_dict : extent of every index.
     sliced : ordered ``[(ind, size, project)]`` as ``tree.sliced_inds``.
+    precision : ``"3xtf32"`` (default) or ``"tf32"``, the compute mode of the float32 / complex64
+        tensor-core nodes (``lowering.PRECISIONS``); ``"tf32"`` with a double dtype raises ``ValueError``.
     """
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None):
+                 variant=None, precision="3xtf32"):
         self.dtype = dtype_name(dtype)
+        self.precision = check_precision(precision, self.dtype)
         self.esize = DTYPE_SIZES[self.dtype]
         self.contractions = tuple(contractions)
         self.inputs = [tuple(t) for t in inputs]
@@ -394,7 +398,8 @@ class ExecPlan(_DevicePlan):
             acc = is_root and not self.strip_exponent
             dense = 0 if (is_root and not self.strip_exponent) else math.prod(dims.out_shape)
             plan = build_pair_desc(dims, self.dtype, accumulate=acc, sm_count=self.sm_count,
-                                   allow_dmma=allow_dmma, c_dense_elems=dense, variant=variant)
+                                   allow_dmma=allow_dmma, c_dense_elems=dense, variant=variant,
+                                   precision=self.precision)
             dst = _Slot(dims.out_shape, row_major_strides(dims.out_shape), K_SCRATCH,
                         max(math.prod(dims.out_shape), 1) * self.esize, variant=A.variant or Bt.variant)
             a, b = (Bt, A) if plan.swapped else (A, Bt)

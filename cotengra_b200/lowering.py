@@ -90,6 +90,13 @@ VARIANT_TILES = {
     VAR_TF32_32x32: (32, 32, 16),
 }
 
+# compute modes of the float32 / complex64 tensor-core variants: "3xtf32" (the default, fp32 accuracy:
+# hi*hi + hi*lo + lo*hi) or "tf32" (ONE round-to-nearest tf32 pass, fp32 accumulation: about 1e-3
+# relative error per product).  "tf32" sets descriptor flags bit7 on exactly these variants.
+PRECISIONS = ("3xtf32", "tf32")
+FLAG_TF32_ONE_PASS = 128
+TF32_VARIANTS = (VAR_DMMA_128x64, VAR_DMMA_64x128, VAR_DMMA_256x32, VAR_DMMA_256x16, VAR_TF32_32x32) + TC05_VARIANTS
+
 DTYPE_CODES = {"float32": 0, "float64": 1, "complex64": 2, "complex128": 3}
 DTYPE_SIZES = {"float32": 4, "float64": 8, "complex64": 8, "complex128": 16}
 
@@ -104,6 +111,16 @@ def dtype_name(dtype) -> str:
     if name not in DTYPE_CODES:
         raise TypeError(f"unsupported dtype {dtype!r}")
     return name
+
+
+def check_precision(precision, dtype=None):
+    """``precision`` if it is one of ``PRECISIONS`` (and, with ``dtype``, one that dtype has), else
+    ``ValueError``: there is no TF32 path for float64 / complex128."""
+    if not isinstance(precision, str) or precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
+    if precision == "tf32" and dtype is not None and dtype_name(dtype) in ("float64", "complex128"):
+        raise ValueError(f"precision='tf32' applies to float32 and complex64, not {dtype_name(dtype)}")
+    return precision
 
 
 def row_major_strides(shape):
@@ -407,9 +424,11 @@ def choose_variant(dtype, B, M, N, K, allow_dmma=True, allow_stream=True, allow_
 
 def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
                     variant=None, allow_dmma=True, c_dense_elems=0,
-                    force_splitk=None) -> PairPlan:
-    """Pack a classified node into descriptor words."""
+                    force_splitk=None, precision="3xtf32") -> PairPlan:
+    """Pack a classified node into descriptor words.  ``precision`` (``PRECISIONS``) selects the
+    compute mode of the float32 / complex64 tensor-core variants; it changes no other word."""
     dtype = dtype_name(dtype)
+    check_precision(precision, dtype)
     m = coalesce([[d[0], d[1], d[3]] for d in dims.m])          # ext, sA, sC
     n = coalesce([[d[0], d[2], d[3]] for d in dims.n])          # ext, sB, sC
     k = coalesce([[d[0], d[1], d[2]] for d in dims.k])          # ext, sA, sB
@@ -551,20 +570,23 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
             fb = choose_variant(dtype, B, M, N, K, allow_dmma, allow_tc05=False)
             return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=fb,
                                    allow_dmma=allow_dmma, c_dense_elems=c_dense_elems,
-                                   force_splitk=force_splitk)
+                                   force_splitk=force_splitk, precision=precision)
     if variant == VAR_DOTSTREAM and (not (M == 1 and N == 1 and B == 1) or len(gk) > 40 or steps_k >= 1 << 31
                                     or (pk is not None and pk[1] % pk[2] != 0)):
         return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_KRED,
-                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk)
+                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
+                               precision=precision)
     if variant == VAR_DOTSTREAM4 and (not (M <= 4 and N <= 4 and B == 1) or len(gk) > 40 or steps_k >= 1 << 31
                                      or pm is not None or pn is not None
                                      or (pk is not None and pk[1] % pk[2] != 0)
                                      or not (accumulate or c_dense_elems == M * N)):
         return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_SIMT_64x64,
-                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk)
+                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
+                               precision=precision)
     if variant == VAR_DMMASTREAM and (pn is not None or pk is not None or (pm is not None and pm[1] % pm[2] != 0)):
         return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_DMMA_256x16,
-                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk)
+                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
+                               precision=precision)
     if variant == VAR_ROWSTREAM_K:
         # exact tiles, and the k offsets must decompose as chunk_base[k // 8] + in_chunk[k % 8]
         def _koff(e, col):
@@ -579,13 +601,13 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
             return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count,
                                    variant=VAR_ROW_256x4 if N <= 4 else VAR_ROW_128x8,
                                    allow_dmma=allow_dmma, c_dense_elems=c_dense_elems,
-                                   force_splitk=force_splitk)
+                                   force_splitk=force_splitk, precision=precision)
     if variant == VAR_ROWSTREAM and pm is not None and pm[1] % pm[2] != 0:
         # ragged blocked m dim: fall back to the staged row policy
         return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count,
                                variant=VAR_ROW_256x4 if N <= 4 else VAR_ROW_128x8,
                                allow_dmma=allow_dmma, c_dense_elems=c_dense_elems,
-                               force_splitk=force_splitk)
+                               force_splitk=force_splitk, precision=precision)
     # 8-byte element types: groups of 4 (bit4) / 2 (bit5) columns adjacent in C and
     # 32- / 16-byte aligned -> vector row stores in the streaming row kernel
     def _cols_ok(g):
@@ -641,7 +663,8 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
     W[W_RUNA] = run_a
     W[W_FLAGS] = ((1 if accumulate else 0) | (2 if pair_ok else 0) | (4 if grid_pow2 else 0)
                   | (8 if m_pow2 else 0) | (16 if _cols_ok(4) else 0) | (32 if _cols_ok(2) else 0)
-                  | (64 if bulk_a else 0))
+                  | (64 if bulk_a else 0)
+                  | (FLAG_TF32_ONE_PASS if precision == "tf32" and variant in TF32_VARIANTS else 0))
     W[W_VARIANT] = variant
     W[W_CELEMS] = int(c_dense_elems)
 

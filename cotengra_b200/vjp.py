@@ -160,20 +160,21 @@ class VjpPlan(_DevicePlan):
     values in phase 2.  ``None``, or a budget at or above the plan's own size, gives the plan
     without recomputation.  A budget below the smallest the planner reaches raises
     ``MemoryError``.  ``recompute_macs`` are the MACs of the phase-2 forward nodes of one slice;
-    ``min_bytes`` is the smallest budget the planner reached (``total_bytes`` without a budget)."""
+    ``min_bytes`` is the smallest budget the planner reached (``total_bytes`` without a budget).
+    ``precision`` applies to the forward, recomputed and backward nodes alike."""
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  wrt=None, strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None, max_bytes=None):
+                 variant=None, max_bytes=None, precision="3xtf32"):
         if max_bytes is not None and (isinstance(max_bytes, bool) or not isinstance(max_bytes, numbers.Integral)
                                       or max_bytes <= 0):
             raise ValueError(f"max_bytes must be a positive integer, got {max_bytes!r}")
         if strip_exponent:
             raise NotImplementedError("gradients of strip_exponent results are not supported")
         fwd = ExecPlan(contractions, inputs, output, size_dict, sliced, dtype=dtype, hoist=hoist,
-                       allow_dmma=allow_dmma, sm_count=sm_count)
+                       allow_dmma=allow_dmma, sm_count=sm_count, precision=precision)
         self.fwd = fwd
-        self.dtype, self.esize, self.sm_count = fwd.dtype, fwd.esize, fwd.sm_count
+        self.dtype, self.esize, self.sm_count, self.precision = fwd.dtype, fwd.esize, fwd.sm_count, fwd.precision
         self.inputs, self.output, self.sliced = fwd.inputs, fwd.output, fwd.sliced
         self.nslices, self.out_shape, self.out_elements = fwd.nslices, fwd.out_shape, fwd.out_elements
         self.slice_out_stride = fwd.slice_out_stride
@@ -313,7 +314,8 @@ class VjpPlan(_DevicePlan):
                 if v is None:
                     v = choose_vjp_variant(dtype, *dims.sizes())
                 plan = build_pair_desc(dims, dtype, accumulate=acc, sm_count=self.sm_count,
-                                       allow_dmma=allow_dmma, c_dense_elems=dense, variant=v)
+                                       allow_dmma=allow_dmma, c_dense_elems=dense, variant=v,
+                                       precision=self.precision)
                 a, b = (Yv, Hc) if plan.swapped else (Hc, Yv)
                 bwd_nodes[ph].append(dict(kind=0, a=a, b=b, c=HX, words=plan.words, phase=ph,
                                           zero_fill=diag and HX.kind == K_SCRATCH, plan=plan, fwd_index=i))
