@@ -192,10 +192,15 @@ class TreeExecutor:
 
     ``precision`` is the compute mode of the float32 / complex64 tensor-core nodes of every plan it
     builds (forward, output chunks, reverse mode): ``"3xtf32"`` (default) or ``"tf32"``.
+
+    ``stripped_grad=True`` (with ``strip_exponent``) differentiates the mantissa ``m`` of a result
+    ``(m, e)`` with the exponent held constant, ``dm/dx = 10^-e damp/dx``: exact for every loss that
+    depends on the result only through ``m 10^e``.  ``vjp`` then takes the forward's ``exponent``.
     """
 
     def __init__(self, tree, dtype="complex128", strip_exponent=False, device=None,
-                 contractions=None, fuse=True, vjp_max_bytes=None, precision="3xtf32", **plan_opts):
+                 contractions=None, fuse=True, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False,
+                 **plan_opts):
         check_precision(precision, dtype)
         self.spec = tree if isinstance(tree, TreeSpec) else TreeSpec.from_cotengra(tree)
         # stem fusion (fusion.py): an execution-plan transformation of the tree cotengra found --
@@ -220,6 +225,7 @@ class TreeExecutor:
         self.dtype = self.plan.dtype
         self.precision = precision
         self.strip_exponent = bool(strip_exponent)
+        self.stripped_grad = bool(stripped_grad)
         self._ws = None
         self._ref_work = None
         self._ir, self._plan_opts = ir, plan_opts
@@ -314,17 +320,23 @@ class TreeExecutor:
                 plan = VjpPlan(self._ir, self.spec.inputs, self.spec.output, self.spec.size_dict,
                                self.spec.sliced, dtype=self.dtype, wrt=wrt,
                                strip_exponent=self.strip_exponent, max_bytes=max_bytes,
-                               precision=self.precision, **self._plan_opts).create()
+                               precision=self.precision, stripped_grad=self.stripped_grad,
+                               **self._plan_opts).create()
             self._vjp_plans[key] = plan
         return plan
 
-    def vjp(self, tensors, cotangent, begin=0, step=1, count=None, wrt=None, max_bytes=None):
+    def vjp(self, tensors, cotangent, begin=0, step=1, count=None, wrt=None, max_bytes=None, exponent=None):
         """Gradients of the sum of slices ``begin, begin+step, ...`` (``count`` of them) for the
         output cotangent ``cotangent`` (the full output's shape): a list with one tensor per input,
         ``None`` for inputs outside ``wrt`` (default: all).  Complex gradients follow torch's
         convention.  Asynchronous on the current stream.  Gradients are linear in the cotangent and
         additive over slices, so one call per rank over ``rank_slices(...)`` followed by an
-        all-reduce gives the gradient of the whole tree.  ``max_bytes`` as for ``vjp_plan``."""
+        all-reduce gives the gradient of the whole tree.  ``max_bytes`` as for ``vjp_plan``.
+
+        With ``strip_exponent`` and ``stripped_grad``, ``cotangent`` is that of the mantissa ``m``
+        and ``exponent`` (a float or a one-element tensor) the ``e`` of the forward call over the
+        same slices that returned ``(m, e)``; the gradients are those of ``m`` with ``e`` held
+        constant."""
         torch = _torch()
         self._check_inputs(tensors)
         begin, step, count = self._check_slice_range(begin, step, count)
@@ -334,6 +346,11 @@ class TreeExecutor:
             ptrs, _keep = self._input_ptrs(tensors)
             if tuple(cotangent.shape) != tuple(plan.out_shape):
                 raise ValueError(f"cotangent has shape {tuple(cotangent.shape)}, the output {tuple(plan.out_shape)}")
+            exp = None
+            if plan.strip_exponent:
+                if exponent is None:
+                    raise ValueError("a stripped gradient needs the exponent of the forward call (exponent=)")
+                exp = torch.as_tensor(exponent, dtype=torch.float64).to(self.device).reshape(1).contiguous()
             cot = cotangent.to(device=self.device, dtype=tdt).contiguous()
             grads = [torch.zeros(tuple(t.shape), dtype=tdt, device=self.device) if i in plan.wrt else None
                      for i, t in enumerate(tensors)]
@@ -341,8 +358,10 @@ class TreeExecutor:
                 self._vjp_ws = None
                 self._vjp_ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
             ws = self._vjp_ws
+            # (only a stripped plan takes the forward's exponent)
+            extra = {} if exp is None else {"exp_ptr": exp.data_ptr()}
             plan.execute(ptrs, cot.data_ptr(), [g.data_ptr() if g is not None else None for g in grads],
-                         ws.data_ptr(), ws.numel(), begin, step, count, _stream_ptr())
+                         ws.data_ptr(), ws.numel(), begin, step, count, _stream_ptr(), **extra)
         return grads
 
     def _check_slice_range(self, begin, step, count):
@@ -431,13 +450,15 @@ class TreeExecutor:
 
 
 def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=None,
-                  slice_ids=None, vjp_max_bytes=None, precision="3xtf32", **plan_opts):
+                  slice_ids=None, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, **plan_opts):
     """``tree.contract(arrays)`` (cotengra/core.py:3943): takes the *unsliced*
     arrays, handles slicing, contraction and gathering, returns the output in
     ``tree.output`` order -- or ``(mantissa, exponent)`` with ``strip_exponent``.
     numpy in -> numpy out; torch CUDA in -> torch CUDA out.  ``vjp_max_bytes`` bounds the
     workspace of the backward pass (``TreeExecutor``); by default an executor's own bound.
-    ``precision`` as for ``TreeExecutor`` (an executor passed in keeps its own)."""
+    ``precision`` and ``stripped_grad`` as for ``TreeExecutor`` (an executor passed in keeps its
+    own): with ``stripped_grad`` a stripped result records the gradient of its mantissa, the
+    exponent (a float, as without it) held constant."""
     torch = _torch()
     if isinstance(tree, TreeExecutor):
         ex = tree
@@ -445,7 +466,7 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
         if dtype is None:
             dtype = dtype_name(arrays[0].dtype)
         ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, vjp_max_bytes=vjp_max_bytes,
-                          precision=precision, **plan_opts)
+                          precision=precision, stripped_grad=stripped_grad, **plan_opts)
     all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
     begin, step, count = (0, 1, None) if slice_ids is None else slice_ids
     if all_numpy:
@@ -455,25 +476,27 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
             return _finish_stripped(m, e, check_zero)
         return res
     tensors = [_to_device(a, ex.device)[0] for a in arrays]
-    if _records_grad(torch, arrays, ex.strip_exponent):
-        return _differentiable(torch, lambda ts: ex.contract_device(ts, begin, step, count),
-                               lambda ts, g, wrt: ex.vjp(ts, g, begin, step, count, wrt=wrt,
-                                                         max_bytes=vjp_max_bytes), tensors)
-    res = ex.contract_device(tensors, begin, step, count)
+    if _records_grad(torch, arrays, ex.strip_exponent, ex.stripped_grad):
+        res = _differentiable(torch, lambda ts: ex.contract_device(ts, begin, step, count),
+                              lambda ts, g, wrt, e=None: ex.vjp(ts, g, begin, step, count, wrt=wrt,
+                                                                max_bytes=vjp_max_bytes, exponent=e), tensors)
+    else:
+        res = ex.contract_device(tensors, begin, step, count)
     if ex.strip_exponent:
         m, e = res
         return _finish_stripped(m, float(e.item()), check_zero)
     return res
 
 
-def _records_grad(torch, arrays, strip_exponent):
+def _records_grad(torch, arrays, strip_exponent, stripped_grad=False):
     """Whether a call records a torch autograd node: torch tensor inputs, at least one requiring
-    grad, grad mode on.  ``strip_exponent`` results get no gradient (a warning says so)."""
+    grad, grad mode on.  ``strip_exponent`` results get no gradient (a warning says so) unless
+    ``stripped_grad`` asks for the mantissa's, with the exponent held constant."""
     if not torch.is_grad_enabled() or not arrays:
         return False
     if not all(isinstance(a, torch.Tensor) for a in arrays) or not any(a.requires_grad for a in arrays):
         return False
-    if strip_exponent:
+    if strip_exponent and not stripped_grad:
         warnings.warn("strip_exponent=True: no gradient is recorded for the (mantissa, exponent) result",
                       UserWarning, stacklevel=3)
         return False
@@ -485,7 +508,9 @@ _GRAD_FN = None
 
 def _differentiable(torch, run, vjp, tensors):
     """``run(tensors)`` as one torch autograd node whose backward is ``vjp(tensors, grad, wrt)``
-    (a ``VjpPlan`` on the device; ``wrt`` from ``ctx.needs_input_grad``)."""
+    (a ``VjpPlan`` on the device; ``wrt`` from ``ctx.needs_input_grad``).  A stripped ``run``
+    returns ``(m, e)``: ``e`` is not differentiable, and the backward is
+    ``vjp(tensors, grad_m, wrt, e)``."""
     global _GRAD_FN
     if _GRAD_FN is None:
         from torch.autograd.function import once_differentiable
@@ -494,14 +519,24 @@ def _differentiable(torch, run, vjp, tensors):
             @staticmethod
             def forward(ctx, run, vjp, *tensors):
                 ctx.vjp = vjp
-                ctx.save_for_backward(*tensors)
-                return run(list(tensors))
+                res = run(list(tensors))
+                ctx.stripped = isinstance(res, tuple)
+                if ctx.stripped:
+                    ctx.mark_non_differentiable(res[1])
+                    ctx.save_for_backward(*tensors, res[1])
+                else:
+                    ctx.save_for_backward(*tensors)
+                return res
 
             @staticmethod
             @once_differentiable
-            def backward(ctx, grad):
+            def backward(ctx, grad, *_grad_e):
                 wrt = [i for i, need in enumerate(ctx.needs_input_grad[2:]) if need]
-                grads = ctx.vjp(list(ctx.saved_tensors), grad, wrt)
+                saved = list(ctx.saved_tensors)
+                if ctx.stripped:
+                    grads = ctx.vjp(saved[:-1], grad, wrt, saved[-1])
+                else:
+                    grads = ctx.vjp(saved, grad, wrt)
                 return (None, None, *grads)
 
         _GRAD_FN = _Contract
@@ -666,14 +701,17 @@ class B200Contractor:
     """
 
     __slots__ = ("contractions", "strip_exponent", "check_zero", "implementation", "backend",
-                 "progbar", "vjp_max_bytes", "precision", "_plans", "__weakref__")
+                 "progbar", "vjp_max_bytes", "precision", "stripped_grad", "_plans", "__weakref__")
 
     def __init__(self, contractions, strip_exponent=False, check_zero=False,
-                 implementation="b200", backend=None, progbar=False, vjp_max_bytes=None, precision="3xtf32"):
+                 implementation="b200", backend=None, progbar=False, vjp_max_bytes=None, precision="3xtf32",
+                 stripped_grad=False):
         self.contractions = tuple(contractions)
         # compute mode of the float32 / complex64 tensor-core nodes (TreeExecutor); checked per dtype at call
         self.precision = check_precision(precision)
         self.vjp_max_bytes = vjp_max_bytes  # workspace bound of the backward pass (VjpPlan max_bytes)
+        # stripped results record the mantissa's gradient, the exponent held constant (TreeExecutor)
+        self.stripped_grad = bool(stripped_grad)
         self.strip_exponent = strip_exponent
         self.check_zero = check_zero
         self.implementation = implementation
@@ -696,7 +734,7 @@ class B200Contractor:
             inputs = [tuple((i, k) for k in range(len(s))) for i, s in enumerate(shapes)]
             size_dict = {(i, k): d for i, s in enumerate(shapes) for k, d in enumerate(s)}
             ex = _FlatExecutor(self.contractions, inputs, size_dict, dtype, strip, self.vjp_max_bytes,
-                               self.precision)
+                               self.precision, self.stripped_grad)
             self._plans[key] = ex
         return ex
 
@@ -717,9 +755,12 @@ class B200Contractor:
         with torch.cuda.device(tensors[0].device if tensors else torch.cuda.current_device()):
             ex = self._executor(tuple(tuple(t.shape) for t in tensors), dtype, strip)
             on_dev = [t.to(ex.device) for t in tensors]
-            if _records_grad(torch, arrays, strip):
-                return _differentiable(torch, ex.run, ex.vjp, on_dev)
-            res = ex.run(on_dev)
+            if _records_grad(torch, arrays, strip, self.stripped_grad):
+                res = _differentiable(torch, ex.run, ex.vjp, on_dev)
+                if not strip:
+                    return res
+            else:
+                res = ex.run(on_dev)
         if strip:
             m, e = res
             e = float(e.item())
@@ -733,7 +774,8 @@ class _FlatExecutor:
     """ExecPlan over explicit per-call arrays (no tree-level slicing): the output
     term is whatever the program produces."""
 
-    def __init__(self, contractions, inputs, size_dict, dtype, strip, vjp_max_bytes=None, precision="3xtf32"):
+    def __init__(self, contractions, inputs, size_dict, dtype, strip, vjp_max_bytes=None, precision="3xtf32",
+                 stripped_grad=False):
         torch = _torch()
         out_shape = _program_output_shape(contractions, [tuple(size_dict[ix] for ix in t) for t in inputs])
         output = tuple(("o", k) for k in range(len(out_shape)))
@@ -748,6 +790,7 @@ class _FlatExecutor:
         self._program = (contractions, inputs, output, sd)
         self._vjp_plans = {}
         self.vjp_max_bytes = vjp_max_bytes
+        self.stripped_grad = stripped_grad
 
     def run(self, tensors):
         torch = _torch()
@@ -759,8 +802,9 @@ class _FlatExecutor:
                               self.ws.numel(), 0, 1, 1, _stream_ptr())
         return (out, exp) if self.strip else out
 
-    def vjp(self, tensors, cotangent, wrt):
-        """Input gradients for ``cotangent`` (``None`` outside ``wrt``) through a ``VjpPlan``."""
+    def vjp(self, tensors, cotangent, wrt, exponent=None):
+        """Input gradients for ``cotangent`` (``None`` outside ``wrt``) through a ``VjpPlan``; a
+        stripped plan's for the mantissa, with the forward's ``exponent`` (a device tensor)."""
         from .vjp import VjpPlan
 
         torch = _torch()
@@ -770,15 +814,18 @@ class _FlatExecutor:
             if plan is None:
                 plan = self._vjp_plans[key] = VjpPlan(*self._program, (), dtype=self.plan.dtype, wrt=key,
                                                               max_bytes=self.vjp_max_bytes,
-                                                              precision=self.plan.precision).create()
+                                                              precision=self.plan.precision,
+                                                              strip_exponent=self.strip,
+                                                              stripped_grad=self.stripped_grad).create()
             cot = cotangent.to(device=self.device, dtype=self.tdt).contiguous()
             grads = [torch.zeros(tuple(t.shape), dtype=self.tdt, device=self.device) if i in plan.wrt else None
                      for i, t in enumerate(tensors)]
             ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
             srcs = [t.contiguous() for t in tensors]
+            extra = {} if exponent is None else {"exp_ptr": exponent.data_ptr()}
             plan.execute([t.data_ptr() for t in srcs], cot.data_ptr(),
                          [g.data_ptr() if g is not None else None for g in grads], ws.data_ptr(), ws.numel(),
-                         0, 1, 1, _stream_ptr())
+                         0, 1, 1, _stream_ptr(), **extra)
         return grads
 
 
@@ -810,23 +857,26 @@ def _program_output_shape(contractions, shapes):
 
 
 def make_contractor(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, precision="3xtf32",
-                    **_ignored):
+                    stripped_grad=False, **_ignored):
     """``cotengra.contract.make_contractor`` for ``implementation="b200"``
     (contract.py:925-1006): the per-slice callable for ``tree``."""
     return B200Contractor.from_tree(tree, strip_exponent=strip_exponent, check_zero=check_zero,
-                                    vjp_max_bytes=vjp_max_bytes, precision=precision)
+                                    vjp_max_bytes=vjp_max_bytes, precision=precision, stripped_grad=stripped_grad)
 
 
-def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, precision="3xtf32"):
+def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, precision="3xtf32",
+            stripped_grad=False):
     """Route ``tree.contract(...)`` / ``tree.contract_slice(...)`` of a live
     cotengra tree through this package's contractor by seeding its contractor cache
     (core.py:3699-3711).  Key order: ``(autojit, order, prefer_einsum,
     strip_exponent, check_zero, implementation, progbar)``.  Call after the tree
     is final: slicing/reconfiguration clears the cache (core.py:2040, 2087).  ``vjp_max_bytes``
     bounds the workspace of the backward pass of ``tree.contract`` on torch tensors; ``precision``
-    is the compute mode of its float32 / complex64 tensor-core nodes (``TreeExecutor``)."""
+    is the compute mode of its float32 / complex64 tensor-core nodes (``TreeExecutor``).
+    ``stripped_grad`` with ``strip_exponent``: each slice's ``(m_s, e_s)`` records the gradient of
+    ``m_s`` with ``e_s`` held constant, so that the reference's slice combiner backpropagates."""
     fn = make_contractor(tree, strip_exponent=strip_exponent, check_zero=check_zero,
-                         vjp_max_bytes=vjp_max_bytes, precision=precision)
+                         vjp_max_bytes=vjp_max_bytes, precision=precision, stripped_grad=stripped_grad)
     key = (False, None, False, bool(strip_exponent), check_zero, None, False)
     tree.contraction_cores[key] = fn
     return fn

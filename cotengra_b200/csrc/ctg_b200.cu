@@ -777,6 +777,8 @@ struct ctgb_plan {
     int64_t c_elems;  // dense elements of the result (strip_exponent)
     int measure_after = 0;  // strip_exponent: max|C| needs its own pass (split-K / block partial sums)
     int prescale_b = 0;     // strip_exponent: the small operand is copied, scaled by 1/(fA fB), first
+    int prescale_a = 0;     // stripped reverse mode: a single-operand node reads a copy of A scaled by 1/fA
+    int fa = -1, fb = -1;   // strip_exponent: the factor slots fA, fB it divides by (-1: 1.0)
   };
   std::vector<Tensor> tensors;
   std::vector<Node> nodes;
@@ -793,8 +795,10 @@ struct ctgb_plan {
   // strip_exponent scratch (device): [1] slice exponent, [2] invariant exponent
   double* d_scalars = nullptr;
   // fused strip_exponent: one factor slot per tensor (1.0 for inputs and single-operand results,
-  // max|C| for pairwise results) and the slots to reset / sum per pass
+  // max|C| for pairwise results) and the slots to reset / sum per pass; then slot n_tensors, the
+  // root's seed divisor of a stripped reverse-mode plan, and slot n_tensors + 1, a constant 1.0
   double* d_factors = nullptr;
+  bool scale_pending = false;   // stripped reverse mode: waits for ctgb_plan_set_scale_slots
   char* d_bscale = nullptr;     // scaled copy of the current node's small operand
   size_t bscale_bytes = 0;
   int* d_slot_lists = nullptr;  // [variant slots..., invariant slots...]
@@ -810,6 +814,57 @@ struct ctgb_plan {
   char* h_stage = nullptr;
   size_t h_stage_bytes = 0;
 };
+
+// Factor slots of a strip_exponent plan and the descriptor words that point into them.  A forward
+// plan divides every pairwise node by the factors of its own operands (slot_a = slot_b = null).  A
+// stripped reverse-mode plan names the slots node by node (ctgb_plan_set_scale_slots): its phase 0/1
+// nodes measure max|C| into their own slot as the forward does; a recomputed forward node (phase 2)
+// divides by the phase-1 factors of the values it recomputes and measures nothing, so that it forms
+// the same quotient as phase 1; a backward node divides by f_p and f_r (the seed at the root) and
+// measures nothing.
+static cudaError_t strip_setup(ctgb_plan* p, const int32_t* slot_a, const int32_t* slot_b) {
+  const size_t nt = p->tensors.size();
+  std::vector<double> ones(nt + 2, 1.0);
+  cudaError_t e = cudaMalloc((void**)&p->d_factors, (nt + 2) * sizeof(double));
+  if (e == cudaSuccess) e = cudaMemcpy(p->d_factors, ones.data(), (nt + 2) * sizeof(double), cudaMemcpyHostToDevice);
+  std::vector<int> var_slots, inv_slots;
+  for (size_t i = 0; i < p->nodes.size(); ++i) {
+    auto& n = p->nodes[i];
+    n.fa = slot_a ? slot_a[i] : n.a;
+    n.fb = slot_b ? slot_b[i] : n.b;
+    const bool measures = n.phase <= 1;
+    if (n.kind != 0) {
+      // (a reverse-mode plan whose root is a single-operand node: its adjoint reads the seeded cotangent)
+      n.prescale_a = slot_a != nullptr && n.fa >= 0;
+      if (n.prescale_a && (size_t)p->tensors[n.a].nbytes > p->bscale_bytes) p->bscale_bytes = (size_t)p->tensors[n.a].nbytes;
+      continue;
+    }
+    if (!measures) n.measure_after = 0;
+    int64_t* w = p->descs.data() + n.desc_off;
+    // small second operand (the usual case on a stem): scale a copy of it instead of every
+    // output element; otherwise the epilogue multiplies by 1/(fA fB)
+    const int64_t bbytes = p->tensors[n.b].nbytes;
+    n.prescale_b = bbytes > 0 && bbytes <= (16ll << 20) && p->tensors[n.b].kind != 3;
+    if (n.prescale_b) {
+      if ((size_t)bbytes > p->bscale_bytes) p->bscale_bytes = (size_t)bbytes;
+    } else {
+      w[W_SCALE_A] = (int64_t)(uintptr_t)(p->d_factors + n.fa);
+      w[W_SCALE_B] = (int64_t)(uintptr_t)(p->d_factors + n.fb);
+    }
+    w[W_FACTOR_C] = (n.measure_after || !measures) ? 0 : (int64_t)(uintptr_t)(p->d_factors + n.c);
+    if (measures) (n.phase == 0 ? inv_slots : var_slots).push_back(n.c);
+  }
+  p->n_var_slots = (int)var_slots.size();
+  p->n_inv_slots = (int)inv_slots.size();
+  var_slots.insert(var_slots.end(), inv_slots.begin(), inv_slots.end());
+  if (e == cudaSuccess && p->bscale_bytes) e = cudaMalloc((void**)&p->d_bscale, p->bscale_bytes + 256);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&p->d_slot_lists, (var_slots.size() + 1) * sizeof(int));
+  if (e == cudaSuccess && !var_slots.empty())
+    e = cudaMemcpy(p->d_slot_lists, var_slots.data(), var_slots.size() * sizeof(int), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = cudaMemcpy(p->d_descs, p->descs.data(), p->descs.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
+  return e;
+}
 
 extern "C" {
 
@@ -970,7 +1025,7 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     }
     if (n.phase == 1 || n.phase == 2) per_slice += 1 + q.measure_after + (pd->strip_exponent && n.kind == 0 ? 1 : 0);
   }
-  if (pd->strip_exponent && p->backward) return refuse("strip_exponent plans have no reverse mode");
+  p->scale_pending = pd->strip_exponent && p->backward;
   // kind 3 (the output) belongs to forward plans, kinds 4-6 (cotangent, gradients, H accumulators) to
   // reverse-mode ones: execute checks exactly the buffers the plan's kind needs
   p->grad_elems.assign(pd->n_inputs, 0);
@@ -1004,39 +1059,8 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     e = cudaMemcpy(p->d_descs, p->descs.data(), p->descs.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMalloc((void**)&p->d_scalars, 8 * sizeof(double));
   if (e == cudaSuccess) e = cudaMemset(p->d_scalars, 0, 8 * sizeof(double));
-  if (e == cudaSuccess && p->strip_exponent) {
-    // factor slots + the per-node pointers into them (patched into the plan's descriptors)
-    const size_t nt = p->tensors.size();
-    std::vector<double> ones(nt + 1, 1.0);
-    e = cudaMalloc((void**)&p->d_factors, (nt + 1) * sizeof(double));
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_factors, ones.data(), (nt + 1) * sizeof(double), cudaMemcpyHostToDevice);
-    std::vector<int> var_slots, inv_slots;
-    for (auto& n : p->nodes) {
-      if (n.kind != 0) continue;
-      int64_t* w = p->descs.data() + n.desc_off;
-      // small second operand (the usual case on a stem): scale a copy of it instead of every
-      // output element; otherwise the epilogue multiplies by 1/(fA fB)
-      const int64_t bbytes = p->tensors[n.b].nbytes;
-      n.prescale_b = bbytes > 0 && bbytes <= (16ll << 20) && p->tensors[n.b].kind != 3;
-      if (n.prescale_b) {
-        if ((size_t)bbytes > p->bscale_bytes) p->bscale_bytes = (size_t)bbytes;
-      } else {
-        w[W_SCALE_A] = (int64_t)(uintptr_t)(p->d_factors + n.a);
-        w[W_SCALE_B] = (int64_t)(uintptr_t)(p->d_factors + n.b);
-      }
-      w[W_FACTOR_C] = n.measure_after ? 0 : (int64_t)(uintptr_t)(p->d_factors + n.c);
-      (n.phase == 0 ? inv_slots : var_slots).push_back(n.c);
-    }
-    p->n_var_slots = (int)var_slots.size();
-    p->n_inv_slots = (int)inv_slots.size();
-    var_slots.insert(var_slots.end(), inv_slots.begin(), inv_slots.end());
-    if (e == cudaSuccess && p->bscale_bytes) e = cudaMalloc((void**)&p->d_bscale, p->bscale_bytes + 256);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&p->d_slot_lists, (var_slots.size() + 1) * sizeof(int));
-    if (e == cudaSuccess && !var_slots.empty())
-      e = cudaMemcpy(p->d_slot_lists, var_slots.data(), var_slots.size() * sizeof(int), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-      e = cudaMemcpy(p->d_descs, p->descs.data(), p->descs.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
-  }
+  // (a stripped reverse-mode plan gets its factor slots from ctgb_plan_set_scale_slots)
+  if (e == cudaSuccess && p->strip_exponent && !p->backward) e = strip_setup(p, nullptr, nullptr);
   if (e != cudaSuccess) {
     std::string msg = cudaGetErrorString(e);
     ctgb_plan_destroy(p);
@@ -1113,6 +1137,25 @@ int ctgb_plan_set_chunk_desc(ctgb_plan* p, const int64_t* desc) {
   return CTGB_OK;
 }
 
+int ctgb_plan_set_scale_slots(ctgb_plan* p, const int32_t* slot_a, const int32_t* slot_b, int n) {
+  if (!p || !slot_a || !slot_b) return fail(CTGB_E_VALUE, "null argument");
+  if (!p->scale_pending) return fail(CTGB_E_VALUE, "scale slots belong to stripped reverse-mode plans, once");
+  if (n != (int)p->nodes.size()) return fail(CTGB_E_VALUE, "node count mismatch");
+  const int seed = (int)p->tensors.size();
+  for (int i = 0; i < n; ++i) {
+    const bool pair = p->nodes[i].kind == 0;
+    if (slot_a[i] < (pair ? 0 : -1) || slot_a[i] > seed || slot_b[i] < (pair ? 0 : -1) || slot_b[i] > seed)
+      return fail(CTGB_E_VALUE, "scale slot out of range");
+  }
+  CUDA_TRY(strip_setup(p, slot_a, slot_b));
+  p->scale_pending = false;
+  int64_t per_slice = 3;  // reset slots, sum of logs, seed
+  for (const auto& q : p->nodes)
+    if (q.phase == 1 || q.phase == 2) per_slice += 1 + q.measure_after + q.prescale_b + q.prescale_a;
+  p->launches_per_slice = per_slice;
+  return CTGB_OK;
+}
+
 int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double* exponent_dev,
                       const void* cotangent, void* const* grads, void* workspace, size_t workspace_bytes,
                       int64_t slice_begin, int64_t slice_step, int64_t slice_count, void* stream) {
@@ -1120,9 +1163,12 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   if (workspace_bytes < (size_t)(p->workspace_bytes + p->persistent_bytes))
     return fail(CTGB_E_MEMORY, "workspace too small");
   if (!inputs) return fail(CTGB_E_VALUE, "null inputs");
-  if (p->strip_exponent && (!exponent_dev || p->chunk_desc.empty()))
+  if (p->strip_exponent && !p->backward && (!exponent_dev || p->chunk_desc.empty()))
     return fail(CTGB_E_VALUE, "strip_exponent needs an exponent buffer and a chunk descriptor");
-  if (p->strip_exponent && p->root < 0) return fail(CTGB_E_VALUE, "plan has no root node");
+  if (p->strip_exponent && !p->backward && p->root < 0) return fail(CTGB_E_VALUE, "plan has no root node");
+  // a stripped reverse-mode plan reads the exponent of the forward call it differentiates
+  if (p->strip_exponent && p->backward && (!exponent_dev || p->scale_pending))
+    return fail(CTGB_E_VALUE, "a stripped reverse-mode plan needs the forward's exponent and its scale slots");
   if ((p->backward || p->cot_offset >= 0) && !cotangent) return fail(CTGB_E_VALUE, "the plan needs a cotangent");
   for (int i = 0; i < p->n_inputs; ++i)
     if (p->grad_elems[i] > 0 && (!grads || !grads[i]))
@@ -1167,15 +1213,30 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
       char* B = n.kind == 0 ? resolve(n.b, out_off) : nullptr;
       char* C = resolve(n.c, out_off);
       if (n.zero_fill) CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)p->tensors[n.c].nbytes, st));
+      // the whole underlying buffer of an operand (a sliced input, or the cotangent's slice view,
+      // keeps its base offset into a copy)
+      auto under = [&](const ctgb_plan::Tensor& t) -> char* {
+        if (t.kind == 0) return (char*)inputs[t.input_index];
+        if (t.kind == 4) return (char*)mem.cot;
+        return (t.kind == 1 ? scratch : persistent) + t.offset;
+      };
       if (n.prescale_b) {
-        // the whole underlying buffer of the small operand (a sliced input keeps its base
-        // offset into the copy), scaled by 1/(fA fB) read from the factor slots on the device
+        // the small operand, scaled by 1/(fA fB) read from the factor slots on the device
         const ctgb_plan::Tensor& tb = p->tensors[n.b];
-        char* under = tb.kind == 0 ? (char*)inputs[tb.input_index] : (tb.kind == 1 ? scratch : persistent) + tb.offset;
-        if (int r = scale_copy(p->dtype, under, p->d_bscale, tb.nbytes / (int64_t)es, p->d_factors + n.a,
-                               p->d_factors + n.b, st))
+        char* base = under(tb);
+        if (int r = scale_copy(p->dtype, base, p->d_bscale, tb.nbytes / (int64_t)es, p->d_factors + n.fa,
+                               p->d_factors + n.fb, st))
           return r;
-        B = p->d_bscale + (B - under);
+        B = p->d_bscale + (B - base);
+      }
+      if (n.prescale_a) {
+        const ctgb_plan::Tensor& ta = p->tensors[n.a];
+        char* base = under(ta);
+        const double* one = p->d_factors + p->tensors.size() + 1;
+        if (int r = scale_copy(p->dtype, base, p->d_bscale, ta.nbytes / (int64_t)es, p->d_factors + n.fa,
+                               n.fb >= 0 ? p->d_factors + n.fb : one, st))
+          return r;
+        A = p->d_bscale + (A - base);
       }
       if (int r = launch_node(n.kind, h, d, A, B, C, st)) return r;
       // contract.py:816-829 strips after every *pairwise* node (single-operand preprocessing
@@ -1213,10 +1274,18 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
       g_launches.fetch_add(1, std::memory_order_relaxed);
     }
     if ((rc = run_phase(1, out_off))) return rc;
-    if ((rc = run_phase(2, out_off))) return rc;
     if (p->strip_exponent) {
       sum_log_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists, p->n_var_slots, d_slice_exp, d_inv_exp);
       g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    if (p->strip_exponent && p->backward) {
+      // the root is not run: d_slice_exp is the slice's exponent without the root's own factor, and
+      // the backward steps next to the root divide by the seed 10^(e - e'_s)
+      strip_seed_kernel<<<1, 1, 0, st>>>(p->d_factors + p->tensors.size(), exponent_dev, d_slice_exp);
+      g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    if ((rc = run_phase(2, out_off))) return rc;
+    if (p->strip_exponent && !p->backward) {
       // the root wrote a dense mantissa into its workspace slot; fold it into the
       // output against the running exponent (core.py:163-170, 3856-3861)
       const ctgb_plan::Node& root = p->nodes[p->root];

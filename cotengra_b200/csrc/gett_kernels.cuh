@@ -840,6 +840,21 @@ __global__ void sum_log_kernel(const double* __restrict__ f, const int* __restri
     *exponent = t;
   }
 }
+// stripped reverse mode, once per slice after its forward phase: the divisor 10^(e - e'_s) that
+// turns the conjugated cotangent of the mantissa m = amp 10^-e into that of the slice's raw root
+// product (e: the forward call's exponent, e'_s: the slice's exponent without the root's factor).
+// 0 (the nodes' "scale 0" rule) when the slice or the whole result is zero, so that the seed is
+// zero rather than NaN; NaN when either exponent is.
+__global__ void strip_seed_kernel(double* __restrict__ seed, const double* __restrict__ e,
+                                  const double* __restrict__ es) {
+  const double E = *e, s = *es;
+  if (E != E || s != s)
+    *seed = __longlong_as_double(0x7ff8000000000000LL);
+  else if (E == -CUDART_INF || s == -CUDART_INF)
+    *seed = 0.0;
+  else
+    *seed = pow(10.0, E - s);
+}
 __global__ void set_double_kernel(double* p, double v) { *p = v; }
 
 // in-place complex conjugate (VJP plans: the incoming cotangent's copy and the finished input gradients)

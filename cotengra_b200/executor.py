@@ -200,6 +200,8 @@ class _DevicePlan:
     handle = None
     strip_exponent = False
     cotangent_offset = -1
+    _chunk_words = None  # strip_exponent forward plans: ctgb_plan_set_chunk_desc
+    scale_slots = None   # stripped reverse-mode plans: ctgb_plan_set_scale_slots, ([slot_a], [slot_b])
 
     def _marshal(self):
         keep = self._keep = []
@@ -260,15 +262,30 @@ class _DevicePlan:
         h = C.c_void_p()
         _lib.check(lib.ctgb_plan_create(C.byref(self._pd), C.byref(h)))
         self.handle = h
-        if self.strip_exponent:
+        if self._chunk_words is not None:
             w = self._chunk_words
             _lib.check(lib.ctgb_plan_set_chunk_desc(h, w.ctypes.data_as(C.c_void_p)))
+        if self.scale_slots is not None:
+            n = len(self.nodes)
+            sa, sb = ((C.c_int32 * max(n, 1))(*s) for s in self.scale_slots)
+            _lib.check(lib.ctgb_plan_set_scale_slots(h, sa, sb, n))
         return self
 
     def destroy(self):
         if self.handle is not None:
             _lib.load().ctgb_plan_destroy(self.handle)
             self.handle = None
+
+    def launches_per_slice(self):
+        return int(_lib.load().ctgb_plan_launches_per_slice(self.handle))
+
+    def strip_modes(self):
+        """strip_exponent plans: ``(prescale_b, measure_after)`` of every node of ``self.nodes``
+        (ctgb_plan_strip_modes; prescale_b is -1 for single-operand nodes)."""
+        n = len(self.nodes)
+        pre, after = (C.c_int32 * n)(), (C.c_int32 * n)()
+        _lib.check(_lib.load().ctgb_plan_strip_modes(self.handle, pre, after, n))
+        return [(int(a), int(b)) for a, b in zip(pre, after)]
 
     def __del__(self):
         try:
@@ -493,14 +510,3 @@ class ExecPlan(_DevicePlan):
         ms = (C.c_float * n)()
         _lib.check(_lib.load().ctgb_plan_profile_read(self.handle, ms, n))
         return [float(x) for x in ms]
-
-    def launches_per_slice(self):
-        return int(_lib.load().ctgb_plan_launches_per_slice(self.handle))
-
-    def strip_modes(self):
-        """strip_exponent plans: ``(prescale_b, measure_after)`` of every node of ``self.nodes``
-        (ctgb_plan_strip_modes; prescale_b is -1 for single-operand nodes)."""
-        n = len(self.nodes)
-        pre, after = (C.c_int32 * n)(), (C.c_int32 * n)()
-        _lib.check(_lib.load().ctgb_plan_strip_modes(self.handle, pre, after, n))
-        return [(int(a), int(b)) for a, b in zip(pre, after)]

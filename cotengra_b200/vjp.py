@@ -36,6 +36,22 @@ descriptor) with phase 2 and a fresh scratch slot, emitted right before the firs
 that reads the value and kept until its last read.  A dropped value whose operands were dropped
 recomputes them first, from the nearest kept values.  Which values to drop is a greedy search on
 the arena size ``executor.layout`` reports (see ``VjpPlan._fit``).
+
+With ``strip_exponent`` and ``stripped_grad`` the plan differentiates the mantissa ``m`` of a
+stripped result ``(m, e)``, ``amp = m 10^e``, with the exponent held constant:
+``dm/dx = 10^-e damp/dx``.  The forward nodes keep the forward plan's lazy scheme: a pairwise
+value is stored raw, ``S_p = (S_l/f_l)(S_r/f_r)``, and records ``f_p = max|S_p|``; every non-root
+pairwise node runs in phase 0 or 1 so that the slice exponent without the root's factor, ``e'_s``,
+is complete before phase 2.  The plan propagates ``H~ = conj(dm/dp~)`` of the normalised values
+``p~ = S_p/f_p``:
+
+    seed        H~_root = conj(g_m)[slice view] * 10^(e'_s - e)      (the divisor 10^(e - e'_s))
+    pairwise    H~_l = contract(H~_p, S_r) / (f_p f_r)               (f_p: the seed at the root)
+    single      H~_x = adjoint(H~_c)                                 (factor 1; seeded at the root)
+
+Inputs have factor 1, so ``H~_x`` is ``conj(dm/dx)``.  A recomputed value divides by the phase-1
+factors of its operands and records none, so it is the quotient phase 1 formed.  A slice with a
+zero factor, or a zero result (``e = -inf``), contributes zero; a NaN exponent gives NaN.
 """
 
 from __future__ import annotations
@@ -161,16 +177,22 @@ class VjpPlan(_DevicePlan):
     without recomputation.  A budget below the smallest the planner reaches raises
     ``MemoryError``.  ``recompute_macs`` are the MACs of the phase-2 forward nodes of one slice;
     ``min_bytes`` is the smallest budget the planner reached (``total_bytes`` without a budget).
-    ``precision`` applies to the forward, recomputed and backward nodes alike."""
+    ``precision`` applies to the forward, recomputed and backward nodes alike.
+
+    ``strip_exponent=True`` needs ``stripped_grad=True``: the plan then differentiates the mantissa
+    of a stripped result with its exponent held constant (see the module notes), and ``execute``
+    takes the forward's exponent.  Without ``stripped_grad`` it raises ``NotImplementedError``."""
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  wrt=None, strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None, max_bytes=None, precision="3xtf32"):
+                 variant=None, max_bytes=None, precision="3xtf32", stripped_grad=False):
         if max_bytes is not None and (isinstance(max_bytes, bool) or not isinstance(max_bytes, numbers.Integral)
                                       or max_bytes <= 0):
             raise ValueError(f"max_bytes must be a positive integer, got {max_bytes!r}")
-        if strip_exponent:
-            raise NotImplementedError("gradients of strip_exponent results are not supported")
+        if strip_exponent and not stripped_grad:
+            raise NotImplementedError("gradients of strip_exponent results are only defined with "
+                                      "stripped_grad=True (the exponent held constant)")
+        self.strip_exponent = bool(strip_exponent)
         fwd = ExecPlan(contractions, inputs, output, size_dict, sliced, dtype=dtype, hoist=hoist,
                        allow_dmma=allow_dmma, sm_count=sm_count, precision=precision)
         self.fwd = fwd
@@ -212,12 +234,13 @@ class VjpPlan(_DevicePlan):
             needs[id(nd["c"])] = any(needs[id(t)] for t, _ in opl)
         need = lambda t: needs.get(id(t), False)  # noqa: E731
 
-        # which forward values are read (by a backward step or a forward node that runs)
+        # which forward values are read (by a backward step or a forward node that runs); stripped,
+        # every non-root node runs, because e'_s needs every factor
         n_nodes = len(nodes)
         value, runs = set(), [False] * n_nodes
         for i in range(n_nodes - 1, -1, -1):
             nd, (opl, _to) = nodes[i], ops[i]
-            if i < n_nodes - 1 and id(nd["c"]) in value:
+            if i < n_nodes - 1 and (id(nd["c"]) in value or self.strip_exponent):
                 runs[i] = True
                 value.update(id(t) for t, _ in opl)
             if need(nd["c"]) and len(opl) == 2:
@@ -271,6 +294,8 @@ class VjpPlan(_DevicePlan):
                            zero_fill=False, fwd_index=i)
                 if nd["kind"] == 0:
                     rec["plan"] = nd["plan"]
+                    if self.strip_exponent:
+                        rec["scale"] = (a, b)  # (kept by a recomputation: the phase-1 factors)
                 fwd_nodes[ph].append(rec)
 
         bwd_nodes = {PHASE_VAR_BWD: [], PHASE_INV_BWD: []}
@@ -297,9 +322,14 @@ class VjpPlan(_DevicePlan):
                 diag = _is_diagonal(tx, X.shape)
                 acc = HX.kind in (K_GRAD, K_HACC) or diag
                 words = build_single_desc(odims, [], dtype, accumulate=acc)
-                bwd_nodes[ph].append(dict(kind=1, a=Hc, b=None, c=HX, words=words, phase=ph,
-                                          zero_fill=diag and HX.kind == K_SCRATCH, fwd_index=i))
+                rec = dict(kind=1, a=Hc, b=None, c=HX, words=words, phase=ph,
+                           zero_fill=diag and HX.kind == K_SCRATCH, fwd_index=i)
+                if self.strip_exponent and i == n_nodes - 1:
+                    rec["scale"] = (None,)  # None: the root's seed
+                bwd_nodes[ph].append(rec)
                 continue
+            # stripped: H~_p divides by f_p (the seed at the root), the value read by its factor
+            hp_factor = None if i == n_nodes - 1 else vals.get(id(nd["c"]))
             n_h = 0
             for (X, tx), (Y, ty) in ((opl[0], opl[1]), (opl[1], opl[0])):
                 if not need(X):
@@ -317,8 +347,11 @@ class VjpPlan(_DevicePlan):
                                        allow_dmma=allow_dmma, c_dense_elems=dense, variant=v,
                                        precision=self.precision)
                 a, b = (Yv, Hc) if plan.swapped else (Hc, Yv)
-                bwd_nodes[ph].append(dict(kind=0, a=a, b=b, c=HX, words=plan.words, phase=ph,
-                                          zero_fill=diag and HX.kind == K_SCRATCH, plan=plan, fwd_index=i))
+                rec = dict(kind=0, a=a, b=b, c=HX, words=plan.words, phase=ph,
+                           zero_fill=diag and HX.kind == K_SCRATCH, plan=plan, fwd_index=i)
+                if self.strip_exponent:
+                    rec["scale"] = (Yv, hp_factor) if plan.swapped else (hp_factor, Yv)
+                bwd_nodes[ph].append(rec)
                 n_h += 1
             if n_h:
                 Bn, M, N, K = nd["plan"].sizes
@@ -338,6 +371,13 @@ class VjpPlan(_DevicePlan):
         self.nodes = [nd for nd in sched if nd is not None]
         self.tensors = _slots(sched)
         self.workspace_bytes, self.persistent_bytes, self.cotangent_offset = sizes
+        if self.strip_exponent:
+            # factor slot of every operand a node divides by: a tensor slot, or the seed (n_tensors)
+            slot = {id(t): i for i, t in enumerate(self.tensors)}
+            seed = len(self.tensors)
+            scale = [nd.get("scale", ()) for nd in self.nodes]
+            self.scale_slots = tuple([-1 if len(s) <= k else seed if s[k] is None else slot[id(s[k])] for s in scale]
+                                     for k in (0, 1))
         self._marshal()
 
     # ------------------------------------------------------------------ recomputation
@@ -367,11 +407,11 @@ class VjpPlan(_DevicePlan):
         head, tail = fwd_nodes[PHASE_INV_FWD] + [None], bwd_nodes[PHASE_INV_BWD]
 
         def schedule(dropped):
-            # phase 1 forms the kept values and what they are formed from
+            # phase 1 forms the kept values and what they are formed from (stripped: every factor)
             kept = saved.keys() - dropped
             want, run1 = set(kept), []
             for rec in reversed(var_fwd):
-                if id(rec["c"]) in want:
+                if id(rec["c"]) in want or self.strip_exponent:
                     run1.append(rec)
                     want.update(id(s) for s in (rec["a"], rec["b"]) if s is not None)
             run1.reverse()
@@ -445,9 +485,11 @@ class VjpPlan(_DevicePlan):
         return [int(nd["words"][32]) for nd in self.nodes if nd["kind"] == 0 and nd["phase"] in phases]
 
     # ------------------------------------------------------------------ device side
-    def execute(self, input_ptrs, cot_ptr, grad_ptrs, ws_ptr, ws_bytes, begin, step, count, stream=0):
+    def execute(self, input_ptrs, cot_ptr, grad_ptrs, ws_ptr, ws_bytes, begin, step, count, stream=0,
+                exp_ptr=None):
+        """``exp_ptr``: stripped plans, the device double holding the forward's exponent."""
         lib = _lib.load()
         arr = (C.c_void_p * len(input_ptrs))(*input_ptrs)
         grads = (C.c_void_p * len(grad_ptrs))(*grad_ptrs)
-        _lib.check(lib.ctgb_plan_execute(self.handle, arr, None, None, cot_ptr, grads, ws_ptr, ws_bytes, int(begin),
-                                         int(step), int(count), stream))
+        _lib.check(lib.ctgb_plan_execute(self.handle, arr, None, exp_ptr, cot_ptr, grads, ws_ptr, ws_bytes,
+                                         int(begin), int(step), int(count), stream))

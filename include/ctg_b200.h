@@ -152,18 +152,33 @@ typedef struct {
   int64_t out_elements;       /* elements of the full output (or cotangent)  */
   int64_t workspace_bytes;    /* per-slice arena                              */
   int64_t persistent_bytes;   /* arena kept over the whole call               */
-  int32_t strip_exponent;     /* contract.py:816-829 semantics; forward only  */
+  int32_t strip_exponent;     /* contract.py:816-829 semantics (reverse mode:
+                                 ctgb_plan_set_scale_slots)                   */
   int64_t cotangent_offset;   /* complex reverse-mode plans: byte offset of the
                                  conjugated cotangent copy in the persistent
                                  arena; -1 = no copy                          */
 } ctgb_plan_desc;
 
-/* Refuses strip_exponent together with phase 2/3 nodes (CTGB_E_VALUE). */
+/* strip_exponent together with phase 2/3 nodes makes a stripped reverse-mode
+ * plan, which runs only after ctgb_plan_set_scale_slots. */
 int ctgb_plan_create(const ctgb_plan_desc* desc, ctgb_plan** plan);
 /* strip_exponent only: the single-operand descriptor (ctgb_single_desc_words()
  * words) that maps the dense root result of one slice onto its chunk of the
  * output tensor (identity layout when no sliced index is an output index). */
 int ctgb_plan_set_chunk_desc(ctgb_plan* plan, const int64_t* desc);
+/* Stripped reverse-mode plans, once before the first execute: the factor slots
+ * each of the n (= n_nodes) nodes divides its product by, in desc->nodes order.
+ * A slot is a tensor slot index, whose factor is max|value| for a pairwise
+ * result formed in phase 0 or 1 and 1.0 otherwise, or n_tensors: the root's
+ * seed 10^(e - e'_s), formed per slice after phase 1 from the forward's exponent
+ * e and the slice's exponent e'_s without the root's factor.  A pairwise node
+ * divides by slot_a[i] * slot_b[i] (its descriptor's A and B operands); a
+ * single-operand node by slot_a[i] * slot_b[i] when slot_a[i] >= 0, a missing
+ * slot_b (-1) counting as 1.0, and not at all when slot_a[i] is -1.  Phase 0/1
+ * pairwise nodes record max|C| in slot c as in a forward plan; phase 2/3 nodes
+ * record nothing.  The gradient is that of m = amp * 10^-e with e held constant. */
+int ctgb_plan_set_scale_slots(ctgb_plan* plan, const int32_t* slot_a,
+                              const int32_t* slot_b, int n);
 void ctgb_plan_destroy(ctgb_plan* plan);
 size_t ctgb_plan_workspace_bytes(const ctgb_plan* plan);
 int64_t ctgb_plan_launches_per_slice(const ctgb_plan* plan);
@@ -192,7 +207,9 @@ int ctgb_plan_strip_modes(const ctgb_plan* plan, int32_t* prescale_b, int32_t* m
  * differentiated; the caller zeroes the buffers (the final conjugation of
  * complex gradients acts on the whole buffer), and on return they hold the
  * finished gradients in torch's convention (grad_x = sum over outputs of
- * grad_out * conj(d out / d x)).  `out` and `exponent_dev` may be null.
+ * grad_out * conj(d out / d x)).  `out` may be null, and so may `exponent_dev`
+ * except for a stripped plan, which reads from it the exponent e of the forward
+ * result (m, e) whose mantissa's cotangent `cotangent` is.
  *
  * Order: conjugated cotangent copy; phase 0; H accumulators zeroed; per slice
  * phases 1 and 2 (and the stripped accumulation); phase 3; conjugated

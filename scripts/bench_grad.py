@@ -2,7 +2,7 @@
 tree under torch GPU autograd.  Prints one JSON line with the card name and power limit.
 
     python scripts/bench_grad.py --config peps8x8 --dtype complex64 [--steps 10 --warmup 3]
-                                 [--slices-per-gpu 2] [--no-fuse] [--vjp-max-gib 56]
+                                 [--slices-per-gpu 2] [--no-fuse] [--vjp-max-gib 56] [--strip]
 
 Gradient TFLOP/s are quoted on the VJP work: the recomputed forward (root excluded) plus, for each
 differentiated pairwise node, its MACs times the number of H it forms (8 flops per complex
@@ -109,6 +109,23 @@ def run_grad(args):
                    for g, w in zip(grads, tgrads))
         line.update({"torch_autograd_s": t_torch, "speedup_vs_torch_autograd": t_torch / t_both,
                      "max_rel_grad_diff_vs_torch": diff})
+    if args.strip:
+        # the same VJP of the stripped mantissa (stripped_grad): one seed kernel per slice and scaled
+        # epilogues / pre-scaled operands on top of the unstripped plan; timed after it, alone
+        del grads
+        ex._ws = ex._vjp_ws = None
+        torch.cuda.empty_cache()
+        exs = cb.TreeExecutor(spec, dtype=args.dtype, fuse=not args.no_fuse, strip_exponent=True,
+                              stripped_grad=True)
+        _m, e = exs.contract_device(dev, 0, 1, count)
+        splan = exs.vjp_plan(max_bytes=budget)
+        exs._ws = None
+        torch.cuda.empty_cache()
+        t_svjp, _g = timed(lambda: exs.vjp(dev, cot, 0, 1, count, max_bytes=budget, exponent=e))
+        line.update({"strip_vjp_s": t_svjp, "strip_over_unstripped_vjp": t_svjp / t_vjp,
+                     "strip_vjp_workspace_bytes": splan.total_bytes,
+                     "strip_launches_per_slice": splan.launches_per_slice(),
+                     "launches_per_slice": plan.launches_per_slice()})
     print(json.dumps(line))
 
 
@@ -122,6 +139,8 @@ def main():
     ap.add_argument("--no-fuse", action="store_true", help="differentiate the reference's node sequence one to one")
     ap.add_argument("--vjp-max-gib", type=float, default=None,
                     help="workspace budget of the VJP plan in GiB (per-slice values are recomputed to meet it)")
+    ap.add_argument("--strip", action="store_true",
+                    help="also time the VJP of the strip_exponent mantissa (stripped_grad=True)")
     run_grad(ap.parse_args())
 
 
