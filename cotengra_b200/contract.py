@@ -54,9 +54,6 @@ def _torch():
     return torch
 
 
-_NP2T = {"float32": "float32", "float64": "float64", "complex64": "complex64", "complex128": "complex128"}
-
-
 def _to_device(x, device=None):
     """numpy / torch -> contiguous torch CUDA tensor; returns (tensor, was_numpy)."""
     torch = _torch()
@@ -179,72 +176,45 @@ def implementation(precision="3xtf32"):
 # ---------------------------------------------------------------------------
 
 
-class TreeExecutor:
-    """A compiled sliced contraction: ``ContractionTree.contract`` on the GPU.
+class _Executor:
+    """A compiled program ``(contractions, inputs, output, size_dict, sliced)`` on one device: its
+    forward ``ExecPlan`` (``plan``), the workspaces, and the forward and reverse-mode entry points over
+    a range of its slices.  Every option of a contraction lives here, and every entry point forwards
+    its options to the executor it builds:
 
-    Built from a ``TreeSpec`` or from a live cotengra tree (captured through
-    ``TreeSpec.from_cotengra``).  The slice loop, the node loop, the slice
-    accumulation and (optionally) exponent stripping all run inside
-    ``ctgb_plan_execute``.
-
-    ``vjp_max_bytes`` bounds the workspace of its reverse-mode plans (``vjp_plan``, ``vjp``), which
-    then recompute per-slice forward values instead of keeping them (``VjpPlan(max_bytes=...)``).
+    ``strip_exponent`` returns results as ``(mantissa, exponent)``.
 
     ``precision`` is the compute mode of the float32 / complex64 tensor-core nodes of every plan it
     builds (forward, output chunks, reverse mode): ``"3xtf32"`` (default) or ``"tf32"``.
 
+    ``vjp_max_bytes`` bounds the workspace of its reverse-mode plans (``vjp_plan``, ``vjp``), which
+    then recompute per-slice forward values instead of keeping them (``VjpPlan(max_bytes=...)``).
+
     ``stripped_grad=True`` (with ``strip_exponent``) differentiates the mantissa ``m`` of a result
     ``(m, e)`` with the exponent held constant, ``dm/dx = 10^-e damp/dx``: exact for every loss that
     depends on the result only through ``m 10^e``.  ``vjp`` then takes the forward's ``exponent``.
+
+    ``plan_opts`` go to the forward and reverse-mode plans (``ExecPlan`` / ``VjpPlan`` keywords).
     """
 
-    def __init__(self, tree, dtype="complex128", strip_exponent=False, device=None,
-                 contractions=None, fuse=True, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False,
-                 **plan_opts):
-        check_precision(precision, dtype)
-        self.spec = tree if isinstance(tree, TreeSpec) else TreeSpec.from_cotengra(tree)
-        # stem fusion (fusion.py): an execution-plan transformation of the tree cotengra found --
-        # big stem tensors absorb pre-contracted groups of small tensors in one pass.  ``spec``
-        # stays the caller's tree; ``exec_spec`` is what runs.  ``fuse=False`` executes the
-        # reference's own node sequence one to one.
-        self.exec_spec, self.fusion = self.spec, {"changed": False}
-        if fuse and contractions is None:
-            from .fusion import fuse_stems
-
-            # (``fuse`` may be a dict of planner options -- min_big, ratio, min_gain, model -- e.g. to
-            # force fusion on small trees in tests)
-            opts = fuse if isinstance(fuse, dict) else {}
-            self.exec_spec, self.fusion = fuse_stems(self.spec, dtype_name(dtype), **opts)
-        ir = self.exec_spec.contractions() if contractions is None else contractions
+    def __init__(self, contractions, inputs, output, size_dict, sliced, dtype, strip_exponent=False, device=None,
+                 vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, **plan_opts):
         torch = _torch()
+        self._ir, self._plan_opts = contractions, plan_opts
+        # the program without its slicing: the positional head of ``ExecPlan`` and ``VjpPlan``
+        self._program, self._sliced = (contractions, inputs, output, size_dict), sliced
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
         with torch.cuda.device(self.device):
-            self.plan = ExecPlan(ir, self.spec.inputs, self.spec.output, self.spec.size_dict,
-                                 self.spec.sliced, dtype=dtype, strip_exponent=strip_exponent,
+            self.plan = ExecPlan(*self._program, sliced, dtype=dtype, strip_exponent=strip_exponent,
                                  precision=precision, **plan_opts).create()
         self.dtype = self.plan.dtype
         self.precision = precision
         self.strip_exponent = bool(strip_exponent)
         self.stripped_grad = bool(stripped_grad)
-        self._ws = None
-        self._ref_work = None
-        self._ir, self._plan_opts = ir, plan_opts
-        self._vjp_plans, self._vjp_ws = {}, None
         self.vjp_max_bytes = vjp_max_bytes
-
-    @property
-    def reference_work(self):
-        """``(macs_per_slice, macs_invariant, elements_per_slice)`` of the caller's (unfused)
-        tree -- the algorithmic work throughput figures are quoted on."""
-        if self._ref_work is None:
-            if self.fusion.get("changed"):
-                from .fusion import tree_work
-
-                self._ref_work = tree_work(self.spec)
-            else:
-                self._ref_work = (self.plan.macs_per_slice, self.plan.macs_invariant,
-                                  self.plan.elements_per_slice)
-        return self._ref_work
+        self._shapes = [tuple(size_dict[ix] for ix in term) for term in inputs]
+        self._ws = None
+        self._vjp_plans, self._vjp_ws = {}, None
 
     @property
     def nslices(self):
@@ -259,7 +229,7 @@ class TreeExecutor:
         return self._ws
 
     def _check_inputs(self, arrays):
-        shapes = self.spec.shapes()
+        shapes = self._shapes
         if len(arrays) != len(shapes):
             raise ValueError(f"expected {len(shapes)} arrays, got {len(arrays)}")
         for i, (x, s) in enumerate(zip(arrays, shapes)):
@@ -273,7 +243,7 @@ class TreeExecutor:
         torch = _torch()
         self._check_inputs(tensors)
         begin, step, count = self._check_slice_range(begin, step, count)
-        tdt = getattr(torch, _NP2T[self.dtype])
+        tdt = getattr(torch, self.dtype)
         with torch.cuda.device(self.device):
             if out is None:
                 out = torch.zeros(self.plan.out_shape, dtype=tdt, device=self.device)
@@ -309,19 +279,16 @@ class TreeExecutor:
         within ``max_bytes`` of workspace (default: the executor's ``vjp_max_bytes``)."""
         from .vjp import VjpPlan
 
-        n = len(self.spec.inputs)
-        wrt = tuple(range(n)) if wrt is None else tuple(sorted({int(i) for i in wrt}))
+        wrt = tuple(range(len(self._shapes))) if wrt is None else tuple(sorted({int(i) for i in wrt}))
         max_bytes = self.vjp_max_bytes if max_bytes is None else max_bytes
         key = wrt if max_bytes is None else (wrt, max_bytes)
         plan = self._vjp_plans.get(key)
         if plan is None:
             torch = _torch()
             with torch.cuda.device(self.device):
-                plan = VjpPlan(self._ir, self.spec.inputs, self.spec.output, self.spec.size_dict,
-                               self.spec.sliced, dtype=self.dtype, wrt=wrt,
-                               strip_exponent=self.strip_exponent, max_bytes=max_bytes,
-                               precision=self.precision, stripped_grad=self.stripped_grad,
-                               **self._plan_opts).create()
+                plan = VjpPlan(*self._program, self._sliced, dtype=self.dtype, wrt=wrt,
+                               strip_exponent=self.strip_exponent, max_bytes=max_bytes, precision=self.precision,
+                               stripped_grad=self.stripped_grad, **self._plan_opts).create()
             self._vjp_plans[key] = plan
         return plan
 
@@ -341,7 +308,7 @@ class TreeExecutor:
         self._check_inputs(tensors)
         begin, step, count = self._check_slice_range(begin, step, count)
         plan = self.vjp_plan(wrt, max_bytes)
-        tdt = getattr(torch, _NP2T[self.dtype])
+        tdt = getattr(torch, self.dtype)
         with torch.cuda.device(self.device):
             ptrs, _keep = self._input_ptrs(tensors)
             if tuple(cotangent.shape) != tuple(plan.out_shape):
@@ -394,6 +361,53 @@ class TreeExecutor:
                                        _stream_ptr())
         return (out, e) if self.strip_exponent else out
 
+
+class TreeExecutor(_Executor):
+    """A compiled sliced contraction: ``ContractionTree.contract`` on the GPU.
+
+    Built from a ``TreeSpec`` or from a live cotengra tree (captured through
+    ``TreeSpec.from_cotengra``).  The slice loop, the node loop, the slice
+    accumulation and (optionally) exponent stripping all run inside
+    ``ctgb_plan_execute``.  The options are those of ``_Executor``.
+    """
+
+    def __init__(self, tree, dtype="complex128", strip_exponent=False, device=None,
+                 contractions=None, fuse=True, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False,
+                 **plan_opts):
+        check_precision(precision, dtype)
+        self.spec = spec = tree if isinstance(tree, TreeSpec) else TreeSpec.from_cotengra(tree)
+        # stem fusion (fusion.py): an execution-plan transformation of the tree cotengra found --
+        # big stem tensors absorb pre-contracted groups of small tensors in one pass.  ``spec``
+        # stays the caller's tree; ``exec_spec`` is what runs.  ``fuse=False`` executes the
+        # reference's own node sequence one to one.
+        self.exec_spec, self.fusion = spec, {"changed": False}
+        if fuse and contractions is None:
+            from .fusion import fuse_stems
+
+            # (``fuse`` may be a dict of planner options -- min_big, ratio, min_gain, model -- e.g. to
+            # force fusion on small trees in tests)
+            opts = fuse if isinstance(fuse, dict) else {}
+            self.exec_spec, self.fusion = fuse_stems(spec, dtype_name(dtype), **opts)
+        ir = self.exec_spec.contractions() if contractions is None else contractions
+        super().__init__(ir, spec.inputs, spec.output, spec.size_dict, spec.sliced, dtype,
+                         strip_exponent=strip_exponent, device=device, vjp_max_bytes=vjp_max_bytes,
+                         precision=precision, stripped_grad=stripped_grad, **plan_opts)
+        self._ref_work = None
+
+    @property
+    def reference_work(self):
+        """``(macs_per_slice, macs_invariant, elements_per_slice)`` of the caller's (unfused)
+        tree -- the algorithmic work throughput figures are quoted on."""
+        if self._ref_work is None:
+            if self.fusion.get("changed"):
+                from .fusion import tree_work
+
+                self._ref_work = tree_work(self.spec)
+            else:
+                self._ref_work = (self.plan.macs_per_slice, self.plan.macs_invariant,
+                                  self.plan.elements_per_slice)
+        return self._ref_work
+
     def __call__(self, arrays, **kw):
         return contract_tree(self, arrays, **kw)
 
@@ -428,8 +442,10 @@ class TreeExecutor:
         all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
         tensors = [_to_device(a, self.device)[0] for a in arrays]
         ptrs = [t.data_ptr() for t in tensors]
-        tdt = getattr(torch, _NP2T[self.dtype])
+        tdt = getattr(torch, self.dtype)
         need = plan.total_bytes
+        # a buffer of its own, not ``_ws``: the generator yields between launches, and a
+        # ``contract_device`` call in between must not overwrite the arena of a pending chunk
         with torch.cuda.device(self.device):
             ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
         for o in range(nchunks):
@@ -454,38 +470,46 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
     """``tree.contract(arrays)`` (cotengra/core.py:3943): takes the *unsliced*
     arrays, handles slicing, contraction and gathering, returns the output in
     ``tree.output`` order -- or ``(mantissa, exponent)`` with ``strip_exponent``.
-    numpy in -> numpy out; torch CUDA in -> torch CUDA out.  ``vjp_max_bytes`` bounds the
-    workspace of the backward pass (``TreeExecutor``); by default an executor's own bound.
-    ``precision`` and ``stripped_grad`` as for ``TreeExecutor`` (an executor passed in keeps its
-    own): with ``stripped_grad`` a stripped result records the gradient of its mantissa, the
-    exponent (a float, as without it) held constant."""
+    numpy in -> numpy out; torch CUDA in -> torch CUDA out.  The options are the executor's
+    (``TreeExecutor``); an executor passed in keeps its own, except that ``vjp_max_bytes``, when
+    given, bounds the workspace of this call's backward pass.  With ``stripped_grad`` a stripped
+    result records the gradient of its mantissa, the exponent (a float, as without it) held constant."""
     torch = _torch()
-    if isinstance(tree, TreeExecutor):
-        ex = tree
-    else:
-        if dtype is None:
-            dtype = dtype_name(arrays[0].dtype)
-        ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, vjp_max_bytes=vjp_max_bytes,
-                          precision=precision, stripped_grad=stripped_grad, **plan_opts)
-    all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
-    begin, step, count = (0, 1, None) if slice_ids is None else slice_ids
-    if all_numpy:
-        res = ex.contract_host(arrays, begin, step, count)
-        if ex.strip_exponent:
-            m, e = res
-            return _finish_stripped(m, e, check_zero)
-        return res
+    ex = _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent, vjp_max_bytes=vjp_max_bytes,
+                       precision=precision, stripped_grad=stripped_grad, **plan_opts)
+    slices = (0, 1, None) if slice_ids is None else slice_ids
+    if all(not isinstance(a, torch.Tensor) for a in arrays):
+        res = ex.contract_host(arrays, *slices)
+        return _finish_stripped(*res, check_zero) if ex.strip_exponent else res
     tensors = [_to_device(a, ex.device)[0] for a in arrays]
+    return _run_device(ex, arrays, tensors, slices, check_zero, max_bytes=vjp_max_bytes)
+
+
+def _executor_for(tree, arrays, dtype=None, **opts):
+    """``tree`` itself if it is a ``TreeExecutor`` (which keeps its own options), else a ``TreeExecutor``
+    built from it with ``opts``, for ``dtype`` or by default that of ``arrays[0]``."""
+    if isinstance(tree, TreeExecutor):
+        return tree
+    return TreeExecutor(tree, dtype=dtype_name(arrays[0].dtype) if dtype is None else dtype, **opts)
+
+
+def _run_device(ex, arrays, tensors, slices, check_zero=False, max_bytes=None, as_numpy=False):
+    """``ex.contract_device`` of the device ``tensors`` (made from the caller's ``arrays``) over the
+    slices ``(begin, step, count)``: one torch autograd node when ``_records_grad`` says so, whose
+    backward is ``ex.vjp`` over the same slices within ``max_bytes``; a plain run otherwise.  The
+    result comes back as numpy with ``as_numpy``, and a stripped one as ``(mantissa, float exponent)``."""
+    torch = _torch()
+    begin, step, count = slices
     if _records_grad(torch, arrays, ex.strip_exponent, ex.stripped_grad):
         res = _differentiable(torch, lambda ts: ex.contract_device(ts, begin, step, count),
                               lambda ts, g, wrt, e=None: ex.vjp(ts, g, begin, step, count, wrt=wrt,
-                                                                max_bytes=vjp_max_bytes, exponent=e), tensors)
+                                                                max_bytes=max_bytes, exponent=e), tensors)
     else:
         res = ex.contract_device(tensors, begin, step, count)
     if ex.strip_exponent:
         m, e = res
-        return _finish_stripped(m, float(e.item()), check_zero)
-    return res
+        return _finish_stripped(m, float(e.item()), check_zero, as_numpy)
+    return _from_device(res, as_numpy)
 
 
 def _records_grad(torch, arrays, strip_exponent, stripped_grad=False):
@@ -498,7 +522,7 @@ def _records_grad(torch, arrays, strip_exponent, stripped_grad=False):
         return False
     if strip_exponent and not stripped_grad:
         warnings.warn("strip_exponent=True: no gradient is recorded for the (mantissa, exponent) result",
-                      UserWarning, stacklevel=3)
+                      UserWarning, stacklevel=4)  # (the caller of contract_tree / B200Contractor, past _run_device)
         return False
     return True
 
@@ -547,12 +571,7 @@ def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=
                       **plan_opts):
     """``tree.gen_output_chunks(arrays, with_key=...)`` (cotengra/core.py:3884-3941) on the
     GPU executor; see ``TreeExecutor.gen_output_chunks``."""
-    if isinstance(tree, TreeExecutor):
-        ex = tree
-    else:
-        if dtype is None:
-            dtype = dtype_name(arrays[0].dtype)
-        ex = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, precision=precision, **plan_opts)
+    ex = _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent, precision=precision, **plan_opts)
     yield from ex.gen_output_chunks(arrays, with_key=with_key)
 
 
@@ -569,8 +588,8 @@ def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warm
     import time
 
     torch = _torch()
-    ex = executor if executor is not None else TreeExecutor(tree, dtype=dtype, precision=precision, **plan_opts)
-    tdt = getattr(torch, _NP2T[ex.dtype])
+    ex = executor if executor is not None else _executor_for(tree, (), dtype, precision=precision, **plan_opts)
+    tdt = getattr(torch, ex.dtype)
     gen = torch.Generator(device=ex.device)
     gen.manual_seed(0)
     tensors = []
@@ -638,12 +657,8 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     import hashlib
     import os
 
-    if executor is None:
-        if dtype is None:
-            dtype = dtype_name(arrays[0].dtype)
-        executor = TreeExecutor(tree, dtype=dtype, strip_exponent=strip_exponent, precision=precision,
-                                **plan_opts)
-    ex = executor
+    ex = executor if executor is not None else _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent,
+                                                             precision=precision, **plan_opts)
     spec = ex.spec
     host = [np.asarray(a, dtype=ex.dtype, order="C") for a in arrays]
     h = hashlib.sha256()
@@ -683,11 +698,11 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     return (total, exponent) if ex.strip_exponent else total
 
 
-def _finish_stripped(m, e, check_zero):
+def _finish_stripped(m, e, check_zero, as_numpy=False):
     if check_zero and e == -math.inf:
         # contract.py:819-820
         return 0.0, float("-inf")
-    return m, e
+    return _from_device(m, as_numpy), e
 
 
 class B200Contractor:
@@ -729,13 +744,16 @@ class B200Contractor:
         key = (shapes, dtype, strip, _torch().cuda.current_device())
         ex = self._plans.get(key)
         if ex is None:
-            # synthesise a flat (unsliced) network whose inputs are the given arrays
-            n_in = len(shapes)
+            # synthesise a flat (unsliced) network whose inputs are the given arrays and whose
+            # output term is whatever the program produces
             inputs = [tuple((i, k) for k in range(len(s))) for i, s in enumerate(shapes)]
             size_dict = {(i, k): d for i, s in enumerate(shapes) for k, d in enumerate(s)}
-            ex = _FlatExecutor(self.contractions, inputs, size_dict, dtype, strip, self.vjp_max_bytes,
-                               self.precision, self.stripped_grad)
-            self._plans[key] = ex
+            out_shape = _program_output_shape(self.contractions, shapes)
+            output = tuple(("o", k) for k in range(len(out_shape)))
+            size_dict.update({("o", k): d for k, d in enumerate(out_shape)})
+            ex = self._plans[key] = _Executor(self.contractions, inputs, output, size_dict, (), dtype,
+                                              strip_exponent=strip, vjp_max_bytes=self.vjp_max_bytes,
+                                              precision=self.precision, stripped_grad=self.stripped_grad)
         return ex
 
     def __call__(self, *arrays, **kwargs):
@@ -747,86 +765,13 @@ class B200Contractor:
         if kwargs:
             raise TypeError(f"Unknown keyword arguments: {kwargs}.")
         torch = _torch()
-        strip = strip_exponent is not False
         devs = [_to_device(a) for a in arrays]
         tensors = [d[0] for d in devs]
-        as_numpy = all(d[1] for d in devs)
         dtype = _common_dtype(*tensors)
         with torch.cuda.device(tensors[0].device if tensors else torch.cuda.current_device()):
-            ex = self._executor(tuple(tuple(t.shape) for t in tensors), dtype, strip)
-            on_dev = [t.to(ex.device) for t in tensors]
-            if _records_grad(torch, arrays, strip, self.stripped_grad):
-                res = _differentiable(torch, ex.run, ex.vjp, on_dev)
-                if not strip:
-                    return res
-            else:
-                res = ex.run(on_dev)
-        if strip:
-            m, e = res
-            e = float(e.item())
-            if check_zero and e == -math.inf:
-                return 0.0, float("-inf")
-            return _from_device(m, as_numpy), e
-        return _from_device(res, as_numpy)
-
-
-class _FlatExecutor:
-    """ExecPlan over explicit per-call arrays (no tree-level slicing): the output
-    term is whatever the program produces."""
-
-    def __init__(self, contractions, inputs, size_dict, dtype, strip, vjp_max_bytes=None, precision="3xtf32",
-                 stripped_grad=False):
-        torch = _torch()
-        out_shape = _program_output_shape(contractions, [tuple(size_dict[ix] for ix in t) for t in inputs])
-        output = tuple(("o", k) for k in range(len(out_shape)))
-        sd = dict(size_dict)
-        sd.update({("o", k): d for k, d in enumerate(out_shape)})
-        self.device = torch.device("cuda", torch.cuda.current_device())
-        self.plan = ExecPlan(contractions, inputs, output, sd, (), dtype=dtype,
-                             strip_exponent=strip, precision=precision).create()
-        self.strip = strip
-        self.ws = torch.empty(max(self.plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
-        self.tdt = getattr(torch, _NP2T[self.plan.dtype])
-        self._program = (contractions, inputs, output, sd)
-        self._vjp_plans = {}
-        self.vjp_max_bytes = vjp_max_bytes
-        self.stripped_grad = stripped_grad
-
-    def run(self, tensors):
-        torch = _torch()
-        with torch.cuda.device(self.device):
-            out = torch.zeros(self.plan.out_shape, dtype=self.tdt, device=self.device)
-            exp = torch.full((1,), -math.inf, dtype=torch.float64, device=self.device) if self.strip else None
-            self.plan.execute([t.data_ptr() for t in tensors], out.data_ptr(),
-                              exp.data_ptr() if exp is not None else None, self.ws.data_ptr(),
-                              self.ws.numel(), 0, 1, 1, _stream_ptr())
-        return (out, exp) if self.strip else out
-
-    def vjp(self, tensors, cotangent, wrt, exponent=None):
-        """Input gradients for ``cotangent`` (``None`` outside ``wrt``) through a ``VjpPlan``; a
-        stripped plan's for the mantissa, with the forward's ``exponent`` (a device tensor)."""
-        from .vjp import VjpPlan
-
-        torch = _torch()
-        key = tuple(sorted(wrt))
-        with torch.cuda.device(self.device):
-            plan = self._vjp_plans.get(key)
-            if plan is None:
-                plan = self._vjp_plans[key] = VjpPlan(*self._program, (), dtype=self.plan.dtype, wrt=key,
-                                                              max_bytes=self.vjp_max_bytes,
-                                                              precision=self.plan.precision,
-                                                              strip_exponent=self.strip,
-                                                              stripped_grad=self.stripped_grad).create()
-            cot = cotangent.to(device=self.device, dtype=self.tdt).contiguous()
-            grads = [torch.zeros(tuple(t.shape), dtype=self.tdt, device=self.device) if i in plan.wrt else None
-                     for i, t in enumerate(tensors)]
-            ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
-            srcs = [t.contiguous() for t in tensors]
-            extra = {} if exponent is None else {"exp_ptr": exponent.data_ptr()}
-            plan.execute([t.data_ptr() for t in srcs], cot.data_ptr(),
-                         [g.data_ptr() if g is not None else None for g in grads], ws.data_ptr(), ws.numel(),
-                         0, 1, 1, _stream_ptr(), **extra)
-        return grads
+            ex = self._executor(tuple(tuple(t.shape) for t in tensors), dtype, strip_exponent is not False)
+            return _run_device(ex, arrays, [t.to(ex.device) for t in tensors], (0, 1, 1), check_zero,
+                               as_numpy=all(d[1] for d in devs))
 
 
 def _program_output_shape(contractions, shapes):
@@ -913,10 +858,8 @@ def contract_distributed(tree, arrays, root=None, group=None, strip_exponent=Fal
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     rank_slices(rank, world, spec.nslices)  # raises like core.py:4062-4066
     if executor is None:
-        if dtype is None:
-            dtype = dtype_name(arrays[0].dtype)
-        executor = TreeExecutor(spec, dtype=dtype, strip_exponent=strip_exponent, precision=precision,
-                                **plan_opts)
+        executor = _executor_for(spec, arrays, dtype, strip_exponent=strip_exponent, precision=precision,
+                                 **plan_opts)
     all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
     tensors = [_to_device(a, executor.device)[0] for a in arrays]
     begin, step, count = rank_slices(rank, world, spec.nslices)

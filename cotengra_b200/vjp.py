@@ -469,11 +469,6 @@ class VjpPlan(_DevicePlan):
         sched, sizes, _total, _t, _held, self.recompute_macs = schedule(fits[0])
         return sched, sizes
 
-    @property
-    def _vd(self):
-        """The plan's ``ctgb_plan_desc`` (``_pd``) under the name VJP emulation code reads it by."""
-        return self._pd
-
     # ------------------------------------------------------------------ work
     def vjp_macs(self, count):
         """Scalar MACs of one call over ``count`` slices: the recomputed forward (root excluded)

@@ -157,6 +157,30 @@ def test_tree_executor_plans_carry_the_bit(monkeypatch):
     a = cb.contract_tree(spec, arrays, dtype="complex64", fuse=False)
     b = cb.contract_tree(spec, arrays, dtype="complex64", fuse=False, precision="tf32")
     assert np.allclose(a, b)
+    # gen_output_chunks and contract_distributed (one gloo rank) hand the mode to the plans they launch
+    import torch.distributed as dist
+
+    seen = []
+    launch = cb.ExecPlan.execute  # (the emulated launch)
+
+    def spy(self, *args, **kw):
+        seen.append(self.precision)
+        return launch(self, *args, **kw)
+
+    monkeypatch.setattr(cb.ExecPlan, "execute", spy)
+    want = list(ex0.gen_output_chunks(arrays))
+    for prec in ("3xtf32", "tf32"):
+        seen.clear()
+        got = list(cb.gen_output_chunks(spec, arrays, dtype="complex64", fuse=False, precision=prec))
+        assert len(seen) == len(got) == len(want) and set(seen) == {prec}
+        assert all(np.allclose(g, w) for g, w in zip(got, want))
+        seen.clear()
+        dist.init_process_group("gloo", rank=0, world_size=1, store=dist.HashStore())
+        try:
+            got = cb.contract_distributed(spec, arrays, dtype="complex64", fuse=False, precision=prec)
+        finally:
+            dist.destroy_process_group()
+        assert seen == [prec] and np.allclose(got, a)
 
 
 def _tag(spec, dtype, strip, arrays, extra=b""):

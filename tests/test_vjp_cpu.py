@@ -242,9 +242,11 @@ def test_strip_exponent_with_grad_warns(monkeypatch):
     rec, spec, ex = _emulated_executor(monkeypatch, "lattice4x4_sliced", strip_exponent=True)
     arrays = make_arrays(spec.shapes(), rec["dtype"], seed=rec["seed"])
     m0, e0 = cb.contract_tree(ex, [torch.tensor(a) for a in arrays])
-    with pytest.warns(UserWarning, match="no gradient"):
+    with pytest.warns(UserWarning, match="no gradient") as warned:
         m, e = cb.contract_tree(ex, [torch.tensor(a, requires_grad=True) for a in arrays])
     assert e == e0 and torch.equal(m, m0) and m.grad_fn is None
+    # the warning points at the caller's line
+    assert [w.filename for w in warned if "no gradient" in str(w.message)] == [__file__]
     with pytest.raises(NotImplementedError):
         ex.vjp([torch.tensor(a) for a in arrays], torch.ones(ex.plan.out_shape, dtype=m.dtype))
 

@@ -284,9 +284,17 @@ def test_default_path_unchanged(monkeypatch):
     emu_strip.install(monkeypatch)
     rec, spec, arrays = _case("lattice4x4_sliced")
     ex = cb.TreeExecutor(spec, dtype=rec["dtype"], strip_exponent=True)
-    with pytest.warns(UserWarning, match="no gradient"):
+    with pytest.warns(UserWarning, match="no gradient") as warned:
         m, _e = cb.contract_tree(ex, [torch.tensor(a, requires_grad=True) for a in arrays])
     assert m.grad_fn is None
+    # the same from the per-slice drop-in contractor; both warnings point at the caller's line
+    con = cb.B200Contractor.from_tree(spec, strip_exponent=True)
+    sl = go.slice_arrays(spec.inputs, spec.sliced, arrays, 0)
+    with pytest.warns(UserWarning, match="no gradient") as warned_con:
+        ms, _es = con(*[torch.tensor(np.ascontiguousarray(a), requires_grad=True) for a in sl])
+    assert ms.grad_fn is None
+    for w in (warned, warned_con):
+        assert [x.filename for x in w if "no gradient" in str(x.message)] == [__file__]
     with pytest.raises(NotImplementedError):
         VjpPlan(spec.contractions(), spec.inputs, spec.output, spec.size_dict, spec.sliced,
                 dtype=rec["dtype"], strip_exponent=True)
