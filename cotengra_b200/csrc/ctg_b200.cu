@@ -521,9 +521,10 @@ int launch_gett_typed(const int64_t* h, const int64_t* d, const void* A, const v
   }
   if constexpr (sizeof(T) == 16 || (sizeof(T) == 8 && std::is_same<T, double>::value)) {
     switch (variant) {
-      case VAR_DMMA_128x64: return launch_gett_policy<T, DmmaPolicy<T, 4, 2, 4, 4, 16, 3>>(h, d, A, B, C, st);
-      case VAR_DMMA_64x128: return launch_gett_policy<T, DmmaPolicy<T, 2, 4, 4, 4, 16, 3>>(h, d, A, B, C, st);
-      case VAR_DMMA_256x32: return launch_gett_policy<T, DmmaPolicy<T, 8, 1, 4, 4, 8, 4>>(h, d, A, B, C, st);
+      // (B slots: K = 64 keeps the small operand resident -- four k-steps of 16, eight of 8)
+      case VAR_DMMA_128x64: return launch_gett_policy<T, DmmaPolicy<T, 4, 2, 4, 4, 16, 3, false, 4>>(h, d, A, B, C, st);
+      case VAR_DMMA_64x128: return launch_gett_policy<T, DmmaPolicy<T, 2, 4, 4, 4, 16, 3, false, 4>>(h, d, A, B, C, st);
+      case VAR_DMMA_256x32: return launch_gett_policy<T, DmmaPolicy<T, 8, 1, 4, 4, 8, 4, false, 8>>(h, d, A, B, C, st);
       case VAR_DMMA_256x16: return launch_gett_policy<T, DmmaPolicy<T, 8, 1, 4, 2, 8, 5>>(h, d, A, B, C, st);
       // (K 16 x 4 stages = 80 KB per CTA: with K 32 x 3 stages -- 122 KB -- only ONE CTA fitted an SM,
       // four consumer warps, tensor pipe 72 % under ncu)

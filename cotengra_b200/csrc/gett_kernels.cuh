@@ -19,6 +19,8 @@
 #include <math_constants.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "gett_desc.h"
 
 namespace ctgb {
@@ -492,7 +494,10 @@ __device__ __forceinline__ void dmma16x8x4(double (&lo)[2], double (&hi)[2], dou
 // instead: rows g and g + 8 of the instruction are rows g of fragments i and i + 1,
 // and a lane owns two adjacent columns of C in one row.
 
-template <typename T, int WARPS_M, int WARPS_N, int FM, int FN, int KT_, int STAGES_, bool M3_ = false>
+// B_SLOTS_: shared-memory slots for the small operand's tile (at least STAGES): a node with up to that
+// many k-steps keeps it resident (gett_ws.cuh b_resident)
+template <typename T, int WARPS_M, int WARPS_N, int FM, int FN, int KT_, int STAGES_, bool M3_ = false,
+          int B_SLOTS_ = STAGES_>
 struct DmmaPolicy {
   // T is double (real) or double2 (complex)
   static constexpr bool CPLX = sizeof(T) == 16;
@@ -500,6 +505,7 @@ struct DmmaPolicy {
   static constexpr int MT = WARPS_M * FM * 8, NT = WARPS_N * FN * 8, KT = KT_, STAGES = STAGES_;
   static constexpr int THREADS = WARPS_M * WARPS_N * 32;
   static constexpr int A_ELEMS = MT * KT, B_ELEMS = NT * KT;
+  static constexpr int B_SLOTS = B_SLOTS_;
   static constexpr int SCRATCH_ELEMS = 0;
   // 8 consumer warps x 232 + 4 producer warps x 40 registers = 64512 <= 65536
   static constexpr int CONSUMER_REGS = (THREADS == 256) ? 232 : 0, PRODUCER_REGS = 40;

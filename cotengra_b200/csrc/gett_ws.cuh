@@ -66,6 +66,18 @@ struct BCacheOf<P, true> {
   using type = typename P::BCache;
 };
 
+// B slots of a policy: the ring's STAGES, or P::B_SLOTS where the policy declares more -- a resident
+// small operand (gett_kernel's b_resident) keeps one slot per k-step of the node, so that nodes with
+// more k-steps than ring stages keep it too
+template <class P, class = void>
+struct BSlotsOf {
+  static constexpr int value = P::STAGES;
+};
+template <class P>
+struct BSlotsOf<P, std::void_t<decltype(P::B_SLOTS)>> {
+  static constexpr int value = P::B_SLOTS > P::STAGES ? P::B_SLOTS : P::STAGES;
+};
+
 template <class P>
 struct GettSmem {
   static constexpr int NA = (P::A_ELEMS + PRODUCER_THREADS - 1) / PRODUCER_THREADS;
@@ -78,7 +90,8 @@ struct GettSmem {
   static constexpr int TI = P::STAGES + 2;
   template <typename T>
   static constexpr size_t bytes() {
-    return sizeof(T) * ((size_t)P::STAGES * (P::A_ELEMS + P::B_ELEMS) + P::SCRATCH_ELEMS)  // ring + scratch
+    return sizeof(T) * ((size_t)P::STAGES * P::A_ELEMS + (size_t)BSlotsOf<P>::value * P::B_ELEMS +
+                        P::SCRATCH_ELEMS)                                                    // ring + scratch
            + 8 * (size_t)(NA + NB) * PRODUCER_THREADS                                      // element deltas
            + 8 * (size_t)(P::MT + P::NT)                                                   // C offsets
            + 8 * (size_t)2 * KCHUNK                                                        // k-step bases
@@ -93,13 +106,13 @@ struct GettSmem {
 template <typename T, class P>
 __global__ void __launch_bounds__(P::THREADS + PRODUCER_THREADS, P::MIN_BLOCKS)
 gett_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B, T* __restrict__ C) {
-  constexpr int MT = P::MT, NT = P::NT, STAGES = P::STAGES;
+  constexpr int MT = P::MT, NT = P::NT, STAGES = P::STAGES, BSLOTS = BSlotsOf<P>::value;
   constexpr int NCONS = P::THREADS, NPROD = PRODUCER_THREADS, NTHR = NCONS + NPROD;
   constexpr int NA = GettSmem<P>::NA, NB = GettSmem<P>::NB, TI = GettSmem<P>::TI;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   T* sA = reinterpret_cast<T*>(smem_raw);
   T* sB = sA + STAGES * P::A_ELEMS;
-  T* scratch = sB + STAGES * P::B_ELEMS;
+  T* scratch = sB + BSLOTS * P::B_ELEMS;
   long long* gA = reinterpret_cast<long long*>(scratch + P::SCRATCH_ELEMS);
   long long* gB = gA + NA * NPROD;
   long long* offMC = gB + NB * NPROD;
@@ -157,7 +170,7 @@ gett_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __r
 
   // ---- one-time tables (all threads) ----
   // zero the operand ring: rows/cols/k beyond the actual tile are never loaded
-  for (int i = tid; i < STAGES * (P::A_ELEMS + P::B_ELEMS); i += NTHR) sA[i] = zero_of<T>();
+  for (int i = tid; i < STAGES * P::A_ELEMS + BSLOTS * P::B_ELEMS; i += NTHR) sA[i] = zero_of<T>();
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&bar_full[s], NPROD);
@@ -263,17 +276,20 @@ gett_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __r
     k1 = min(steps_k, k0 + steps_per_split);
   };
 
+  // The small operand's tile of k-step s never changes when every work item of this CTA has the same n
+  // tile (no batch grid, no split-K, a grid that is a multiple of tiles_n: t % tiles_n is
+  // blockIdx.x % tiles_n) and every k-step has a B slot of its own: it is fetched once, into slot s,
+  // with the first work item, and stays.  For a K = 64, N = 128 node that is two thirds of what the
+  // producers would otherwise move per tile, all of it the same.
+  const bool b_resident = splitk == 1 && n_gb == 0 && (gridDim.x % tiles_n) == 0 && steps_k <= (unsigned)BSLOTS;
+  // B slot of a step: its k-step when resident, else its ring stage
+  auto b_slot = [&](unsigned step, int st) -> int { return b_resident ? (int)step : st; };
+
   if (is_producer) {
     // ===================================================== PRODUCER WARPS
     if constexpr (P::CONSUMER_REGS > 0) reg_dealloc<P::PRODUCER_REGS>();
     unsigned ktab_base = 0;
     unsigned g = 0;  // global stage counter
-    // The small operand's tile of a ring slot never changes when there is no n / batch grid and the
-    // k-steps of a work item map onto the slots the same way every time (steps_k divides STAGES):
-    // it is fetched once per slot and stays -- for a K = 16, N = 128 node that is 32 of the 48 KB the
-    // producers would move per tile, all of it the same 32 KB.
-    const bool b_resident = splitk == 1 && n_gn == 0 && n_gb == 0 && steps_k <= (unsigned)STAGES &&
-                            ((unsigned)STAGES % steps_k) == 0;
     for (unsigned j = 0; j < nw; ++j) {
       unsigned k0, k1;
       work_krange(j, k0, k1);
@@ -358,7 +374,7 @@ gett_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __r
         const int st = (int)(g % STAGES);
         mbar_wait(&bar_empty[st], ((g / STAGES) & 1) ^ 1);
         T* dA = sA + st * P::A_ELEMS;
-        T* dB = sB + st * P::B_ELEMS;
+        T* dB = sB + b_slot(step, st) * P::B_ELEMS;
         const unsigned ti = step - ktab_base;
         const T* srcA = A + tA + kbA[ti];
         const T* srcB = B + tB + kbB[ti];
@@ -380,8 +396,8 @@ gett_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __r
             }
           }
         }
-        if (b_resident && g >= (unsigned)STAGES) {
-          // (this slot already holds the tile)
+        if (b_resident && g >= steps_k) {
+          // (slot `step` already holds the tile: the first work item, k-steps 0 .. steps_k - 1, filled it)
         } else if (exactB) {
 #pragma unroll
           for (int i = 0; i < NB; ++i) {
@@ -433,15 +449,15 @@ gett_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __r
         if constexpr (P::HAS_BCACHE) {
           if (b_invariant) {
             if (!b_loaded) {
-              P::load_b(sB + st * P::B_ELEMS, bcache);
+              P::load_b(sB + b_slot(step, st) * P::B_ELEMS, bcache);
               b_loaded = true;
             }
             P::compute_cached(sA + st * P::A_ELEMS, bcache, acc, kv, NTa);
           } else {
-            P::compute(sA + st * P::A_ELEMS, sB + st * P::B_ELEMS, acc, kv, NTa);
+            P::compute(sA + st * P::A_ELEMS, sB + b_slot(step, st) * P::B_ELEMS, acc, kv, NTa);
           }
         } else
-          P::compute(sA + st * P::A_ELEMS, sB + st * P::B_ELEMS, acc, kv, NTa);
+          P::compute(sA + st * P::A_ELEMS, sB + b_slot(step, st) * P::B_ELEMS, acc, kv, NTa);
         __syncwarp();
         if (lane == 0) mbar_arrive(&bar_empty[st]);
       }
