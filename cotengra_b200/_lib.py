@@ -40,8 +40,10 @@ EXPORTS = (
     "ctgb_plan_profile_read",
     "ctgb_probe_fp64_peaks",
     "ctgb_tc05_launch_config",
+    "ctgb_dmmastream_launch_config",
 )
 TC05_LAUNCH_FIELDS = ("b_stat", "nb", "sa", "grid", "smem", "tm_rank", "bulk", "chunk_steps", "chunks")
+DMMASTREAM_LAUNCH_FIELDS = ("nj", "rows", "grid")
 
 
 class CtgbTensor(C.Structure):
@@ -141,6 +143,7 @@ def load():
     lib.ctgb_probe_fp64_peaks.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p]
     lib.ctgb_tc05_launch_config.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_uint64,
                                             C.POINTER(C.c_int64), C.c_int]
+    lib.ctgb_dmmastream_launch_config.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.c_int]
     if lib.ctgb_abi_version() != 2:
         raise ImportError("libctgb200.so: ABI version mismatch")
     if lib.ctgb_desc_words() != lowering.DESC_WORDS:
@@ -191,3 +194,14 @@ def tc05_launch_config(words, a_addr, sms, smem_optin) -> dict:
     check(load().ctgb_tc05_launch_config(w.ctypes.data, int(a_addr), int(sms), int(smem_optin), out,
                                          len(TC05_LAUNCH_FIELDS)))
     return dict(zip(TC05_LAUNCH_FIELDS, (int(x) for x in out)))
+
+
+def dmmastream_launch_config(words, sms) -> dict:
+    """The DMMA stream kernel's instantiation (``nj`` column fragments, ``rows`` per warp block) and
+    grid for descriptor ``words`` on a device with ``sms`` SMs (include/ctg_b200.h).  Needs no device."""
+    import numpy as np
+
+    w = np.ascontiguousarray(words, dtype=np.int64)
+    out = (C.c_int64 * len(DMMASTREAM_LAUNCH_FIELDS))()
+    check(load().ctgb_dmmastream_launch_config(w.ctypes.data, int(sms), out, len(DMMASTREAM_LAUNCH_FIELDS)))
+    return dict(zip(DMMASTREAM_LAUNCH_FIELDS, (int(x) for x in out)))

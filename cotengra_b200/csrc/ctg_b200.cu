@@ -238,31 +238,54 @@ int launch_dotstream(const int64_t* h, const int64_t* d, const void* A, const vo
   return CTGB_OK;
 }
 
-int launch_dmmastream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
-  DevInfo& di = devinfo();
-  if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
+// The DMMA stream kernel's instantiation and grid for a descriptor: pure host code, so
+// ctgb_dmmastream_launch_config reports exactly what launch_dmmastream runs.
+struct DsLaunch {
+  int nj = 0;                       // column fragments (N <= 8*nj)
+  int rows = 0;                     // rows of one warp block (8 per row group)
+  unsigned long long blocks = 0;    // CTAs (0: nothing to launch)
+};
+
+int dmmastream_launch_config(const int64_t* h, int sms, DsLaunch& lc) {
   const int N = (int)h[W_NTA], K = (int)h[W_KTA];
-  if (h[W_DTYPE] != CTGB_C128 || N > 32 || K > DS_KMAX || h[W_TILES_N] != 1 || h[W_TILES_B] != 1 ||
-      h[W_STEPS_K] != 1 || h[W_SPLITK] != 1 || h[W_PGM] >= 0 && (h[W_MFULL] % h[W_MTEXT]) != 0 || h[W_PGN] >= 0 ||
-      h[W_PGK] >= 0)
+  if (h[W_DTYPE] != CTGB_C128 || N > 64 || K > (N <= 32 ? DS_KMAX : DS_KMAX_WIDE) || h[W_TILES_N] != 1 ||
+      h[W_TILES_B] != 1 || h[W_STEPS_K] != 1 || h[W_SPLITK] != 1 ||
+      h[W_PGM] >= 0 && (h[W_MFULL] % h[W_MTEXT]) != 0 || h[W_PGN] >= 0 || h[W_PGK] >= 0)
     return fail(CTGB_E_VALUE, "descriptor does not fit the DMMA stream kernel");
   const unsigned long long M = (unsigned long long)h[W_MTA] * (unsigned long long)h[W_TILES_M];
   if (M >= (1ull << 32)) return fail(CTGB_E_VALUE, "too many rows for the DMMA stream kernel");
-  if (M == 0) return CTGB_OK;
-  unsigned long long blocks = (M + 127) / 128;  // 4 warps x 32 rows per block and pass
-  const unsigned long long cap = (unsigned long long)di.sms * 12;
-  if (blocks > cap) blocks = cap;
+  // 64 accumulator doubles per lane at most: 32-row warp blocks up to N = 32, 16-row ones beyond
+  lc.nj = N <= 8 ? 1 : N <= 16 ? 2 : N <= 32 ? 4 : 8;
+  lc.rows = lc.nj <= 4 ? 32 : 16;
+  const unsigned long long per = 4ull * lc.rows;  // 4 warps per block and pass
+  lc.blocks = (M + per - 1) / per;
+  const unsigned long long cap = (unsigned long long)sms * 12;
+  if (lc.blocks > cap) lc.blocks = cap;
+  return CTGB_OK;
+}
+
+template <int NJ, int RG>
+void dmmastream_launch(bool strip, unsigned blocks, const int64_t* d, const double2* a, const double2* b, double2* c,
+                       cudaStream_t st) {
+  if (strip) dmmastream_kernel<NJ, RG, true><<<blocks, 128, 0, st>>>(d, a, b, c);
+  else dmmastream_kernel<NJ, RG><<<blocks, 128, 0, st>>>(d, a, b, c);
+}
+
+int launch_dmmastream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
+  DevInfo& di = devinfo();
+  if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
+  DsLaunch lc;
+  if (int rc = dmmastream_launch_config(h, di.sms, lc)) return rc;
+  if (lc.blocks == 0) return CTGB_OK;
   const bool strip = h[W_SCALE_A] != 0 || h[W_FACTOR_C] != 0;  // fused strip_exponent: separate instantiations
   const double2 *a = (const double2*)A, *b = (const double2*)B;
-  if (N <= 8) {
-    if (strip) dmmastream_kernel<1, true><<<(unsigned)blocks, 128, 0, st>>>(d, a, b, (double2*)C);
-    else dmmastream_kernel<1><<<(unsigned)blocks, 128, 0, st>>>(d, a, b, (double2*)C);
-  } else if (N <= 16) {
-    if (strip) dmmastream_kernel<2, true><<<(unsigned)blocks, 128, 0, st>>>(d, a, b, (double2*)C);
-    else dmmastream_kernel<2><<<(unsigned)blocks, 128, 0, st>>>(d, a, b, (double2*)C);
-  } else {
-    if (strip) dmmastream_kernel<4, true><<<(unsigned)blocks, 128, 0, st>>>(d, a, b, (double2*)C);
-    else dmmastream_kernel<4><<<(unsigned)blocks, 128, 0, st>>>(d, a, b, (double2*)C);
+  double2* c = (double2*)C;
+  const unsigned blocks = (unsigned)lc.blocks;
+  switch (lc.nj) {
+    case 1: dmmastream_launch<1, 4>(strip, blocks, d, a, b, c, st); break;
+    case 2: dmmastream_launch<2, 4>(strip, blocks, d, a, b, c, st); break;
+    case 4: dmmastream_launch<4, 4>(strip, blocks, d, a, b, c, st); break;
+    default: dmmastream_launch<8, 2>(strip, blocks, d, a, b, c, st); break;
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   CUDA_TRY(cudaGetLastError());
@@ -904,6 +927,20 @@ int ctgb_tc05_launch_config(const int64_t* words, uint64_t a_addr, int sms, uint
   const int64_t v[9] = {lc.b_stat, lc.nb, lc.sa, (int64_t)lc.grid, (int64_t)lc.smem, lc.tm_rank, lc.bulk,
                         (int64_t)lc.chunk, (int64_t)lc.chunks};
   for (int i = 0; i < 9; ++i) out[i] = v[i];
+  return CTGB_OK;
+}
+
+int ctgb_dmmastream_launch_config(const int64_t* words, int sms, int64_t* out, int n_out) {
+  if (!words || !out) return fail(CTGB_E_VALUE, "null argument");
+  if (words[W_MAGIC] != DESC_MAGIC) return fail(CTGB_E_VALUE, "bad descriptor");
+  if (n_out < 3) return fail(CTGB_E_VALUE, "ctgb_dmmastream_launch_config writes 3 words");
+  if (sms < 1) return fail(CTGB_E_VALUE, "sms must be positive");
+  if (words[W_VARIANT] != VAR_DMMASTREAM) return fail(CTGB_E_VALUE, "not a DMMA stream descriptor");
+  DsLaunch lc;
+  if (int rc = dmmastream_launch_config(words, sms, lc)) return rc;
+  out[0] = lc.nj;
+  out[1] = lc.rows;
+  out[2] = (int64_t)lc.blocks;
   return CTGB_OK;
 }
 

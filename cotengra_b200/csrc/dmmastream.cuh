@@ -1,9 +1,9 @@
 // dmmastream.cuh -- fp64 tensor-core streaming kernel for narrow complex128 nodes
-// (N <= 8*NJ, K <= 64, no batch): the rowstream idea with DMMA fragments.
+// (N <= 8*NJ, K <= 64 -- K <= 32 for NJ = 8 --, no batch): the rowstream idea with DMMA fragments.
 //
-// Every warp owns blocks of 32 output rows and runs them start to finish on its own:
+// Every warp owns blocks of 8*RG output rows and runs them start to finish on its own:
 // A fragments straight from global memory into registers (a lane holds one complex element
-// per 8-row group: two LDG.64, 32 of them in flight per lane), B fragments from a
+// per 8-row group: two LDG.64, 8*RG of them in flight per lane), B fragments from a
 // zero-padded shared-memory copy made once per CTA, 4 real m16n8k4 DMMAs per pair of 8-row
 // groups and B fragment, 128-bit stores.  No operand staging, no producer warps, no CTA
 // barriers in the loop: the warps of an SM drift apart, so loads, DMMAs and stores of different row blocks overlap by themselves
@@ -12,21 +12,24 @@
 // (included inside namespace ctgb)
 #pragma once
 
-constexpr int DS_KMAX = 64;
+constexpr int DS_KMAX = 64;       // k rows of the s_B copy for NJ <= 4
+constexpr int DS_KMAX_WIDE = 32;  // ... for NJ = 8 (64 x 64 complex doubles would be 64 KB of static shared memory)
 
-// NJ = column fragments (N <= 8*NJ).  128 threads x 3 blocks (NJ <= 2: <= 170 registers) or x 2 blocks
-// (NJ = 4: 128 accumulator registers), 16 loads in flight per lane.  NJ = 1 serves skinny nodes
+// NJ = column fragments (N <= 8*NJ), RG = 8-row groups per warp block (4: 32 rows, 2: 16 rows -- one
+// m16 pair).  128 threads x 3 blocks (NJ <= 2: <= 170 registers) or x 2 blocks (NJ = 4 at 32 rows and
+// NJ = 8 at 16 rows: both 64 accumulator doubles per lane).  NJ = 1 serves skinny nodes
 // whose contracted space is too long for the row-stream kernel (N <= 8, 8 < K <= 64: the staged
 // row policy ran the M = 2^22, N = 8, K = 64 node of the Sycamore slice at 0.57 of its roofline)
-template <int NJ, bool STRIP = false>
+template <int NJ, int RG, bool STRIP = false>
 __global__ void __launch_bounds__(128, NJ <= 2 ? 3 : 2)
 dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, const double2* __restrict__ B,
                   double2* __restrict__ C) {
-  constexpr int DS_NMAX = NJ * 8;
+  static_assert(RG == 2 || RG == 4, "a warp block is one or two m16 fragment pairs");
+  constexpr int DS_NMAX = NJ * 8, DS_KB = NJ <= 4 ? DS_KMAX : DS_KMAX_WIDE, ROWS = RG * 8;
   __shared__ long long s_akoff[DS_KMAX], s_bkoff[DS_KMAX], s_bnoff[DS_NMAX], s_cnoff[DS_NMAX];
   __shared__ long long s_msA[RS_MAXDIMS], s_msC[RS_MAXDIMS];
   __shared__ unsigned s_mext[RS_MAXDIMS];
-  __shared__ double2 s_B[DS_KMAX * DS_NMAX];  // [k][n], zero beyond (K, N)
+  __shared__ double2 s_B[DS_KB * DS_NMAX];  // [k][n], zero beyond (K, N); the launcher keeps K <= DS_KB
   const int tid = threadIdx.x, lane = tid & 31;
   const int n_tm = (int)D[W_NTM], n_gm = (int)D[W_NGM], n_tk = (int)D[W_NTK], n_tn = (int)D[W_NTN];
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
@@ -80,7 +83,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
     s_cnoff[c] = o;
   }
   __syncthreads();
-  for (int i = tid; i < DS_KMAX * DS_NMAX; i += blockDim.x) {
+  for (int i = tid; i < DS_KB * DS_NMAX; i += blockDim.x) {
     const int kk = i / DS_NMAX, c = i % DS_NMAX;
     s_B[i] = (kk < K && c < N) ? B[s_bkoff[kk] + s_bnoff[c]] : make_double2(0.0, 0.0);
   }
@@ -92,16 +95,16 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
   const int n8s = (N + 7) >> 3;       // column fragments in use
   const int kchunks = (K + 15) >> 4;  // chunks of 16 k (4 k4-steps each)
   const unsigned long long M = (unsigned long long)D[W_MTA] * (unsigned long long)D[W_TILES_M];
-  const unsigned long long nblk = (M + 31) >> 5;
+  const unsigned long long nblk = (M + ROWS - 1) / ROWS;
   const unsigned long long wstride = (unsigned long long)gridDim.x * (blockDim.x >> 5);
   for (unsigned long long blk = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (tid >> 5); blk < nblk;
        blk += wstride) {
-    // the lane's four rows, one per 8-row group (groups 0,1 and 2,3 each form an m16 fragment)
-    long long oa[4], oc[4];
-    bool live[4];
+    // the lane's RG rows, one per 8-row group (groups 0,1 and 2,3 each form an m16 fragment)
+    long long oa[RG], oc[RG];
+    bool live[RG];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const unsigned long long m = blk * 32 + (unsigned)(i * 8 + frow);
+    for (int i = 0; i < RG; ++i) {
+      const unsigned long long m = blk * ROWS + (unsigned)(i * 8 + frow);
       live[i] = m < M;
       unsigned e = live[i] ? (unsigned)m : 0u;
       long long xa = 0, xc = 0;
@@ -125,24 +128,24 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
       oa[i] = xa;
       oc[i] = xc;
     }
-    double re[4][NJ][2], im[4][NJ][2];
+    double re[RG][NJ][2], im[RG][NJ][2];
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+    for (int i = 0; i < RG; ++i)
 #pragma unroll
       for (int j = 0; j < NJ; ++j) re[i][j][0] = re[i][j][1] = im[i][j][0] = im[i][j][1] = 0.0;
     for (int kc = 0; kc < kchunks; ++kc) {
-      // 32 independent 64-bit loads per lane: element (row i*8 + frow, k = kc*16 + k4*4 + fk).
+      // 8*RG independent 64-bit loads per lane: element (row i*8 + frow, k = kc*16 + k4*4 + fk).
       // Not one 128-bit load per element: an m16n8k4 A operand is the real (or imaginary)
       // parts of two rows in adjacent registers, and 128-bit loads make ptxas copy them
       // there, which spilled the NJ = 2 kernels.
-      double2 a[4][4];
+      double2 a[RG][4];
 #pragma unroll
       for (int k4 = 0; k4 < 4; ++k4) {
         const int kk = kc * 16 + k4 * 4 + fk;
         const long long ko = s_akoff[kk & (DS_KMAX - 1)];
         const bool kin = kk < K;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
+        for (int i = 0; i < RG; ++i) {
           const double* pa = reinterpret_cast<const double*>(A + oa[i] + ko);
           a[i][k4].x = kin ? __ldg(pa) : 0.0;
           a[i][k4].y = kin ? __ldg(pa + 1) : 0.0;
@@ -156,22 +159,22 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
 #pragma unroll
         for (int j = 0; j < NJ; ++j) b[j] = s_B[(kc * 16 + k4 * 4 + fk) * DS_NMAX + j * 8 + frow];
 #pragma unroll
-        for (int i = 0; i < 4; i += 2)
+        for (int i = 0; i < RG; i += 2)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
             if (j < n8s) dmma16x8x4(re[i][j], re[i + 1][j], a[i][k4].x, a[i + 1][k4].x, b[j].x);
 #pragma unroll
-        for (int i = 0; i < 4; i += 2)
+        for (int i = 0; i < RG; i += 2)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
             if (j < n8s) dmma16x8x4(im[i][j], im[i + 1][j], a[i][k4].x, a[i + 1][k4].x, b[j].y);
 #pragma unroll
-        for (int i = 0; i < 4; i += 2)
+        for (int i = 0; i < RG; i += 2)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
             if (j < n8s) dmma16x8x4(re[i][j], re[i + 1][j], a[i][k4].y, a[i + 1][k4].y, -b[j].y);
 #pragma unroll
-        for (int i = 0; i < 4; i += 2)
+        for (int i = 0; i < RG; i += 2)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
             if (j < n8s) dmma16x8x4(im[i][j], im[i + 1][j], a[i][k4].y, a[i + 1][k4].y, b[j].x);
@@ -182,7 +185,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
         // max|C|: integer scan over the accumulators, then (rarely) the values (see gett_ws.cuh)
         int hmax = 0;
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < RG; ++i)
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
 #pragma unroll
@@ -190,7 +193,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
               hmax = max(hmax, max(strip_hi(re[i][j][e]), strip_hi(im[i][j][e])));
         if (strip_hot<double2>(sctx, hmax)) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
+          for (int i = 0; i < RG; ++i)
 #pragma unroll
             for (int j = 0; j < NJ; ++j)
 #pragma unroll
@@ -201,7 +204,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
     }
     // a lane owns columns (fc, fc+1) of fragment j in row i*8 + frow
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < RG; ++i) {
       if (!live[i]) continue;
       double2* crow = C + oc[i];
 #pragma unroll

@@ -83,7 +83,7 @@ enum : int {
   VAR_DMMA3M_128x32 = 12,  // complex128, 3M complex product (three DMMAs per fragment pair)
   VAR_DMMA3M_256x16 = 13,
   VAR_DOTSTREAM = 15,      // M = N = 1: the final inner product, operands straight from global memory
-  VAR_DMMASTREAM = 14,     // complex128, 8 < N <= 16, K <= 32: DMMA fragments straight from global memory
+  VAR_DMMASTREAM = 14,     // complex128, N <= 32 with K <= 64, N <= 64 with K <= 32: DMMA fragments straight from global memory
   VAR_DOTSTREAM4 = 16,     // M, N <= 4 over a huge contracted range: a peeled stem tail times the other stem
   // (17: a DMMA-fragments-from-global variant of the next one, measured slower -- 11.1 vs 10.1 ms on
   //  the M = N = 32, K = 2^25 node -- and removed)

@@ -61,7 +61,22 @@ VAR_DMMA_256x16, VAR_ROW_128x8, VAR_ROW_256x4, VAR_ROWSTREAM = 5, 6, 7, 8
 VAR_TC05_128x64, VAR_TC05_128x32, VAR_TC05_128x16 = 9, 10, 11
 VAR_DMMA3M_128x32, VAR_DMMA3M_256x16, VAR_DMMASTREAM, VAR_DOTSTREAM, VAR_DOTSTREAM4 = 12, 13, 14, 15, 16
 VAR_DMMA_32x32, VAR_ROWSTREAM_K, VAR_TF32_32x32 = 18, 19, 20
-DMMASTREAM_MAX_N = 16  # the kernel takes N <= 32, but at N = 32 the staged 256x32 policy is faster (31.8 vs 26 TFLOP/s)
+# the DMMA stream kernel (csrc/dmmastream.cuh) takes N <= 32 with K <= 64 (32-row warp blocks) and
+# 32 < N <= 64 with K <= 32 (16-row warp blocks)
+DMMASTREAM_KMAX, DMMASTREAM_WIDE_N, DMMASTREAM_WIDE_KMAX = 64, 64, 32
+
+
+def dmmastream_fits(N, K):
+    return (N <= 32 and K <= DMMASTREAM_KMAX) or (N <= DMMASTREAM_WIDE_N and K <= DMMASTREAM_WIDE_KMAX)
+
+
+# choose_variant sends it the complex128 nodes with N <= 32, K <= 64.  One Sycamore-m20 slice on an H100
+# 80GB HBM3 (700 W), per node against the staged tiles (DESIGN.md 6a): N = 32 ran at 2.4-2.8 TB/s against
+# 2.0-2.4 (2^25 x 32 x 32: 12.25 vs 15.71 ms; 2^24 x 32 x 64: 9.26 vs 12.66 ms), but the 16-row N = 64
+# blocks were not faster than DMMA_128x64 (2^24 x 64 x 32: 11.3-11.8 vs 10.8 ms), so N > 32 stays staged.
+DMMASTREAM_MAX_N = 32
+
+
 TC05_VARIANTS = (VAR_TC05_128x64, VAR_TC05_128x32, VAR_TC05_128x16)
 TC05_MAX_K = 16384       # 1024 k-steps (the kernel's k table); beyond 256 in chunks of 256
 TC05_CHUNK_STEPS = 16    # full k-steps accumulated in one register accumulation before a round-to-nearest fold (tc05_chunk_steps in
@@ -82,7 +97,7 @@ VARIANT_TILES = {
     VAR_TC05_128x16: (128, 16, 16),
     VAR_DMMA3M_128x32: (128, 32, 16),
     VAR_DMMA3M_256x16: (256, 16, 8),
-    VAR_DMMASTREAM: (256, 32, 64),
+    VAR_DMMASTREAM: (256, 64, 64),
     VAR_DOTSTREAM: (1, 1, 2048),
     VAR_DOTSTREAM4: (4, 4, 1024),
     VAR_DMMA_32x32: (32, 32, 16),
@@ -383,7 +398,7 @@ def choose_variant(dtype, B, M, N, K, allow_dmma=True, allow_stream=True, allow_
     # narrow complex128 nodes: DMMA fragments streamed from global memory, no staging
     # (N <= 8 with a contracted space too long for the row-stream kernel included)
     if (allow_dmma and allow_stream and dtype == "complex128" and B == 1 and 4096 <= M < 1 << 32
-            and ((N <= DMMASTREAM_MAX_N and K <= 32) or (N <= 8 and 8 < K <= 64))):
+            and N <= DMMASTREAM_MAX_N and K <= DMMASTREAM_KMAX):
         return VAR_DMMASTREAM
     # ... and the narrower element types: the row stream walked in chunks of 8 k
     if (allow_stream and DTYPE_SIZES[dtype] <= 8 and N <= 8 and 8 < K <= 64 and B == 1
@@ -450,7 +465,7 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
     if variant in (VAR_DMMA3M_128x32, VAR_DMMA3M_256x16) and dtype != "complex128":
         # the 3M identity is a complex128 kernel: other dtypes take the plain tensor-core tiles
         variant = VAR_DMMA_256x32 if variant == VAR_DMMA3M_128x32 else VAR_DMMA_256x16
-    if variant == VAR_DMMASTREAM and not (dtype == "complex128" and N <= 32 and K <= 64 and B == 1 and M < 1 << 32):
+    if variant == VAR_DMMASTREAM and not (dtype == "complex128" and dmmastream_fits(N, K) and B == 1 and M < 1 << 32):
         variant = VAR_DMMA_256x16
     if variant == VAR_ROWSTREAM:
         # (a ragged blocked m dim is caught after tiling, below)
@@ -583,8 +598,12 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
         return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_SIMT_64x64,
                                allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
                                precision=precision)
-    if variant == VAR_DMMASTREAM and (pn is not None or pk is not None or (pm is not None and pm[1] % pm[2] != 0)):
-        return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_DMMA_256x16,
+    if variant == VAR_DMMASTREAM and (pn is not None or pk is not None or (pm is not None and pm[1] % pm[2] != 0)
+                                      or tiles_n != 1 or steps_k != 1):
+        # ragged, or more dims than one tile holds: the staged tile choose_variant picks without the
+        # stream kernel (N <= 16: 256x16, as before N = 17..32 streamed)
+        fb = VAR_DMMA_256x16 if N <= 16 else choose_variant(dtype, B, M, N, K, allow_dmma, allow_stream=False)
+        return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=fb,
                                allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
                                precision=precision)
     if variant == VAR_ROWSTREAM_K:

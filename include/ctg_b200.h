@@ -265,6 +265,14 @@ int64_t ctgb_tensor_map_launches(void);
 int ctgb_tc05_launch_config(const int64_t* words, uint64_t a_addr, int sms,
                             uint64_t smem_optin, int64_t* out, int n_out);
 
+/* The instantiation and grid ctgb_contract_pair launches for a DMMA stream (complex128)
+ * descriptor on a device with `sms` SMs.  Touches no device.  Writes n_out >= 3 words:
+ *   out[0] column fragments of 8 (N <= 8*out[0])
+ *   out[1] rows of one warp block (32, or 16 for N > 32)
+ *   out[2] CTAs (0: nothing to launch)
+ * A descriptor the kernel does not take fails as ctgb_contract_pair would. */
+int ctgb_dmmastream_launch_config(const int64_t* words, int sms, int64_t* out, int n_out);
+
 #ifdef __cplusplus
 }
 #endif
