@@ -28,6 +28,7 @@ EXPORTS = (
     "ctgb_plan_create",
     "ctgb_plan_set_chunk_desc",
     "ctgb_plan_set_scale_slots",
+    "ctgb_plan_set_accumulator",
     "ctgb_plan_destroy",
     "ctgb_plan_workspace_bytes",
     "ctgb_plan_launches_per_slice",
@@ -127,6 +128,7 @@ def load():
     lib.ctgb_plan_create.argtypes = [C.POINTER(CtgbPlanDesc), C.POINTER(C.c_void_p)]
     lib.ctgb_plan_set_chunk_desc.argtypes = [C.c_void_p, C.c_void_p]
     lib.ctgb_plan_set_scale_slots.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]
+    lib.ctgb_plan_set_accumulator.argtypes = [C.c_void_p, C.c_int32]
     lib.ctgb_plan_destroy.argtypes = [C.c_void_p]
     lib.ctgb_plan_destroy.restype = None
     lib.ctgb_plan_execute.argtypes = [

@@ -33,6 +33,7 @@ from .executor import ExecPlan, output_chunking
 from .lowering import (
     build_pair_desc,
     build_single_desc,
+    check_accumulate,
     check_precision,
     check_tensordot_shapes,
     classify_pair,
@@ -187,6 +188,12 @@ class _Executor:
     ``precision`` is the compute mode of the float32 / complex64 tensor-core nodes of every plan it
     builds (forward, output chunks, reverse mode): ``"3xtf32"`` (default) or ``"tf32"``.
 
+    ``accumulate`` is where the slices are summed: ``"native"`` (default, the plan dtype) or
+    ``"double"``, with which a float32 / complex64 program adds every slice to a float64 / complex128
+    output in double precision and returns it unrounded (``ExecPlan``); for the double dtypes it is
+    ``"native"``.  Gradients through a wide result keep the inputs' dtype: the cotangent is cast to the
+    plan dtype and the reverse-mode plans are those of ``"native"``.
+
     ``vjp_max_bytes`` bounds the workspace of its reverse-mode plans (``vjp_plan``, ``vjp``), which
     then recompute per-slice forward values instead of keeping them (``VjpPlan(max_bytes=...)``).
 
@@ -198,7 +205,7 @@ class _Executor:
     """
 
     def __init__(self, contractions, inputs, output, size_dict, sliced, dtype, strip_exponent=False, device=None,
-                 vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, **plan_opts):
+                 vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, accumulate="native", **plan_opts):
         torch = _torch()
         self._ir, self._plan_opts = contractions, plan_opts
         # the program without its slicing: the positional head of ``ExecPlan`` and ``VjpPlan``
@@ -206,9 +213,11 @@ class _Executor:
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
         with torch.cuda.device(self.device):
             self.plan = ExecPlan(*self._program, sliced, dtype=dtype, strip_exponent=strip_exponent,
-                                 precision=precision, **plan_opts).create()
+                                 precision=precision, accumulate=accumulate, **plan_opts).create()
         self.dtype = self.plan.dtype
         self.precision = precision
+        self.accumulate = accumulate
+        self.out_dtype = self.plan.acc_dtype  # of results: the plan dtype, or its double counterpart
         self.strip_exponent = bool(strip_exponent)
         self.stripped_grad = bool(stripped_grad)
         self.vjp_max_bytes = vjp_max_bytes
@@ -243,13 +252,14 @@ class _Executor:
         torch = _torch()
         self._check_inputs(tensors)
         begin, step, count = self._check_slice_range(begin, step, count)
-        tdt = getattr(torch, self.dtype)
+        tdt = getattr(torch, self.out_dtype)
         with torch.cuda.device(self.device):
             if out is None:
                 out = torch.zeros(self.plan.out_shape, dtype=tdt, device=self.device)
             elif (out.device != self.device or not out.is_contiguous() or out.dtype != tdt
                   or tuple(out.shape) != tuple(self.plan.out_shape)):
-                raise ValueError("out must be a contiguous tensor of the plan's output shape, dtype and device")
+                raise ValueError("out must be a contiguous tensor of the plan's output shape, accumulator dtype "
+                                 "and device")
             if self.strip_exponent and exponent is None:
                 exponent = torch.full((1,), -math.inf, dtype=torch.float64, device=self.device)
             ws = self.workspace()
@@ -354,7 +364,7 @@ class _Executor:
         self._check_inputs(arrays)
         begin, step, count = self._check_slice_range(begin, step, count)
         host = [np.asarray(a, dtype=self.dtype, order="C") for a in arrays]
-        out = np.zeros(self.plan.out_shape, dtype=self.dtype)
+        out = np.zeros(self.plan.out_shape, dtype=self.out_dtype)
         with torch.cuda.device(self.device):
             ws = self.workspace(host_staging=True)
             e = self.plan.execute_host(host, out, ws.data_ptr(), ws.numel(), begin, step, count,
@@ -373,8 +383,9 @@ class TreeExecutor(_Executor):
 
     def __init__(self, tree, dtype="complex128", strip_exponent=False, device=None,
                  contractions=None, fuse=True, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False,
-                 **plan_opts):
+                 accumulate="native", **plan_opts):
         check_precision(precision, dtype)
+        check_accumulate(accumulate)
         self.spec = spec = tree if isinstance(tree, TreeSpec) else TreeSpec.from_cotengra(tree)
         # stem fusion (fusion.py): an execution-plan transformation of the tree cotengra found --
         # big stem tensors absorb pre-contracted groups of small tensors in one pass.  ``spec``
@@ -391,7 +402,7 @@ class TreeExecutor(_Executor):
         ir = self.exec_spec.contractions() if contractions is None else contractions
         super().__init__(ir, spec.inputs, spec.output, spec.size_dict, spec.sliced, dtype,
                          strip_exponent=strip_exponent, device=device, vjp_max_bytes=vjp_max_bytes,
-                         precision=precision, stripped_grad=stripped_grad, **plan_opts)
+                         precision=precision, stripped_grad=stripped_grad, accumulate=accumulate, **plan_opts)
         self._ref_work = None
 
     @property
@@ -423,7 +434,8 @@ class TreeExecutor(_Executor):
             with torch.cuda.device(self.device):
                 self._chunk = ExecPlan(spec.contractions(), spec.inputs, chunk_out, spec.size_dict,
                                        spec.sliced, dtype=self.dtype,
-                                       strip_exponent=self.strip_exponent, precision=self.precision).create()
+                                       strip_exponent=self.strip_exponent, precision=self.precision,
+                                       accumulate=self.accumulate).create()
         return self._chunk
 
     def gen_output_chunks(self, arrays, with_key=False):
@@ -442,7 +454,7 @@ class TreeExecutor(_Executor):
         all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
         tensors = [_to_device(a, self.device)[0] for a in arrays]
         ptrs = [t.data_ptr() for t in tensors]
-        tdt = getattr(torch, self.dtype)
+        tdt = getattr(torch, self.out_dtype)
         need = plan.total_bytes
         # a buffer of its own, not ``_ws``: the generator yields between launches, and a
         # ``contract_device`` call in between must not overwrite the arena of a pending chunk
@@ -466,7 +478,8 @@ class TreeExecutor(_Executor):
 
 
 def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=None,
-                  slice_ids=None, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, **plan_opts):
+                  slice_ids=None, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False,
+                  accumulate="native", **plan_opts):
     """``tree.contract(arrays)`` (cotengra/core.py:3943): takes the *unsliced*
     arrays, handles slicing, contraction and gathering, returns the output in
     ``tree.output`` order -- or ``(mantissa, exponent)`` with ``strip_exponent``.
@@ -476,7 +489,7 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
     result records the gradient of its mantissa, the exponent (a float, as without it) held constant."""
     torch = _torch()
     ex = _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent, vjp_max_bytes=vjp_max_bytes,
-                       precision=precision, stripped_grad=stripped_grad, **plan_opts)
+                       precision=precision, stripped_grad=stripped_grad, accumulate=accumulate, **plan_opts)
     slices = (0, 1, None) if slice_ids is None else slice_ids
     if all(not isinstance(a, torch.Tensor) for a in arrays):
         res = ex.contract_host(arrays, *slices)
@@ -568,15 +581,16 @@ def _differentiable(torch, run, vjp, tensors):
 
 
 def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=None, precision="3xtf32",
-                      **plan_opts):
+                      accumulate="native", **plan_opts):
     """``tree.gen_output_chunks(arrays, with_key=...)`` (cotengra/core.py:3884-3941) on the
     GPU executor; see ``TreeExecutor.gen_output_chunks``."""
-    ex = _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent, precision=precision, **plan_opts)
+    ex = _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent, precision=precision,
+                       accumulate=accumulate, **plan_opts)
     yield from ex.gen_output_chunks(arrays, with_key=with_key)
 
 
 def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warmup=True,
-              executor=None, precision="3xtf32", **plan_opts):
+              executor=None, precision="3xtf32", accumulate="native", **plan_opts):
     """``tree.benchmark(dtype, max_time, min_reps, max_reps, warmup)`` (cotengra/core.py:
     4092-4164) on the GPU executor, same protocol and same keys: random inputs, ``warmup``
     untimed slices, then single slices ``i % nslices`` (each one synchronised, as the
@@ -588,7 +602,8 @@ def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warm
     import time
 
     torch = _torch()
-    ex = executor if executor is not None else _executor_for(tree, (), dtype, precision=precision, **plan_opts)
+    ex = executor if executor is not None else _executor_for(tree, (), dtype, precision=precision,
+                                                             accumulate=accumulate, **plan_opts)
     tdt = getattr(torch, ex.dtype)
     gen = torch.Generator(device=ex.device)
     gen.manual_seed(0)
@@ -598,7 +613,7 @@ def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warm
         (torch.view_as_real(t) if t.is_complex() else t).normal_(generator=gen)
         tensors.append(t / max(1.0, float(t.numel()) ** 0.5))
     nslices = int(ex.nslices)
-    out = torch.zeros(ex.plan.out_shape, dtype=tdt, device=ex.device)
+    out = torch.zeros(ex.plan.out_shape, dtype=getattr(torch, ex.out_dtype), device=ex.device)
 
     def one(i):
         ex.contract_device(tensors, begin=i % nslices, step=1, count=1, out=out)
@@ -641,7 +656,7 @@ def _combine_stripped(m1, e1, m2, e2):
 
 
 def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=False, dtype=None,
-                          executor=None, on_block=None, precision="3xtf32", **plan_opts):
+                          executor=None, on_block=None, precision="3xtf32", accumulate="native", **plan_opts):
     """``tree.contract(arrays)`` for runs too long to lose (SURVEY 8f-4, partial-sum
     checkpointing; the reference has no equivalent -- ``tree.contract`` restarts at
     slice 0): the slices are contracted in blocks of ``every``, and after each block
@@ -653,12 +668,15 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     overwritten.  Slices are independent, so the result equals the uninterrupted
     run up to floating-point summation order.  numpy inputs and outputs (host path).
     ``on_block(next_slice, nslices)`` is called after every saved block.  A file written
-    under the other ``precision`` is refused too: the two modes give different sums."""
+    under the other ``precision`` is refused too: the two modes give different sums.  With
+    ``accumulate="double"`` on a float32 / complex64 tree the stored partial is the float64 /
+    complex128 one, and a file of one accumulation mode is refused by the other."""
     import hashlib
     import os
 
     ex = executor if executor is not None else _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent,
-                                                             precision=precision, **plan_opts)
+                                                             precision=precision, accumulate=accumulate,
+                                                             **plan_opts)
     spec = ex.spec
     host = [np.asarray(a, dtype=ex.dtype, order="C") for a in arrays]
     h = hashlib.sha256()
@@ -667,6 +685,9 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     precision = getattr(ex, "precision", "3xtf32")
     if precision != "3xtf32":  # (the default mode hashes as before: existing checkpoints resume)
         h.update(f"precision={precision}|".encode())
+    out_dtype = getattr(ex, "out_dtype", ex.dtype)
+    if out_dtype != ex.dtype:  # (as above: the native tag is the one files already carry)
+        h.update(f"accumulate={out_dtype}|".encode())
     for a in host:
         h.update(str(a.shape).encode())
         h.update(a.tobytes())
@@ -678,7 +699,8 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     if os.path.exists(checkpoint):
         with np.load(checkpoint, allow_pickle=False) as z:
             if str(z["tag"]) != tag:
-                raise ValueError(f"{checkpoint} belongs to a different tree, dtype, precision or set of input values")
+                raise ValueError(f"{checkpoint} belongs to a different tree, dtype, precision, accumulator or set of "
+                                 f"input values")
             done, total, exponent = int(z["next_slice"]), z["partial"], float(z["exponent"])
     while done < nslices:
         count = min(every, nslices - done)
@@ -716,12 +738,13 @@ class B200Contractor:
     """
 
     __slots__ = ("contractions", "strip_exponent", "check_zero", "implementation", "backend",
-                 "progbar", "vjp_max_bytes", "precision", "stripped_grad", "_plans", "__weakref__")
+                 "progbar", "vjp_max_bytes", "precision", "stripped_grad", "accumulate", "_plans", "__weakref__")
 
     def __init__(self, contractions, strip_exponent=False, check_zero=False,
                  implementation="b200", backend=None, progbar=False, vjp_max_bytes=None, precision="3xtf32",
-                 stripped_grad=False):
+                 stripped_grad=False, accumulate="native"):
         self.contractions = tuple(contractions)
+        self.accumulate = check_accumulate(accumulate)  # dtype the result is summed and returned in (TreeExecutor)
         # compute mode of the float32 / complex64 tensor-core nodes (TreeExecutor); checked per dtype at call
         self.precision = check_precision(precision)
         self.vjp_max_bytes = vjp_max_bytes  # workspace bound of the backward pass (VjpPlan max_bytes)
@@ -753,7 +776,8 @@ class B200Contractor:
             size_dict.update({("o", k): d for k, d in enumerate(out_shape)})
             ex = self._plans[key] = _Executor(self.contractions, inputs, output, size_dict, (), dtype,
                                               strip_exponent=strip, vjp_max_bytes=self.vjp_max_bytes,
-                                              precision=self.precision, stripped_grad=self.stripped_grad)
+                                              precision=self.precision, stripped_grad=self.stripped_grad,
+                                              accumulate=self.accumulate)
         return ex
 
     def __call__(self, *arrays, **kwargs):
@@ -802,15 +826,16 @@ def _program_output_shape(contractions, shapes):
 
 
 def make_contractor(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, precision="3xtf32",
-                    stripped_grad=False, **_ignored):
+                    stripped_grad=False, accumulate="native", **_ignored):
     """``cotengra.contract.make_contractor`` for ``implementation="b200"``
     (contract.py:925-1006): the per-slice callable for ``tree``."""
     return B200Contractor.from_tree(tree, strip_exponent=strip_exponent, check_zero=check_zero,
-                                    vjp_max_bytes=vjp_max_bytes, precision=precision, stripped_grad=stripped_grad)
+                                    vjp_max_bytes=vjp_max_bytes, precision=precision, stripped_grad=stripped_grad,
+                                    accumulate=accumulate)
 
 
 def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, precision="3xtf32",
-            stripped_grad=False):
+            stripped_grad=False, accumulate="native"):
     """Route ``tree.contract(...)`` / ``tree.contract_slice(...)`` of a live
     cotengra tree through this package's contractor by seeding its contractor cache
     (core.py:3699-3711).  Key order: ``(autojit, order, prefer_einsum,
@@ -819,9 +844,12 @@ def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, pr
     bounds the workspace of the backward pass of ``tree.contract`` on torch tensors; ``precision``
     is the compute mode of its float32 / complex64 tensor-core nodes (``TreeExecutor``).
     ``stripped_grad`` with ``strip_exponent``: each slice's ``(m_s, e_s)`` records the gradient of
-    ``m_s`` with ``e_s`` held constant, so that the reference's slice combiner backpropagates."""
+    ``m_s`` with ``e_s`` held constant, so that the reference's slice combiner backpropagates.
+    ``accumulate="double"``: every slice of a float32 / complex64 tree comes back as float64 /
+    complex128 (a dot-type root summed in double), so that the reference's slice sum runs in double."""
     fn = make_contractor(tree, strip_exponent=strip_exponent, check_zero=check_zero,
-                         vjp_max_bytes=vjp_max_bytes, precision=precision, stripped_grad=stripped_grad)
+                         vjp_max_bytes=vjp_max_bytes, precision=precision, stripped_grad=stripped_grad,
+                         accumulate=accumulate)
     key = (False, None, False, bool(strip_exponent), check_zero, None, False)
     tree.contraction_cores[key] = fn
     return fn
@@ -833,7 +861,7 @@ def install(tree, strip_exponent=False, check_zero=False, vjp_max_bytes=None, pr
 
 
 def contract_distributed(tree, arrays, root=None, group=None, strip_exponent=False,
-                         dtype=None, executor=None, precision="3xtf32", **plan_opts):
+                         dtype=None, executor=None, precision="3xtf32", accumulate="native", **plan_opts):
     """``tree.contract_mpi(arrays, comm, root)`` (cotengra/core.py:4032-4090)
     over ``torch.distributed`` (NCCL on NVLink): rank ``r`` of ``W`` contracts
     slices ``r, r+W, ...`` (core.py:4070), sums them locally on its GPU, then a
@@ -843,7 +871,8 @@ def contract_distributed(tree, arrays, root=None, group=None, strip_exponent=Fal
     (core.py:4051-4055), are sharded too (SURVEY 8f-4): every rank scatters its
     slices into the chunks of a zeroed full-size output (the executor's root
     strides, core.py:3865-3876), so the same single all-reduce assembles the
-    stacked result; only the combination with ``strip_exponent`` stays refused."""
+    stacked result; only the combination with ``strip_exponent`` stays refused.  With
+    ``accumulate="double"`` the ranks' float64 / complex128 partials are what is reduced."""
     import torch.distributed as dist
 
     torch = _torch()
@@ -859,7 +888,7 @@ def contract_distributed(tree, arrays, root=None, group=None, strip_exponent=Fal
     rank_slices(rank, world, spec.nslices)  # raises like core.py:4062-4066
     if executor is None:
         executor = _executor_for(spec, arrays, dtype, strip_exponent=strip_exponent, precision=precision,
-                                 **plan_opts)
+                                 accumulate=accumulate, **plan_opts)
     all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
     tensors = [_to_device(a, executor.device)[0] for a in arrays]
     begin, step, count = rank_slices(rank, world, spec.nslices)

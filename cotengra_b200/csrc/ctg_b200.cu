@@ -208,7 +208,12 @@ int launch_rowstream_longk(const int64_t* h, const int64_t* d, const void* A, co
   }
 }
 
-template <typename T>
+// flags bit8: C is the wide type (double for float32, complex128 for complex64) and the dot-stream
+// kernels sum in it; set on the dot-stream roots of accumulate="double" plans only
+constexpr int64_t FLAG_WIDE_C = 256;
+
+// (CT: the type of C and of the sums, T or WideOf<T>)
+template <typename T, typename CT>
 int launch_dotstream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
   DevInfo& di = devinfo();
   if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
@@ -223,16 +228,16 @@ int launch_dotstream(const int64_t* h, const int64_t* d, const void* A, const vo
     // block partial sums are added atomically: a dense result is zeroed first
     const long long celems = h[W_MTA] * h[W_NTA];
     if (celems > 1 && h[W_CELEMS] != celems) return fail(CTGB_E_VALUE, "dot-stream into a strided C needs accumulate");
-    CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)celems * sizeof(T), st));
+    CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)celems * sizeof(CT), st));
   }
   unsigned long long blocks = (unsigned long long)h[W_STEPS_K];
   // one wave: two resident blocks per SM (one for the 16-accumulator variant)
   const unsigned long long cap = (unsigned long long)di.sms * (mn ? 1 : 2);
   if (blocks > cap) blocks = cap;
   if (mn)
-    dotstream_kernel<T, DOT4_MN, DOT4_MN, dot4_u<T>()><<<(unsigned)blocks, DOT_THREADS, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C);
+    dotstream_kernel<T, DOT4_MN, DOT4_MN, dot4_u<T>(), CT><<<(unsigned)blocks, DOT_THREADS, 0, st>>>(d, (const T*)A, (const T*)B, (CT*)C);
   else
-    dotstream_kernel<T, 1, 1, DOT_U><<<(unsigned)blocks, DOT_THREADS, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C);
+    dotstream_kernel<T, 1, 1, DOT_U, CT><<<(unsigned)blocks, DOT_THREADS, 0, st>>>(d, (const T*)A, (const T*)B, (CT*)C);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   CUDA_TRY(cudaGetLastError());
   return CTGB_OK;
@@ -529,7 +534,13 @@ int launch_gett_typed(const int64_t* h, const int64_t* d, const void* A, const v
   if (variant == VAR_ROWSTREAM) return launch_rowstream<T>(h, d, A, B, C, st);
   if (variant == VAR_ROWSTREAM_K) return launch_rowstream_longk<T>(h, d, A, B, C, st);
   if (variant == VAR_DMMASTREAM) return launch_dmmastream(h, d, A, B, C, st);
-  if (variant == VAR_DOTSTREAM || variant == VAR_DOTSTREAM4) return launch_dotstream<T>(h, d, A, B, C, st);
+  if (h[W_FLAGS] & FLAG_WIDE_C) {
+    using Wide = typename WideOf<T>::type;
+    if (std::is_same<Wide, T>::value || (variant != VAR_DOTSTREAM && variant != VAR_DOTSTREAM4))
+      return fail(CTGB_E_VALUE, "a wide C belongs to float32 / complex64 dot-stream nodes");
+    return launch_dotstream<T, Wide>(h, d, A, B, C, st);
+  }
+  if (variant == VAR_DOTSTREAM || variant == VAR_DOTSTREAM4) return launch_dotstream<T, T>(h, d, A, B, C, st);
   if constexpr (std::is_same<T, float2>::value) {
     if (variant == VAR_TC05_128x64) return one ? launch_tc05<64, true>(h, d, A, B, C, st) : launch_tc05<64, false>(h, d, A, B, C, st);
     if (variant == VAR_TC05_128x32) return one ? launch_tc05<32, true>(h, d, A, B, C, st) : launch_tc05<32, false>(h, d, A, B, C, st);
@@ -663,26 +674,44 @@ int absmax_into(int dtype, const void* p, long long n, unsigned long long* slot,
   return fail(CTGB_E_VALUE, "bad dtype");
 }
 
-template <typename T>
+int wide_dtype(int dtype) { return dtype == CTGB_F32 ? CTGB_F64 : dtype == CTGB_C64 ? CTGB_C128 : dtype; }
+
+// (O: the type of the output accumulator, T or WideOf<T>)
+template <typename T, typename O>
 int accum_stripped_typed(const int64_t* dchunk, const int64_t* hchunk, void* out, void* chunk, long long out_elems,
                          const void* m, double* E, const double* es, const double* froot, cudaStream_t st) {
-  rescale_out_kernel<T><<<flat_grid(out_elems), 256, 0, st>>>((T*)out, out_elems, E, es);
-  add_chunk_kernel<T><<<flat_grid(hchunk[S_OUT_ELEMS]), 256, 0, st>>>(dchunk, (T*)chunk, (const T*)m, E, es, froot);
+  rescale_out_kernel<T, O><<<flat_grid(out_elems), 256, 0, st>>>((O*)out, out_elems, E, es);
+  add_chunk_kernel<T, O><<<flat_grid(hchunk[S_OUT_ELEMS]), 256, 0, st>>>(dchunk, (O*)chunk, (const T*)m, E, es, froot);
   commit_exponent_kernel<<<1, 1, 0, st>>>(E, es);
   g_launches.fetch_add(3, std::memory_order_relaxed);
   CUDA_TRY(cudaGetLastError());
   return CTGB_OK;
 }
-int accum_stripped(int dtype, const int64_t* dchunk, const int64_t* hchunk, void* out, void* chunk,
+int accum_stripped(int dtype, bool wide, const int64_t* dchunk, const int64_t* hchunk, void* out, void* chunk,
                    long long out_elems, const void* m, double* E, const double* es, const double* froot,
                    cudaStream_t st) {
   switch (dtype) {
-    case CTGB_F32: return accum_stripped_typed<float>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
-    case CTGB_F64: return accum_stripped_typed<double>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
-    case CTGB_C64: return accum_stripped_typed<float2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
-    case CTGB_C128: return accum_stripped_typed<double2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
+    case CTGB_F32:
+      return wide ? accum_stripped_typed<float, double>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st)
+                  : accum_stripped_typed<float, float>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
+    case CTGB_F64: return accum_stripped_typed<double, double>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
+    case CTGB_C64:
+      return wide ? accum_stripped_typed<float2, double2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st)
+                  : accum_stripped_typed<float2, float2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
+    case CTGB_C128: return accum_stripped_typed<double2, double2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
   }
   return fail(CTGB_E_VALUE, "bad dtype");
+}
+
+// the dense float32 / complex64 root result of one slice, added into its chunk of the double output
+int add_chunk_wide(int dtype, const int64_t* dchunk, const int64_t* hchunk, void* chunk, const void* m, cudaStream_t st) {
+  const unsigned grid = flat_grid(hchunk[S_OUT_ELEMS]);
+  if (dtype == CTGB_F32) add_chunk_wide_kernel<float, double><<<grid, 256, 0, st>>>(dchunk, (double*)chunk, (const float*)m);
+  else if (dtype == CTGB_C64) add_chunk_wide_kernel<float2, double2><<<grid, 256, 0, st>>>(dchunk, (double2*)chunk, (const float2*)m);
+  else return fail(CTGB_E_VALUE, "a wide accumulator belongs to float32 / complex64 plans");
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  CUDA_TRY(cudaGetLastError());
+  return CTGB_OK;
 }
 
 template <typename T>
@@ -724,6 +753,7 @@ struct ctgb_slice_mem {
   char* out = nullptr;                  // kind 3
   const char* cot = nullptr;            // kind 4
   size_t es = 0;
+  size_t out_es = 0;                    // element size of the output accumulator (kind 3)
   const int64_t* digits = nullptr;
 };
 
@@ -740,7 +770,7 @@ static char* resolve_tensor(const ctgb_tensor_rec& q, const ctgb_slice_mem& m, i
     case 6: return m.persistent + q.offset;
     case 4: return (char*)m.cot + out_off * (int64_t)m.es;
     case 5: return sliced(m.grads[q.input_index]);
-    default: return m.out + out_off * (int64_t)m.es;
+    default: return m.out + out_off * (int64_t)m.out_es;
   }
 }
 
@@ -811,6 +841,11 @@ struct ctgb_plan {
   std::vector<int64_t> radix, project, out_stride;
   int64_t out_elements = 0, workspace_bytes = 0, persistent_bytes = 0;
   int strip_exponent = 0;
+  // dtype of the output accumulator (ctgb_plan_set_accumulator): the plan's, or its double counterpart.
+  // A wide forward plan either has a flagged dot-stream root that adds into `out` in double, or a
+  // root that stores its slice densely in the plan dtype (as stripped plans do), folded afterwards.
+  int acc_dtype = 0;
+  bool wide_desc = false;           // a descriptor carries FLAG_WIDE_C: runs only with a wide accumulator
   int root = -1;                    // the node that writes the output
   bool backward = false;            // phase 2/3 nodes: needs a cotangent and the gradient buffers
   int64_t cot_offset = -1;          // conjugated cotangent copy in the persistent arena
@@ -1021,7 +1056,7 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     delete p;
     return fail(CTGB_E_VALUE, msg);
   };
-  p->dtype = pd->dtype;
+  p->dtype = p->acc_dtype = pd->dtype;
   p->n_inputs = pd->n_inputs;
   if (int rc = copy_tensors(pd->tensors, pd->n_tensors, pd->n_inputs, pd->n_sliced, p->tensors)) {
     delete p;
@@ -1047,6 +1082,10 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     if (bad(n.a) || bad(n.c) || (n.kind == 0 && bad(n.b))) return refuse("node refers to a missing tensor");
     p->backward |= n.phase >= 2;
     if (n.is_root) p->root = i;
+    if (n.kind == 0 && (n.desc[W_FLAGS] & FLAG_WIDE_C)) {
+      if (!n.is_root || pd->strip_exponent) return refuse("a wide C belongs to the root of an unstripped plan");
+      p->wide_desc = true;
+    }
     q.desc_off = p->descs.size();
     p->descs.insert(p->descs.end(), n.desc, n.desc + words);
     q.c_elems = p->tensors[n.c].nbytes / (int64_t)es;
@@ -1175,6 +1214,26 @@ int ctgb_plan_set_chunk_desc(ctgb_plan* p, const int64_t* desc) {
   return CTGB_OK;
 }
 
+int ctgb_plan_set_accumulator(ctgb_plan* p, int32_t dtype) {
+  if (!p) return fail(CTGB_E_VALUE, "null plan");
+  if (dtype != p->dtype && dtype != wide_dtype(p->dtype))
+    return fail(CTGB_E_VALUE, "the accumulator has the plan's dtype or its double counterpart");
+  const bool wide = dtype != p->dtype;
+  if (wide && p->backward) return fail(CTGB_E_VALUE, "a wide accumulator belongs to forward plans");
+  if (wide && !p->strip_exponent) {
+    // the root adds into the double output itself (a flagged dot-stream node) or leaves its slice in
+    // the per-slice workspace for add_chunk_wide
+    if (p->root < 0) return fail(CTGB_E_VALUE, "plan has no root node");
+    const int ckind = p->tensors[p->nodes[p->root].c].kind;
+    if (ckind != (p->wide_desc ? 3 : 1)) return fail(CTGB_E_VALUE, "root slot does not match the wide accumulator");
+    if (!p->wide_desc && p->acc_dtype == p->dtype) p->launches_per_slice += 1;
+  } else if (p->wide_desc) {
+    return fail(CTGB_E_VALUE, "the plan's root descriptor needs a wide accumulator");
+  }
+  p->acc_dtype = dtype;
+  return CTGB_OK;
+}
+
 int ctgb_plan_set_scale_slots(ctgb_plan* p, const int32_t* slot_a, const int32_t* slot_b, int n) {
   if (!p || !slot_a || !slot_b) return fail(CTGB_E_VALUE, "null argument");
   if (!p->scale_pending) return fail(CTGB_E_VALUE, "scale slots belong to stripped reverse-mode plans, once");
@@ -1203,6 +1262,10 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   if (!inputs) return fail(CTGB_E_VALUE, "null inputs");
   if (p->strip_exponent && !p->backward && (!exponent_dev || p->chunk_desc.empty()))
     return fail(CTGB_E_VALUE, "strip_exponent needs an exponent buffer and a chunk descriptor");
+  const bool wide = p->acc_dtype != p->dtype;
+  if (p->wide_desc && !wide) return fail(CTGB_E_VALUE, "the plan's root descriptor needs a wide accumulator");
+  const bool wide_fold = wide && !p->strip_exponent && !p->wide_desc;  // dense root + add_chunk_wide
+  if (wide_fold && p->chunk_desc.empty()) return fail(CTGB_E_VALUE, "a wide accumulator needs a chunk descriptor");
   if (p->strip_exponent && !p->backward && p->root < 0) return fail(CTGB_E_VALUE, "plan has no root node");
   // a stripped reverse-mode plan reads the exponent of the forward call it differentiates
   if (p->strip_exponent && p->backward && (!exponent_dev || p->scale_pending))
@@ -1228,6 +1291,7 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   mem.out = (char*)out;
   mem.cot = (const char*)cotangent;
   mem.es = es;
+  mem.out_es = elem_size(p->acc_dtype);
   mem.digits = digits.data();
   auto resolve = [&](int t, int64_t out_off) -> char* { return resolve_tensor(p->tensors[t], mem, out_off); };
   int rc;
@@ -1330,8 +1394,14 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
       char* m = resolve(root.c, 0);
       // (the stored root is the raw product: its own factor divides it here)
       const double* froot = root.kind == 0 ? p->d_factors + root.c : nullptr;
-      rc = accum_stripped(p->dtype, p->d_chunk_desc, p->chunk_desc.data(), out, (char*)out + out_off * (int64_t)es,
-                          p->out_elements, m, exponent_dev, d_slice_exp, froot, st);
+      rc = accum_stripped(p->dtype, wide, p->d_chunk_desc, p->chunk_desc.data(), out,
+                          (char*)out + out_off * (int64_t)mem.out_es, p->out_elements, m, exponent_dev, d_slice_exp,
+                          froot, st);
+      if (rc) return rc;
+    }
+    if (wide_fold) {
+      rc = add_chunk_wide(p->dtype, p->d_chunk_desc, p->chunk_desc.data(), (char*)out + out_off * (int64_t)mem.out_es,
+                          resolve(p->nodes[p->root].c, 0), st);
       if (rc) return rc;
     }
   }
@@ -1348,7 +1418,7 @@ int ctgb_plan_execute_host(ctgb_plan* p, const void* const* host_inputs, const i
                            int64_t slice_step, int64_t slice_count, void* stream) {
   if (!p) return fail(CTGB_E_VALUE, "null plan");
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t es = elem_size(p->dtype);
+  const size_t es = elem_size(p->acc_dtype);  // (of the output: the inputs come with their byte counts)
   const size_t core = (size_t)(p->workspace_bytes + p->persistent_bytes);
   // staging area at the tail of the workspace: inputs, output, exponent
   size_t need = core;

@@ -24,10 +24,21 @@ constexpr int DOT4_MN = 4;
 template <typename T> constexpr int dot4_u() { return sizeof(T) >= 16 ? 4 : 8; }
 template <typename T> constexpr int dot4_kt() { return dot4_u<T>() * DOT_THREADS; }
 
-template <typename T, int MT, int NT, int U>
+// CT is the type of C and of every sum on the way to it.  CT = T is the plan dtype's own arithmetic.
+// CT = WideOf<T> (descriptor flags bit8, float32 / complex64 roots of accumulate="double" plans) loads
+// the operands exactly as above and converts them in registers: products and per-thread sums are
+// DFMAs, the warp and block reductions and the one atomicAdd per block and real component are double,
+// so the result is the dot product of the fp32 operands to about 1e-15 * sum |a||b|.
+template <typename T, int MT, int NT, int U, typename CT = T>
 __global__ void __launch_bounds__(DOT_THREADS, (MT * NT > 1) ? 1 : 2)
-dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B, T* __restrict__ C) {
-  __shared__ T s_part[DOT_THREADS / 32][MT * NT];
+dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B, CT* __restrict__ C) {
+  __shared__ CT s_part[DOT_THREADS / 32][MT * NT];
+  // the 16 double accumulators of the wide M, N <= 4 kernel (64 registers for complex64) leave no room
+  // for the launch-invariant offsets next to the 16 + 16 loads in flight (128 registers): there they
+  // wait in shared memory, 2 * U conflict-free and MT + NT broadcast reads per tile of 2 * U * 4 loads
+  constexpr bool OFFS_SMEM = MT * NT > 1 && sizeof(CT) > sizeof(T);
+  __shared__ long long s_am[OFFS_SMEM ? MT : 1], s_bn[OFFS_SMEM ? NT : 1];
+  __shared__ long long s_la[OFFS_SMEM ? U : 1][OFFS_SMEM ? DOT_THREADS : 1], s_lb[OFFS_SMEM ? U : 1][OFFS_SMEM ? DOT_THREADS : 1];
   const int tid = threadIdx.x, lane = tid & 31;
   const int n_tk = (int)D[W_NTK], n_gk = (int)D[W_NGK];
   const int KTa = (int)D[W_KTA], MTa = (int)D[W_MTA], NTa = (int)D[W_NTA];
@@ -45,6 +56,7 @@ dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
         e /= (unsigned)L[0];
       }
     am[i] = a;
+    if (OFFS_SMEM && tid == 0) s_am[i] = a;
   }
 #pragma unroll
   for (int i = 0; i < NT; ++i) {
@@ -57,7 +69,9 @@ dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
         e /= (unsigned)L[0];
       }
     bn[i] = b;
+    if (OFFS_SMEM && tid == 0) s_bn[i] = b;
   }
+  if (OFFS_SMEM) __syncthreads();
   // tile-local offsets of this thread's elements (tile dims: dim 0 fastest)
   long long la[U], lb[U];
   bool in_tile[U];
@@ -76,6 +90,10 @@ dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
     }
     la[j] = a;
     lb[j] = b;
+    if (OFFS_SMEM) {
+      s_la[j][tid] = a;
+      s_lb[j][tid] = b;
+    }
   }
   // this lane's grid dims (at most 2 per lane: MAX_G = 40 <= 64)
   unsigned g_ext[2] = {1u, 1u};
@@ -92,11 +110,11 @@ dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
       g_sb[h] = G[3];
     }
   }
-  T acc[MT][NT];
+  CT acc[MT][NT];
 #pragma unroll
   for (int i = 0; i < MT; ++i)
 #pragma unroll
-    for (int c = 0; c < NT; ++c) acc[i][c] = zero_of<T>();
+    for (int c = 0; c < NT; ++c) acc[i][c] = zero_of<CT>();
   for (unsigned t = blockIdx.x; t < steps; t += gridDim.x) {
     long long ta = 0, tb = 0;
 #pragma unroll
@@ -111,9 +129,11 @@ dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
 #pragma unroll
     for (int j = 0; j < U; ++j) {
 #pragma unroll
-      for (int i = 0; i < MT; ++i) a[j][i] = (in_tile[j] && i < MTa) ? A[ta + la[j] + am[i]] : zero_of<T>();
+      for (int i = 0; i < MT; ++i)
+        a[j][i] = (in_tile[j] && i < MTa) ? A[ta + (OFFS_SMEM ? s_la[j][tid] + s_am[i] : la[j] + am[i])] : zero_of<T>();
 #pragma unroll
-      for (int c = 0; c < NT; ++c) b[j][c] = (in_tile[j] && c < NTa) ? B[tb + lb[j] + bn[c]] : zero_of<T>();
+      for (int c = 0; c < NT; ++c)
+        b[j][c] = (in_tile[j] && c < NTa) ? B[tb + (OFFS_SMEM ? s_lb[j][tid] + s_bn[c] : lb[j] + bn[c])] : zero_of<T>();
     }
 #pragma unroll
     for (int j = 0; j < U; ++j)
@@ -127,7 +147,7 @@ dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
   for (int i = 0; i < MT; ++i)
 #pragma unroll
     for (int c = 0; c < NT; ++c) {
-      T v = acc[i][c];
+      CT v = acc[i][c];
 #pragma unroll
       for (int d = 16; d > 0; d >>= 1) v = add_of(v, shfl_down_of(v, d));
       if (lane == 0) s_part[tid >> 5][i * NT + c] = v;
@@ -136,7 +156,7 @@ dotstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
   if (tid < MT * NT) {
     const int i = tid / NT, c = tid % NT;
     if (i < MTa && c < NTa) {
-      T v = s_part[0][tid];
+      CT v = s_part[0][tid];
       for (int w = 1; w < DOT_THREADS / 32; ++w) v = add_of(v, s_part[w][tid]);
       StripCtx sctx = strip_begin(D);  // strip_exponent: partial sums are only scaled here
       if (sctx.scale) v = strip_apply(sctx, v);

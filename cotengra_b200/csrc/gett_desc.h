@@ -40,7 +40,9 @@ enum : int {
                        // bit2: tile-grid extents are powers of two; bit3: all m dims are powers of two;
                        // bit4/5: column quads/pairs of 8-byte elements adjacent+aligned in C;
                        // bit6: wgmma A tile made of contiguous runs; bit7: float32/complex64
-                       // tensor-core variants run ONE round-to-nearest tf32 pass (precision="tf32")
+                       // tensor-core variants run ONE round-to-nearest tf32 pass (precision="tf32");
+                       // bit8: C is the wide type (double / complex128 for float32 / complex64) and the
+                       // sums are formed in it -- dot-stream roots of accumulate="double" plans only
   W_VARIANT = 32,      // kernel variant chosen by the host
   W_CELEMS = 33,       // elements of a dense C (memset before split-K atomics); 0: strided C
   W_RUNA = 34,         // wgmma: elements of the contiguous runs the A tile is made of (flags bit6)

@@ -40,6 +40,16 @@ __device__ __forceinline__ void mac(double2& c, double2 a, double2 b) {
   c.y = fma(a.x, b.y, c.y);
   c.y = fma(a.y, b.x, c.y);
 }
+// single-precision operands into a double accumulator: convert, then DFMA (the products of two
+// floats are exact in double)
+__device__ __forceinline__ void mac(double& c, float a, float b) { c = fma((double)a, (double)b, c); }
+__device__ __forceinline__ void mac(double2& c, float2 a, float2 b) {
+  mac(c, make_double2((double)a.x, (double)a.y), make_double2((double)b.x, (double)b.y));
+}
+// the double counterpart of an element type: what accumulate="double" plans sum slices in
+template <typename T> struct WideOf { using type = T; };
+template <> struct WideOf<float> { using type = double; };
+template <> struct WideOf<float2> { using type = double2; };
 template <typename T> __device__ __forceinline__ T zero_of();
 template <> __device__ __forceinline__ float zero_of<float>() { return 0.f; }
 template <> __device__ __forceinline__ double zero_of<double>() { return 0.0; }
@@ -766,8 +776,16 @@ __device__ __forceinline__ double2 mulr_of(double2 v, double s) { return make_do
 __device__ __forceinline__ double exponent_max(double a, double b) {
   return (a != a || b != b) ? __longlong_as_double(0x7ff8000000000000LL) : fmax(a, b);
 }
-template <typename T>
-__global__ void rescale_out_kernel(T* __restrict__ out, long long n, const double* __restrict__ E,
+// (O: the type of ``out`` -- T, or WideOf<T> when the plan accumulates in double; the mantissa slot
+// ``m`` keeps the plan dtype)
+template <typename O, typename T>
+__device__ __forceinline__ O mulr_as(T v, double s) {
+  if constexpr (std::is_same<O, T>::value) return mulr_of(v, s);
+  else if constexpr (std::is_same<T, float>::value) return (double)v * s;
+  else return make_double2((double)v.x * s, (double)v.y * s);
+}
+template <typename T, typename O = T>
+__global__ void rescale_out_kernel(O* __restrict__ out, long long n, const double* __restrict__ E,
                                    const double* __restrict__ es) {
   const double e = exponent_max(*E, *es);
   const double so = (*E == e) ? 1.0 : pow(10.0, *E - e);
@@ -775,8 +793,8 @@ __global__ void rescale_out_kernel(T* __restrict__ out, long long n, const doubl
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     out[i] = mulr_of(out[i], so);
 }
-template <typename T>
-__global__ void add_chunk_kernel(const int64_t* __restrict__ D, T* __restrict__ out, const T* __restrict__ m,
+template <typename T, typename O = T>
+__global__ void add_chunk_kernel(const int64_t* __restrict__ D, O* __restrict__ out, const T* __restrict__ m,
                                  const double* __restrict__ E, const double* __restrict__ es,
                                  const double* __restrict__ froot) {
   // D: single-operand descriptor mapping the dense slice result onto the chunk
@@ -795,7 +813,26 @@ __global__ void add_chunk_kernel(const int64_t* __restrict__ D, T* __restrict__ 
       xo += dig * L[1];
       oo += dig * L[2];
     }
-    out[oo] = add_of(out[oo], mulr_of(m[xo], sn));
+    out[oo] = add_of(out[oo], mulr_as<O>(m[xo], sn));
+  }
+}
+// accumulate="double" plans whose root is not a dot-stream node: the root stores its slice result
+// densely in the plan dtype, and this folds it into its chunk of the double output (D as above) --
+// one pass over the output per slice, none over any intermediate
+template <typename T, typename Wide>
+__global__ void add_chunk_wide_kernel(const int64_t* __restrict__ D, Wide* __restrict__ out, const T* __restrict__ m) {
+  const int n_o = (int)D[S_NO];
+  const long long n = D[S_OUT_ELEMS];
+  for (long long o = blockIdx.x * (long long)blockDim.x + threadIdx.x; o < n; o += (long long)gridDim.x * blockDim.x) {
+    long long t = o, xo = 0, oo = 0;
+    for (int d = 0; d < n_o; ++d) {
+      const int64_t* L = D + OFF_SO + d * 3;
+      long long dig = t % L[0];
+      t /= L[0];
+      xo += dig * L[1];
+      oo += dig * L[2];
+    }
+    out[oo] = add_of(out[oo], mulr_as<Wide>(m[xo], 1.0));
   }
 }
 __global__ void commit_exponent_kernel(double* __restrict__ E, const double* __restrict__ es) {

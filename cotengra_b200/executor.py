@@ -35,6 +35,7 @@ from . import _lib, lowering
 from .lowering import (
     DTYPE_CODES,
     DTYPE_SIZES,
+    accumulator_dtype,
     build_pair_desc,
     build_single_desc,
     check_precision,
@@ -200,7 +201,8 @@ class _DevicePlan:
     handle = None
     strip_exponent = False
     cotangent_offset = -1
-    _chunk_words = None  # strip_exponent forward plans: ctgb_plan_set_chunk_desc
+    acc_dtype = None     # forward plans that sum their slices in double: ctgb_plan_set_accumulator
+    _chunk_words = None  # forward plans whose root stores its slice densely: ctgb_plan_set_chunk_desc
     scale_slots = None   # stripped reverse-mode plans: ctgb_plan_set_scale_slots, ([slot_a], [slot_b])
 
     def _marshal(self):
@@ -265,6 +267,8 @@ class _DevicePlan:
         if self._chunk_words is not None:
             w = self._chunk_words
             _lib.check(lib.ctgb_plan_set_chunk_desc(h, w.ctypes.data_as(C.c_void_p)))
+        if self.acc_dtype not in (None, self.dtype):
+            _lib.check(lib.ctgb_plan_set_accumulator(h, DTYPE_CODES[self.acc_dtype]))
         if self.scale_slots is not None:
             n = len(self.nodes)
             sa, sb = ((C.c_int32 * max(n, 1))(*s) for s in self.scale_slots)
@@ -306,14 +310,22 @@ class ExecPlan(_DevicePlan):
     sliced : ordered ``[(ind, size, project)]`` as ``tree.sliced_inds``.
     precision : ``"3xtf32"`` (default) or ``"tf32"``, the compute mode of the float32 / complex64
         tensor-core nodes (``lowering.PRECISIONS``); ``"tf32"`` with a double dtype raises ``ValueError``.
+    accumulate : ``"native"`` (default) sums the slices in the plan dtype.  ``"double"`` gives a
+        float32 / complex64 plan a float64 / complex128 output (``acc_dtype``) that every slice is added
+        to in double: a dot-stream root sums in double inside the kernel (``lowering.FLAG_WIDE_C``) and
+        adds into the output itself, any other root stores its slice densely in the workspace and one
+        extra launch folds it in through the chunk descriptor.  For float64 / complex128 it is
+        ``"native"``.
     """
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None, precision="3xtf32"):
+                 variant=None, precision="3xtf32", accumulate="native"):
         self.dtype = dtype_name(dtype)
         self.precision = check_precision(precision, self.dtype)
         self.esize = DTYPE_SIZES[self.dtype]
+        self.acc_dtype = accumulator_dtype(self.dtype, accumulate)
+        self.wide = self.acc_dtype != self.dtype
         self.contractions = tuple(contractions)
         self.inputs = [tuple(t) for t in inputs]
         self.output = tuple(output)
@@ -369,6 +381,9 @@ class ExecPlan(_DevicePlan):
 
         tensors = list(cur.values())
         nodes = []  # dicts
+        # does the root write (accumulate into) the output itself?  Not with strip_exponent, and in a
+        # wide plan only a dot-stream root (decided where the root is lowered)
+        direct = not self.strip_exponent and not self.wide
         n_rec = len(self.contractions)
         for step, (p, l, r, tdot, arg, perm) in enumerate(self.contractions):
             is_last = step == n_rec - 1
@@ -380,14 +395,14 @@ class ExecPlan(_DevicePlan):
                 is_root = l is not None
                 if is_root and not is_last:
                     raise ValueError("single-input record must be the only contraction")
-                ostr = root_strides if (is_root and not self.strip_exponent) else None
+                ostr = root_strides if (is_root and direct) else None
                 odims, sdims, oshape = classify_single(terms[0], src.shape, out, out_strides=ostr,
                                                       strides_x=src.strides)
                 if is_root:
                     self._check_root_shape(oshape)
                 # the root always accumulates into the (zeroed) output, so that
                 # slice sums, split-K atomics and plain stores share one path
-                acc = is_root and not self.strip_exponent
+                acc = is_root and direct
                 words = build_single_desc(odims, sdims, self.dtype, accumulate=acc)
                 dst = _Slot(oshape, row_major_strides(oshape), K_SCRATCH, max(math.prod(oshape), 1) * self.esize,
                             variant=src.variant)
@@ -407,16 +422,27 @@ class ExecPlan(_DevicePlan):
                     raise ValueError(f"expected a two-term equation, got {arg!r}")
                 ta, tb = terms
             is_root = is_last
-            ostr = root_strides if (is_root and not self.strip_exponent) else None
-            dims = classify_pair(ta, A.shape, tb, Bt.shape, to, out_strides=ostr,
-                                 strides_a=A.strides, strides_b=Bt.strides)
+
+            def lower(into_output, wide_c=False):
+                ostr = root_strides if into_output else None
+                dims = classify_pair(ta, A.shape, tb, Bt.shape, to, out_strides=ostr,
+                                     strides_a=A.strides, strides_b=Bt.strides)
+                dense = 0 if into_output else math.prod(dims.out_shape)
+                return dims, dense, build_pair_desc(dims, self.dtype, accumulate=into_output,
+                                                    sm_count=self.sm_count, allow_dmma=allow_dmma,
+                                                    c_dense_elems=dense, variant=variant,
+                                                    precision=self.precision, wide_c=wide_c)
+
+            if is_root and self.wide and not self.strip_exponent:
+                # only the dot-stream kernels sum in double: such a root adds into the wide output
+                # itself, any other one stores its slice densely for add_chunk_wide
+                direct = lower(True)[2].variant in lowering.DOTSTREAM_VARIANTS
+                dims, dense, plan = lower(direct, wide_c=direct)
+            else:
+                dims, dense, plan = lower(is_root and direct)
             if is_root:
                 self._check_root_shape(dims.out_shape)
-            acc = is_root and not self.strip_exponent
-            dense = 0 if (is_root and not self.strip_exponent) else math.prod(dims.out_shape)
-            plan = build_pair_desc(dims, self.dtype, accumulate=acc, sm_count=self.sm_count,
-                                   allow_dmma=allow_dmma, c_dense_elems=dense, variant=variant,
-                                   precision=self.precision)
+            acc = is_root and direct
             dst = _Slot(dims.out_shape, row_major_strides(dims.out_shape), K_SCRATCH,
                         max(math.prod(dims.out_shape), 1) * self.esize, variant=A.variant or Bt.variant)
             a, b = (Bt, A) if plan.swapped else (A, Bt)
@@ -427,7 +453,8 @@ class ExecPlan(_DevicePlan):
 
         if not nodes:
             raise ValueError("empty contraction program")
-        if not self.strip_exponent:
+        self.root_direct = direct
+        if direct:
             nodes[-1]["c"].kind = K_OUTPUT  # the root writes the output accumulator directly
         # invariance: hoisted results live in the persistent arena
         for nd in nodes:
@@ -464,7 +491,7 @@ class ExecPlan(_DevicePlan):
 
         self.tensors = tensors
         self._marshal()
-        if self.strip_exponent:
+        if not direct:
             # dense root result -> its chunk of the (strided) output
             rs = self.root_shape
             dense = row_major_strides(rs)
@@ -483,7 +510,7 @@ class ExecPlan(_DevicePlan):
         extra = _align(self.total_bytes) - self.total_bytes
         for n in self.input_nbytes:
             extra += _align(n)
-        return extra + _align(self.out_elements * self.esize) + 512
+        return extra + _align(self.out_elements * DTYPE_SIZES[self.acc_dtype]) + 512
 
     def execute(self, input_ptrs, out_ptr, exp_ptr, ws_ptr, ws_bytes, begin, step, count, stream=0):
         lib = _lib.load()

@@ -112,6 +112,14 @@ PRECISIONS = ("3xtf32", "tf32")
 FLAG_TF32_ONE_PASS = 128
 TF32_VARIANTS = (VAR_DMMA_128x64, VAR_DMMA_64x128, VAR_DMMA_256x32, VAR_DMMA_256x16, VAR_TF32_32x32) + TC05_VARIANTS
 
+# where the slices of a tree are summed: "native" (the plan dtype) or "double" (float64 / complex128
+# for float32 / complex64 trees; the same as "native" for the double dtypes).  A "double" plan sets
+# descriptor flags bit8, "C is the wide type", on its dot-stream root and on nothing else.
+ACCUMULATORS = ("native", "double")
+FLAG_WIDE_C = 256
+WIDE_DTYPES = {"float32": "float64", "complex64": "complex128"}
+DOTSTREAM_VARIANTS = (VAR_DOTSTREAM, VAR_DOTSTREAM4)
+
 DTYPE_CODES = {"float32": 0, "float64": 1, "complex64": 2, "complex128": 3}
 DTYPE_SIZES = {"float32": 4, "float64": 8, "complex64": 8, "complex128": 16}
 
@@ -136,6 +144,19 @@ def check_precision(precision, dtype=None):
     if precision == "tf32" and dtype is not None and dtype_name(dtype) in ("float64", "complex128"):
         raise ValueError(f"precision='tf32' applies to float32 and complex64, not {dtype_name(dtype)}")
     return precision
+
+
+def check_accumulate(accumulate):
+    """``accumulate`` if it is one of ``ACCUMULATORS``, else ``ValueError``."""
+    if not isinstance(accumulate, str) or accumulate not in ACCUMULATORS:
+        raise ValueError(f"accumulate must be one of {ACCUMULATORS}, got {accumulate!r}")
+    return accumulate
+
+
+def accumulator_dtype(dtype, accumulate="native"):
+    """The dtype a tree of ``dtype`` sums its slices in, and returns, under ``accumulate``."""
+    dtype = dtype_name(dtype)
+    return WIDE_DTYPES.get(dtype, dtype) if check_accumulate(accumulate) == "double" else dtype
 
 
 def row_major_strides(shape):
@@ -439,11 +460,15 @@ def choose_variant(dtype, B, M, N, K, allow_dmma=True, allow_stream=True, allow_
 
 def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
                     variant=None, allow_dmma=True, c_dense_elems=0,
-                    force_splitk=None, precision="3xtf32") -> PairPlan:
+                    force_splitk=None, precision="3xtf32", wide_c=False) -> PairPlan:
     """Pack a classified node into descriptor words.  ``precision`` (``PRECISIONS``) selects the
-    compute mode of the float32 / complex64 tensor-core variants; it changes no other word."""
+    compute mode of the float32 / complex64 tensor-core variants; it changes no other word.
+    ``wide_c`` sets flags bit8 (C has ``WIDE_DTYPES[dtype]`` and the kernel sums in it): only the
+    dot-stream kernels have it, so a node that lowers to any other variant raises ``ValueError``."""
     dtype = dtype_name(dtype)
     check_precision(precision, dtype)
+    if wide_c and dtype not in WIDE_DTYPES:
+        raise ValueError(f"a wide C applies to float32 and complex64, not {dtype}")
     m = coalesce([[d[0], d[1], d[3]] for d in dims.m])          # ext, sA, sC
     n = coalesce([[d[0], d[2], d[3]] for d in dims.n])          # ext, sB, sC
     k = coalesce([[d[0], d[1], d[2]] for d in dims.k])          # ext, sA, sB
@@ -472,6 +497,8 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
         ok = N <= 8 and K <= 8 and B == 1 and M < 1 << 32
         if not ok:
             variant = VAR_ROW_256x4 if N <= 4 else VAR_ROW_128x8
+    if wide_c and variant not in DOTSTREAM_VARIANTS:
+        raise ValueError(f"a wide C needs a dot-stream node, this one lowers to variant {variant}")
     MT, NT, KT = VARIANT_TILES[variant]
     if variant == VAR_DOTSTREAM4 and DTYPE_SIZES[dtype] < 16:
         KT = 2048  # 8 k per thread for the narrower element types (csrc/dotstream.cuh dot4_u)
@@ -590,14 +617,14 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
                                     or (pk is not None and pk[1] % pk[2] != 0)):
         return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_KRED,
                                allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
-                               precision=precision)
+                               precision=precision, wide_c=wide_c)
     if variant == VAR_DOTSTREAM4 and (not (M <= 4 and N <= 4 and B == 1) or len(gk) > 40 or steps_k >= 1 << 31
                                      or pm is not None or pn is not None
                                      or (pk is not None and pk[1] % pk[2] != 0)
                                      or not (accumulate or c_dense_elems == M * N)):
         return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_SIMT_64x64,
                                allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
-                               precision=precision)
+                               precision=precision, wide_c=wide_c)
     if variant == VAR_DMMASTREAM and (pn is not None or pk is not None or (pm is not None and pm[1] % pm[2] != 0)
                                       or tiles_n != 1 or steps_k != 1):
         # ragged, or more dims than one tile holds: the staged tile choose_variant picks without the
@@ -683,7 +710,8 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
     W[W_FLAGS] = ((1 if accumulate else 0) | (2 if pair_ok else 0) | (4 if grid_pow2 else 0)
                   | (8 if m_pow2 else 0) | (16 if _cols_ok(4) else 0) | (32 if _cols_ok(2) else 0)
                   | (64 if bulk_a else 0)
-                  | (FLAG_TF32_ONE_PASS if precision == "tf32" and variant in TF32_VARIANTS else 0))
+                  | (FLAG_TF32_ONE_PASS if precision == "tf32" and variant in TF32_VARIANTS else 0)
+                  | (FLAG_WIDE_C if wide_c else 0))
     W[W_VARIANT] = variant
     W[W_CELEMS] = int(c_dense_elems)
 

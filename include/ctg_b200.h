@@ -162,7 +162,8 @@ typedef struct {
 /* strip_exponent together with phase 2/3 nodes makes a stripped reverse-mode
  * plan, which runs only after ctgb_plan_set_scale_slots. */
 int ctgb_plan_create(const ctgb_plan_desc* desc, ctgb_plan** plan);
-/* strip_exponent only: the single-operand descriptor (ctgb_single_desc_words()
+/* strip_exponent plans, and plans with a wide accumulator whose root is not a
+ * dot-stream node: the single-operand descriptor (ctgb_single_desc_words()
  * words) that maps the dense root result of one slice onto its chunk of the
  * output tensor (identity layout when no sliced index is an output index). */
 int ctgb_plan_set_chunk_desc(ctgb_plan* plan, const int64_t* desc);
@@ -179,6 +180,18 @@ int ctgb_plan_set_chunk_desc(ctgb_plan* plan, const int64_t* desc);
  * record nothing.  The gradient is that of m = amp * 10^-e with e held constant. */
 int ctgb_plan_set_scale_slots(ctgb_plan* plan, const int32_t* slot_a,
                               const int32_t* slot_b, int n);
+/* Forward plans, once after ctgb_plan_create: the dtype of the output accumulator,
+ * the plan's dtype (the default) or its double counterpart (CTGB_F64 for CTGB_F32,
+ * CTGB_C128 for CTGB_C64); anything else fails with CTGB_E_VALUE.  With the double
+ * counterpart every slice is added to `out` in double precision.  The root of such a
+ * plan is either a dot-stream node whose descriptor has flags bit 8 set (C is the
+ * wide type: the kernel forms products and sums in double and adds them into the
+ * output tensor slot, kind 3), or any other node that stores its slice densely in a
+ * workspace slot (kind 1) in the plan dtype; ctgb_plan_set_chunk_desc then maps that
+ * slot onto its chunk of the output, one extra launch per slice.  With
+ * strip_exponent the mantissa of a slice stays in the plan dtype and the running
+ * mantissa in `out` is double. */
+int ctgb_plan_set_accumulator(ctgb_plan* plan, int32_t dtype);
 void ctgb_plan_destroy(ctgb_plan* plan);
 size_t ctgb_plan_workspace_bytes(const ctgb_plan* plan);
 int64_t ctgb_plan_launches_per_slice(const ctgb_plan* plan);
@@ -196,7 +209,9 @@ int ctgb_plan_strip_modes(const ctgb_plan* plan, int32_t* prescale_b, int32_t* m
  * needs with CTGB_E_VALUE, before any launch.
  *
  * A forward plan ACCUMULATES the slices' contributions into `out` (device,
- * out_elements of the plan dtype; the caller zeroes it before the first call).
+ * out_elements of the accumulator dtype -- the plan dtype unless
+ * ctgb_plan_set_accumulator chose its double counterpart; the caller zeroes it
+ * before the first call).
  * With strip_exponent the mantissa is accumulated against the running base-10
  * exponent stored in exponent_dev[0] (device double; core.py:163-170).
  * `cotangent` and `grads` may be null.
@@ -221,8 +236,8 @@ int ctgb_plan_execute(ctgb_plan* plan, const void* const* inputs, void* out,
                       int64_t slice_step, int64_t slice_count, void* stream);
 
 /* Same job for a forward plan with HOST buffers: copies the inputs
- * host->device, runs the slices, copies the accumulated output (and exponent)
- * back, synchronises.  This is the end-to-end call bench.py times as `e2e`.  `workspace` stays a device buffer
+ * host->device, runs the slices, copies the accumulated output (out_elements of the
+ * accumulator dtype) and the exponent back, synchronises.  This is the end-to-end call bench.py times as `e2e`.  `workspace` stays a device buffer
  * (it is scratch); input staging memory is taken from its tail. */
 int ctgb_plan_execute_host(ctgb_plan* plan, const void* const* host_inputs,
                            const int64_t* input_nbytes, void* host_out,
