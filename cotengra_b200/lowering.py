@@ -24,6 +24,7 @@ own planners (tests/test_lowering.py).
 from __future__ import annotations
 
 import math
+from collections import Counter, namedtuple
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -458,13 +459,86 @@ def choose_variant(dtype, B, M, N, K, allow_dmma=True, allow_stream=True, allow_
     return VAR_SIMT_64x64
 
 
+# a blocked dim (split_tile's ``partial``), if any, is cut into whole blocks
+_whole = lambda partial: partial is None or partial[1] % partial[2] == 0  # noqa: E731
+# what the hand-over rules read of a node besides its tiling (sizes after the swap)
+_Node = namedtuple("_Node", "dtype B M N K allow_dmma accumulate c_dense_elems")
+# one variant's split of a node: tile dims, grid dims (with their divisors), the blocked dim of each class
+# (split_tile's ``partial``), the tile's extents, the tile dims' local weights and the operand load orders
+_Tiling = namedtuple("_Tiling", "variant tm tn tk gm gn gk gb pm pn pk tiles_m tiles_n tiles_b tiles steps_k "
+                                "MTa NTa KTa wm wn wk lda ldb")
+# How a specialised variant is admitted, and what runs when it is not: ``fits(node)`` is checked on dtype
+# and sizes before tiling (``unfit(node)`` runs if it fails), ``admits(node, tiling)`` on the variant's
+# finished tiling (``to(node)`` runs if it fails).  Variants without an entry in HANDOVER take any node.
+Handover = namedtuple("Handover", "fits unfit admits to", defaults=(lambda nd: True, None, lambda nd, t: True, None))
+
+
+_row_tile = lambda nd: VAR_ROW_256x4 if nd.N <= 4 else VAR_ROW_128x8  # noqa: E731
+
+
+def _rowstream_k_admits(nd, t):
+    # exact tiles, and the k offsets must decompose as chunk_base[k // 8] + in_chunk[k % 8]
+    koff = lambda e: sum((e // w) % d[0] * d[1] for d, w in zip(t.tk, t.wk))  # noqa: E731
+    return (t.pn is None and t.pk is None and _whole(t.pm) and DTYPE_SIZES[nd.dtype] <= 8 and nd.N <= 8
+            and nd.K <= 64 and nd.B == 1 and nd.M < 1 << 32
+            and all(koff(e) == koff(e - e % 8) + koff(e % 8) for e in range(t.KTa)))
+
+
+def _tc05_admits(nd, t):
+    # the wgmma kernel takes tiles of ONE shape: its native 128 x NT x 16, or smaller with
+    # the rest of the tensor-core tile as padding (KTa in steps of 4: whole wgmma k8 groups);
+    # below 40 % occupancy the mma.sync policy is the better choice
+    # (k padding is free -- the wgmmas of missing k8 groups are not issued -- so only rows and columns count)
+    MT, NT, KT = VARIANT_TILES[t.variant]
+    return (t.MTa <= MT and t.NTa <= NT and t.KTa <= KT and t.KTa % 4 == 0 and nd.dtype == "complex64"
+            and (t.MTa * t.NTa) / float(MT * NT) >= 0.4 and t.steps_k <= 1024
+            and (t.KTa >= 8 or t.steps_k == 1)  # many 4-wide k-steps: per-step overhead, mma.sync is better
+            and _whole(t.pm) and _whole(t.pn) and _whole(t.pk))
+
+
+HANDOVER = {
+    # a ragged blocked m dim: the staged row policy
+    VAR_ROWSTREAM: Handover(fits=lambda nd: nd.N <= 8 and nd.K <= 8 and nd.B == 1 and nd.M < 1 << 32,
+                            unfit=_row_tile, admits=lambda nd, t: _whole(t.pm), to=_row_tile),
+    VAR_ROWSTREAM_K: Handover(admits=_rowstream_k_admits, to=_row_tile),
+    # ragged, or more dims than one tile holds: the staged tile choose_variant picks without the
+    # stream kernel (N <= 16: 256x16, as before N = 17..32 streamed)
+    VAR_DMMASTREAM: Handover(
+        fits=lambda nd: nd.dtype == "complex128" and dmmastream_fits(nd.N, nd.K) and nd.B == 1 and nd.M < 1 << 32,
+        unfit=lambda nd: VAR_DMMA_256x16,
+        admits=lambda nd, t: t.pn is None and t.pk is None and _whole(t.pm) and t.tiles_n == 1 and t.steps_k == 1,
+        to=lambda nd: (VAR_DMMA_256x16 if nd.N <= 16 else
+                       choose_variant(nd.dtype, nd.B, nd.M, nd.N, nd.K, nd.allow_dmma, allow_stream=False))),
+    VAR_DOTSTREAM: Handover(
+        admits=lambda nd, t: nd.M == 1 and nd.N == 1 and nd.B == 1 and t.steps_k < 1 << 31 and _whole(t.pk),
+        to=lambda nd: VAR_KRED),
+    VAR_DOTSTREAM4: Handover(
+        admits=lambda nd, t: (nd.M <= 4 and nd.N <= 4 and nd.B == 1 and t.steps_k < 1 << 31
+                              and t.pm is None and t.pn is None and _whole(t.pk)
+                              and (nd.accumulate or nd.c_dense_elems == nd.M * nd.N)),
+        to=lambda nd: VAR_SIMT_64x64),
+    **{v: Handover(admits=_tc05_admits,
+                   to=lambda nd: choose_variant(nd.dtype, nd.B, nd.M, nd.N, nd.K, nd.allow_dmma, allow_tc05=False))
+       for v in TC05_VARIANTS},
+    # the same tile on the fp64 tensor cores
+    VAR_TF32_32x32: Handover(fits=lambda nd: nd.dtype not in ("float64", "complex128"),
+                             unfit=lambda nd: VAR_DMMA_32x32),
+    # the 3M identity is a complex128 kernel: other dtypes take the plain tensor-core tiles
+    VAR_DMMA3M_128x32: Handover(fits=lambda nd: nd.dtype == "complex128", unfit=lambda nd: VAR_DMMA_256x32),
+    VAR_DMMA3M_256x16: Handover(fits=lambda nd: nd.dtype == "complex128", unfit=lambda nd: VAR_DMMA_256x16),
+}
+STAGED = Handover()
+
+
 def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
                     variant=None, allow_dmma=True, c_dense_elems=0,
                     force_splitk=None, precision="3xtf32", wide_c=False) -> PairPlan:
-    """Pack a classified node into descriptor words.  ``precision`` (``PRECISIONS``) selects the
-    compute mode of the float32 / complex64 tensor-core variants; it changes no other word.
-    ``wide_c`` sets flags bit8 (C has ``WIDE_DTYPES[dtype]`` and the kernel sums in it): only the
-    dot-stream kernels have it, so a node that lowers to any other variant raises ``ValueError``."""
+    """Pack a classified node into descriptor words.  ``variant`` (default: ``choose_variant``'s pick)
+    is the kernel to run; a specialised one the node does not suit hands over as ``HANDOVER`` says.
+    ``precision`` (``PRECISIONS``) selects the compute mode of the float32 / complex64 tensor-core
+    variants; it changes no other word.  ``wide_c`` sets flags bit8 (C has ``WIDE_DTYPES[dtype]`` and
+    the kernel sums in it): only the dot-stream kernels have it, so a node that lowers to any other
+    variant raises ``ValueError``."""
     dtype = dtype_name(dtype)
     check_precision(precision, dtype)
     if wide_c and dtype not in WIDE_DTYPES:
@@ -483,26 +557,35 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
         b = [[d[0], d[2], d[1], d[3]] for d in b]
         M, N = N, M
 
+    nd = _Node(dtype, B, M, N, K, allow_dmma, accumulate, c_dense_elems)
     if variant is None:
         variant = choose_variant(dtype, B, M, N, K, allow_dmma)
-    if variant == VAR_TF32_32x32 and dtype in ("float64", "complex128"):
-        variant = VAR_DMMA_32x32  # the same tile on the fp64 tensor cores
-    if variant in (VAR_DMMA3M_128x32, VAR_DMMA3M_256x16) and dtype != "complex128":
-        # the 3M identity is a complex128 kernel: other dtypes take the plain tensor-core tiles
-        variant = VAR_DMMA_256x32 if variant == VAR_DMMA3M_128x32 else VAR_DMMA_256x16
-    if variant == VAR_DMMASTREAM and not (dtype == "complex128" and dmmastream_fits(N, K) and B == 1 and M < 1 << 32):
-        variant = VAR_DMMA_256x16
-    if variant == VAR_ROWSTREAM:
-        # (a ragged blocked m dim is caught after tiling, below)
-        ok = N <= 8 and K <= 8 and B == 1 and M < 1 << 32
-        if not ok:
-            variant = VAR_ROW_256x4 if N <= 4 else VAR_ROW_128x8
-    if wide_c and variant not in DOTSTREAM_VARIANTS:
-        raise ValueError(f"a wide C needs a dot-stream node, this one lowers to variant {variant}")
+    while True:
+        h = HANDOVER.get(variant, STAGED)
+        if not h.fits(nd):
+            variant = h.unfit(nd)
+            continue
+        if wide_c and variant not in DOTSTREAM_VARIANTS:
+            raise ValueError(f"a wide C needs a dot-stream node, this one lowers to variant {variant}")
+        t = _tile(variant, dtype, m, n, k, b)
+        splitk = _splitk(t, sm_count, force_splitk)  # (a node of 2^31 tiles raises before it hands over)
+        if h.admits(nd, t):
+            break
+        variant = h.to(nd)
+
+    run_a, bulk_a, lbopad = _wgmma_words(t) if variant in TC05_VARIANTS else (1, False, 0)
+    flags = ((1 if accumulate else 0) | _layout_flags(dtype, t) | (64 if bulk_a else 0)
+             | (FLAG_TF32_ONE_PASS if precision == "tf32" and variant in TF32_VARIANTS else 0)
+             | (FLAG_WIDE_C if wide_c else 0))
+    words = _pack(dtype, t, splitk, flags, run_a, lbopad, c_dense_elems)
+    return PairPlan(words, variant, (B, M, N, K), swapped, t.tiles, splitk)
+
+
+def _tile(variant, dtype, m, n, k, b):
+    """Split the coalesced classes into the tile and grid dims of ``variant``."""
     MT, NT, KT = VARIANT_TILES[variant]
     if variant == VAR_DOTSTREAM4 and DTYPE_SIZES[dtype] < 16:
         KT = 2048  # 8 k per thread for the narrower element types (csrc/dotstream.cuh dot4_u)
-
     if variant in TC05_VARIANTS:
         # wgmma: the epilogue addresses every row through its own offset, so the rows of a tile need
         # not be neighbours in C -- pick them for the longest contiguous runs of A instead
@@ -520,215 +603,129 @@ def build_pair_desc(dims: PairDims, dtype, accumulate=False, sm_count=132,
     gb = list(b)
     for name, lst, cap in (("m", gm, MAX_G), ("n", gn, MAX_G), ("k", gk, MAX_G), ("batch", gb, MAX_GB)):
         if len(lst) > cap:
-            raise NotImplementedError(
-                f"{len(lst)} non-coalescable {name} dims exceed the descriptor capacity {cap}"
-            )
-    gm, tiles_m = _with_divs(gm)
-    gn, tiles_n = _with_divs(gn)
-    gk, steps_k = _with_divs(gk)
-    gb, tiles_b = _with_divs(gb)
-
-    MTa = math.prod(d[0] for d in tm)
-    NTa = math.prod(d[0] for d in tn)
-    KTa = math.prod(d[0] for d in tk)
+            raise NotImplementedError(f"{len(lst)} non-coalescable {name} dims exceed the descriptor capacity {cap}")
+    (gm, tiles_m), (gn, tiles_n), (gk, steps_k), (gb, tiles_b) = map(_with_divs, (gm, gn, gk, gb))
 
     # local weights (dim 0 fastest; partial dim is last by construction)
-    def weights(tile):
-        w, acc = [], 1
-        for d in tile:
-            w.append(acc)
-            acc *= d[0]
-        return w
-
-    wm, wn, wk = weights(tm), weights(tn), weights(tk)
+    (wm, MTa), (wn, NTa), (wk, KTa) = (_weights(ts) for ts in (tm, tn, tk))
     # operand load orders: ascending stride in that operand (coalesced gathers)
     lda = [[d[0], d[1], w, 0] for d, w in zip(tm, wm)] + [[d[0], d[1], 0, w] for d, w in zip(tk, wk)]
     ldb = [[d[0], d[2], w, 0] for d, w in zip(tk, wk)] + [[d[0], d[1], 0, w] for d, w in zip(tn, wn)]
     key = lambda r: (abs(r[1]) if r[1] else 1 << 62)  # noqa: E731
     lda.sort(key=key)
     ldb.sort(key=key)
+    return _Tiling(variant, tm, tn, tk, gm, gn, gk, gb, pm, pn, pk, tiles_m, tiles_n, tiles_b, tiles_m * tiles_n * tiles_b,
+                   steps_k, MTa, NTa, KTa, wm, wn, wk, lda, ldb)
 
-    tiles = tiles_m * tiles_n * tiles_b
+
+def _weights(tile):
+    """The local weight of every tile dim (the product of the extents before it), and the tile's size."""
+    w, acc = [], 1
+    for d in tile:
+        w.append(acc)
+        acc *= d[0]
+    return w, acc
+
+
+def _splitk(t, sm_count, force_splitk):
     if force_splitk is not None:
-        splitk = max(1, min(int(force_splitk), steps_k))
+        splitk = max(1, min(int(force_splitk), t.steps_k))
     else:
         splitk = 1
-        if tiles < sm_count and steps_k >= 4:
-            splitk = min(steps_k, -(-2 * sm_count // tiles))
-        if variant == VAR_KRED:
-            splitk = min(steps_k, 4 * sm_count)
-        if variant in (VAR_DMMA_32x32, VAR_TF32_32x32) and tiles == 1:
-            splitk = min(steps_k, 2 * sm_count)  # two resident CTAs per SM
+        if t.tiles < sm_count and t.steps_k >= 4:
+            splitk = min(t.steps_k, -(-2 * sm_count // t.tiles))
+        if t.variant == VAR_KRED:
+            splitk = min(t.steps_k, 4 * sm_count)
+        if t.variant in (VAR_DMMA_32x32, VAR_TF32_32x32) and t.tiles == 1:
+            splitk = min(t.steps_k, 2 * sm_count)  # two resident CTAs per SM
     if splitk > 1:
-        per = -(-steps_k // splitk)
-        splitk = -(-steps_k // per)
-    if tiles * splitk >= 1 << 31:
+        per = -(-t.steps_k // splitk)
+        splitk = -(-t.steps_k // per)
+    if t.tiles * splitk >= 1 << 31:
         raise NotImplementedError("node needs more than 2^31 tiles")
+    return splitk
 
-    W = np.zeros(DESC_WORDS, dtype=np.int64)
-    W[W_MAGIC] = DESC_MAGIC
-    W[W_DTYPE] = DTYPE_CODES[dtype]
-    W[W_NTM], W[W_NTN], W[W_NTK] = len(tm), len(tn), len(tk)
-    W[W_NGM], W[W_NGN], W[W_NGK], W[W_NGB] = len(gm), len(gn), len(gk), len(gb)
-    W[W_MTA], W[W_NTA], W[W_KTA] = MTa, NTa, KTa
-    W[W_TILES_M], W[W_TILES_N], W[W_TILES_B], W[W_STEPS_K] = tiles_m, tiles_n, tiles_b, steps_k
-    W[W_SPLITK] = splitk
-    for base, p in ((W_PGM, pm), (W_PGN, pn), (W_PGK, pk)):
-        if p is None:
-            W[base:base + 4] = (-1, 0, 0, 0)
-        else:
-            W[base:base + 4] = p
-    W[W_NLDA], W[W_NLDB] = len(lda), len(ldb)
+
+def _layout_flags(dtype, t):
+    """Flags bits 1-5: what the tiling's layout lets the kernels assume."""
     # bit1: columns (2q, 2q+1) of every tile row are adjacent in C and 32-byte
     # aligned -> the kernels may use 256-bit stores (complex128 only)
-    expected, dense_n = 1, True
-    for d in tn:
-        if d[2] != expected:
-            dense_n = False
-            break
-        expected *= d[0]
-    pair_ok = (
-        dtype == "complex128" and dense_n and pn is None and NTa >= 2 and NTa % 2 == 0
-        and all(d[2] % 2 == 0 for d in tm)
-        and all(g[3] % 2 == 0 for g in gm) and all(g[3] % 2 == 0 for g in gn)
-        and all(g[4] % 2 == 0 for g in gb)
-    )
+    dense_n = all(d[2] == w for d, w in zip(t.tn, t.wn))
+    # (tile rows and the grid steps of m, n and batch move C by multiples of g elements)
+    aligned = lambda g: (all(d[2] % g == 0 for d in t.tm) and all(x[3] % g == 0 for x in t.gm + t.gn)  # noqa: E731
+                         and all(x[4] % g == 0 for x in t.gb))
+    pair_ok = dtype == "complex128" and dense_n and t.pn is None and t.NTa >= 2 and t.NTa % 2 == 0 and aligned(2)
     # bit2: all tile-grid extents are powers of two (Sycamore: always) -> the
     # producers decode tile indices with shifts/masks instead of idiv
     is_p2 = lambda e: e > 0 and (e & (e - 1)) == 0  # noqa: E731
-    grid_pow2 = all(is_p2(g[0]) for g in gm + gn + gb)
-    m_pow2 = all(is_p2(d[0]) for d in tm) and all(is_p2(g[0]) for g in gm)
-    if variant in TC05_VARIANTS:
-        # the wgmma kernel takes tiles of ONE shape: its native 128 x NT x 16, or smaller with
-        # the rest of the tensor-core tile as padding (KTa in steps of 4: whole wgmma k8 groups);
-        # below 40 % occupancy the mma.sync policy is the better choice
-        # (k padding is free -- the wgmmas of missing k8 groups are not issued -- so only rows and columns count)
-        occupancy = (MTa * NTa) / float(MT * NT)
-        exact = (MTa <= MT and NTa <= NT and KTa <= KT and KTa % 4 == 0 and dtype == "complex64"
-                 and occupancy >= 0.4 and steps_k <= 1024
-                 and (KTa >= 8 or steps_k == 1)  # many 4-wide k-steps: per-step overhead, mma.sync is better
-                 and all(p is None or p[1] % p[2] == 0 for p in (pm, pn, pk)))
-        if not exact:
-            fb = choose_variant(dtype, B, M, N, K, allow_dmma, allow_tc05=False)
-            return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=fb,
-                                   allow_dmma=allow_dmma, c_dense_elems=c_dense_elems,
-                                   force_splitk=force_splitk, precision=precision)
-    if variant == VAR_DOTSTREAM and (not (M == 1 and N == 1 and B == 1) or len(gk) > 40 or steps_k >= 1 << 31
-                                    or (pk is not None and pk[1] % pk[2] != 0)):
-        return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_KRED,
-                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
-                               precision=precision, wide_c=wide_c)
-    if variant == VAR_DOTSTREAM4 and (not (M <= 4 and N <= 4 and B == 1) or len(gk) > 40 or steps_k >= 1 << 31
-                                     or pm is not None or pn is not None
-                                     or (pk is not None and pk[1] % pk[2] != 0)
-                                     or not (accumulate or c_dense_elems == M * N)):
-        return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=VAR_SIMT_64x64,
-                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
-                               precision=precision, wide_c=wide_c)
-    if variant == VAR_DMMASTREAM and (pn is not None or pk is not None or (pm is not None and pm[1] % pm[2] != 0)
-                                      or tiles_n != 1 or steps_k != 1):
-        # ragged, or more dims than one tile holds: the staged tile choose_variant picks without the
-        # stream kernel (N <= 16: 256x16, as before N = 17..32 streamed)
-        fb = VAR_DMMA_256x16 if N <= 16 else choose_variant(dtype, B, M, N, K, allow_dmma, allow_stream=False)
-        return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count, variant=fb,
-                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems, force_splitk=force_splitk,
-                               precision=precision)
-    if variant == VAR_ROWSTREAM_K:
-        # exact tiles, and the k offsets must decompose as chunk_base[k // 8] + in_chunk[k % 8]
-        def _koff(e, col):
-            o = 0
-            for d in tk:
-                o += (e % d[0]) * d[col]
-                e //= d[0]
-            return o
-        ok8 = all(_koff(e, 1) == _koff(e - e % 8, 1) + _koff(e % 8, 1) for e in range(KTa))
-        if (not ok8 or pn is not None or pk is not None or (pm is not None and pm[1] % pm[2] != 0)
-                or DTYPE_SIZES[dtype] > 8 or not (N <= 8 and K <= 64 and B == 1 and M < 1 << 32)):
-            return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count,
-                                   variant=VAR_ROW_256x4 if N <= 4 else VAR_ROW_128x8,
-                                   allow_dmma=allow_dmma, c_dense_elems=c_dense_elems,
-                                   force_splitk=force_splitk, precision=precision)
-    if variant == VAR_ROWSTREAM and pm is not None and pm[1] % pm[2] != 0:
-        # ragged blocked m dim: fall back to the staged row policy
-        return build_pair_desc(dims, dtype, accumulate=accumulate, sm_count=sm_count,
-                               variant=VAR_ROW_256x4 if N <= 4 else VAR_ROW_128x8,
-                               allow_dmma=allow_dmma, c_dense_elems=c_dense_elems,
-                               force_splitk=force_splitk, precision=precision)
+    grid_pow2 = all(is_p2(g[0]) for g in t.gm + t.gn + t.gb)
+    m_pow2 = all(is_p2(d[0]) for d in t.tm) and all(is_p2(g[0]) for g in t.gm)
+
     # 8-byte element types: groups of 4 (bit4) / 2 (bit5) columns adjacent in C and
     # 32- / 16-byte aligned -> vector row stores in the streaming row kernel
-    def _cols_ok(g):
-        if variant in TC05_VARIANTS:
+    def cols_ok(g):
+        if t.variant in TC05_VARIANTS:
             # exact tiles: only the leading columns of a tile row have to be adjacent
-            run = 1
-            for d in tn:
-                if d[2] != run:
-                    break
-                run *= d[0]
+            run = next((w for d, w in zip(t.tn, t.wn) if d[2] != w), t.NTa)
             dense = run % g == 0
         else:
-            dense = dense_n and pn is None
-        return (
-            DTYPE_SIZES[dtype] == 8 and dense and NTa % g == 0
-            and all(d[2] % g == 0 for d in tm)
-            and all(x[3] % g == 0 for x in gm) and all(x[3] % g == 0 for x in gn)
-            and all(x[4] % g == 0 for x in gb)
-        )
+            dense = dense_n and t.pn is None
+        return DTYPE_SIZES[dtype] == 8 and dense and t.NTa % g == 0 and aligned(g)
 
-    # wgmma variants: if the A tile is made of long contiguous runs (dense prefix of
-    # the load order), the producers fetch whole runs with TMA bulk copies (bit6)
-    run_a, bulk_a = 1, False
-    if variant in TC05_VARIANTS:
-        for r_ in lda:
-            if r_[1] != run_a:
-                break
-            run_a *= r_[0]
-        rest = [r_[1] for r_ in lda if r_[1] >= run_a] + [g[2] for g in gm] + [g[2] for g in gk] + [g[2] for g in gb]
-        # (cp.async.bulk: 16-byte aligned source, size a multiple of 16 bytes; one run per
-        # producer thread -> at most 128 runs of >= 128 bytes)
-        bulk_a = (run_a >= 16 and run_a % 2 == 0 and (MTa * KTa) % run_a == 0
-                  and all(x % 2 == 0 for x in rest))
-        # chunk-stride padding of the A' images (x16 B): 16 consecutive elements of A's memory
-        # order -- the lanes of a half warp in the scatter pass -- should hit 16 different
-        # 8-byte bank pairs.  Element (r, kk) sits at (kk//2)*LBO + r*16 + (kk%2)*8 bytes.
-        def _conflicts(pad):
-            lbo, worst = MT * 16 + 16 * pad, 0
-            for half in range(2):
-                slots = {}
-                for e in range(16 * half, 16 * half + 16):
-                    r_ = kk_ = 0
-                    x = e
-                    for ext, _s, wr, wk_ in lda:
-                        r_ += (x % ext) * wr
-                        kk_ += (x % ext) * wk_
-                        x //= ext
-                    slot = (((kk_ // 2) * lbo + r_ * 16 + (kk_ % 2) * 8) >> 3) & 15
-                    slots[slot] = slots.get(slot, 0) + 1
-                worst += max(slots.values())
-            return worst
-        W[W_LBOPAD] = min((0, 1, 2, 4), key=_conflicts)
-    W[W_RUNA] = run_a
-    W[W_FLAGS] = ((1 if accumulate else 0) | (2 if pair_ok else 0) | (4 if grid_pow2 else 0)
-                  | (8 if m_pow2 else 0) | (16 if _cols_ok(4) else 0) | (32 if _cols_ok(2) else 0)
-                  | (64 if bulk_a else 0)
-                  | (FLAG_TF32_ONE_PASS if precision == "tf32" and variant in TF32_VARIANTS else 0)
-                  | (FLAG_WIDE_C if wide_c else 0))
-    W[W_VARIANT] = variant
-    W[W_CELEMS] = int(c_dense_elems)
+    return (2 if pair_ok else 0) | (4 if grid_pow2 else 0) | (8 if m_pow2 else 0) | (16 if cols_ok(4) else 0) \
+        | (32 if cols_ok(2) else 0)
 
-    def put(off, rows, width):
+
+def _wgmma_words(t):
+    """``(RUNA, bit6, LBOPAD)`` of a wgmma node."""
+    # if the A tile is made of long contiguous runs (dense prefix of the load order),
+    # the producers fetch whole runs with TMA bulk copies (bit6)
+    run_a = 1
+    for r_ in t.lda:
+        if r_[1] != run_a:
+            break
+        run_a *= r_[0]
+    rest = [r_[1] for r_ in t.lda if r_[1] >= run_a] + [g[2] for g in t.gm + t.gk + t.gb]
+    # (cp.async.bulk: 16-byte aligned source, size a multiple of 16 bytes; one run per
+    # producer thread -> at most 128 runs of >= 128 bytes)
+    bulk_a = (run_a >= 16 and run_a % 2 == 0 and (t.MTa * t.KTa) % run_a == 0
+              and all(x % 2 == 0 for x in rest))
+    # chunk-stride padding of the A' images (x16 B): 16 consecutive elements of A's memory
+    # order -- the lanes of a half warp in the scatter pass -- should hit 16 different
+    # 8-byte bank pairs.  Element (r, kk) sits at (kk//2)*LBO + r*16 + (kk%2)*8 bytes.
+    pos = []
+    for x in range(32):
+        r_ = kk_ = 0
+        for ext, _s, wr, wk_ in t.lda:
+            r_, kk_, x = r_ + (x % ext) * wr, kk_ + (x % ext) * wk_, x // ext
+        pos.append((r_, kk_))
+
+    def conflicts(pad):
+        lbo = VARIANT_TILES[t.variant][0] * 16 + 16 * pad
+        slots = [(((kk_ // 2) * lbo + r_ * 16 + (kk_ % 2) * 8) >> 3) & 15 for r_, kk_ in pos]
+        return sum(max(Counter(slots[h:h + 16]).values()) for h in (0, 16))
+    return run_a, bulk_a, min((0, 1, 2, 4), key=conflicts)
+
+
+def _pack(dtype, t, splitk, flags, run_a, lbopad, c_dense_elems):
+    W = np.zeros(DESC_WORDS, dtype=np.int64)
+    W[W_MAGIC] = DESC_MAGIC
+    W[W_DTYPE] = DTYPE_CODES[dtype]
+    W[W_NTM], W[W_NTN], W[W_NTK] = len(t.tm), len(t.tn), len(t.tk)
+    W[W_NGM], W[W_NGN], W[W_NGK], W[W_NGB] = len(t.gm), len(t.gn), len(t.gk), len(t.gb)
+    W[W_MTA], W[W_NTA], W[W_KTA] = t.MTa, t.NTa, t.KTa
+    W[W_TILES_M], W[W_TILES_N], W[W_TILES_B], W[W_STEPS_K] = t.tiles_m, t.tiles_n, t.tiles_b, t.steps_k
+    W[W_SPLITK] = splitk
+    for base, p in ((W_PGM, t.pm), (W_PGN, t.pn), (W_PGK, t.pk)):
+        W[base:base + 4] = (-1, 0, 0, 0) if p is None else p
+    W[W_NLDA], W[W_NLDB] = len(t.lda), len(t.ldb)
+    W[W_FLAGS], W[W_VARIANT], W[W_CELEMS], W[W_RUNA], W[W_LBOPAD] = flags, t.variant, int(c_dense_elems), run_a, lbopad
+    for off, rows, width in ((OFF_TM, t.tm, 3), (OFF_TN, t.tn, 3), (OFF_TK, t.tk, 3), (OFF_GM, t.gm, 4),
+                             (OFF_GN, t.gn, 4), (OFF_GK, t.gk, 4), (OFF_GB, t.gb, 5), (OFF_LDA, t.lda, 4),
+                             (OFF_LDB, t.ldb, 4)):
         for i, r in enumerate(rows):
             W[off + i * width: off + (i + 1) * width] = r
-
-    put(OFF_TM, tm, 3)
-    put(OFF_TN, tn, 3)
-    put(OFF_TK, tk, 3)
-    put(OFF_GM, gm, 4)
-    put(OFF_GN, gn, 4)
-    put(OFF_GK, gk, 4)
-    put(OFF_GB, gb, 5)
-    put(OFF_LDA, lda, 4)
-    put(OFF_LDB, ldb, 4)
-    return PairPlan(W, variant, (B, M, N, K), swapped, tiles, splitk)
+    return W
 
 
 # ---------------------------------------------------------------------------
