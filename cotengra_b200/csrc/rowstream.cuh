@@ -135,6 +135,12 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
 #pragma unroll
       for (int kk = 0; kk < KMAX; ++kk)
         if (kk < K) a[i][kk] = A[oa[i] + akoff[kk]];
+    // 16-byte types read s_B afresh for every row: through an index the compiler cannot see
+    // through, which keeps it from hoisting all KMAX x NMAX reads out of the row loop (for N = K = 8,
+    // 64 complex128 values = 256 registers: ptxas spilled them to a 984-byte stack frame and the
+    // m20 slice's 2^23 x 8 x 8 nodes streamed at 0.56 TB/s)
+    [[maybe_unused]] int sb0 = 0;
+    if constexpr (!BREG && sizeof(T) >= 16) asm volatile("" : "+r"(sb0));
     // columns in chunks of CH: 16-byte types with 8 columns would otherwise hold 8 accumulators
     // + 8 operand elements per row (114 registers, 2 blocks / SM; ncu: 25 % of the warps resident,
     // short-scoreboard bound) -- 4 + 8 fit three blocks
@@ -157,7 +163,7 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
               if constexpr (BREG) {
                 mac(acc[c], a[i][kk], breg[kk][c0 + c]);
               } else {
-                if (c0 + c < N) mac(acc[c], a[i][kk], s_B[kk * NMAX + c0 + c]);
+                if (c0 + c < N) mac(acc[c], a[i][kk], s_B[sb0 + kk * NMAX + c0 + c]);
               }
             }
           }
