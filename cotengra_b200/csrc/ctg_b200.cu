@@ -137,16 +137,27 @@ int launch_gett_policy(const int64_t* h, const int64_t* d, const void* A, const 
   return CTGB_OK;
 }
 
+unsigned long long stream_row_count(const int64_t* h) {
+  return (unsigned long long)h[W_MTA] * (unsigned long long)h[W_TILES_M];
+}
+// What the row-stream and DMMA stream kernels take (stream_rows.cuh): N <= nmax, K <= kmax,
+// one n tile, one batch tile, one k-step and no split-K, whole m blocks, no blocked n or k dim,
+// and fewer than 2^32 rows (a row index is 32 bits wide)
+bool stream_desc_fits(const int64_t* h, int nmax, int kmax) {
+  return h[W_NTA] <= nmax && h[W_KTA] <= kmax && h[W_TILES_N] == 1 && h[W_TILES_B] == 1 && h[W_STEPS_K] == 1 &&
+         h[W_SPLITK] == 1 && !(h[W_PGM] >= 0 && (h[W_MFULL] % h[W_MTEXT]) != 0) && h[W_PGN] < 0 && h[W_PGK] < 0 &&
+         stream_row_count(h) < (1ull << 32);
+}
+// fused strip_exponent (scale the product or measure C's factor): the STRIP instantiations
+bool desc_stripped(const int64_t* h) { return h[W_SCALE_A] != 0 || h[W_FACTOR_C] != 0; }
+
 template <typename T>
 int launch_rowstream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
   DevInfo& di = devinfo();
   if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
   const int N = (int)h[W_NTA], K = (int)h[W_KTA];
-  if (N > 8 || K > 8 || h[W_TILES_N] != 1 || h[W_TILES_B] != 1 || h[W_STEPS_K] != 1 || h[W_SPLITK] != 1 ||
-      h[W_PGM] >= 0 && (h[W_MFULL] % h[W_MTEXT]) != 0 || h[W_PGN] >= 0 || h[W_PGK] >= 0)
-    return fail(CTGB_E_VALUE, "descriptor does not fit the row-stream kernel");
-  const unsigned long long M = (unsigned long long)h[W_MTA] * (unsigned long long)h[W_TILES_M];
-  if (M >= (1ull << 32)) return fail(CTGB_E_VALUE, "too many rows for the row-stream kernel");
+  if (!stream_desc_fits(h, 8, 8)) return fail(CTGB_E_VALUE, "descriptor does not fit the row-stream kernel");
+  const unsigned long long M = stream_row_count(h);
   unsigned long long blocks = (M + 255) / 256;
   const unsigned long long cap = (unsigned long long)di.sms * 8;
   if (blocks > cap) blocks = cap;
@@ -154,7 +165,7 @@ int launch_rowstream(const int64_t* h, const int64_t* d, const void* A, const vo
   const T* a = (const T*)A;
   const T* b = (const T*)B;
   T* c = (T*)C;
-  const bool strip = h[W_SCALE_A] != 0 || h[W_FACTOR_C] != 0;  // fused strip_exponent: separate instantiations
+  const bool strip = desc_stripped(h);
   if (N <= 4 && K <= 4) {
     if (strip) rowstream_kernel<T, 4, 4, true, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
     else rowstream_kernel<T, 4, 4, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
@@ -177,9 +188,8 @@ int launch_rowstream_longk(const int64_t* h, const int64_t* d, const void* A, co
   if constexpr (sizeof(T) > 8) {
     return fail(CTGB_E_VALUE, "the long-k row stream takes 8-byte and narrower element types");
   } else {
-    const int N = (int)h[W_NTA], K = (int)h[W_KTA];
-    if (N > RSK_NMAX || K > RSK_KMAX || h[W_TILES_N] != 1 || h[W_TILES_B] != 1 || h[W_STEPS_K] != 1 ||
-        h[W_SPLITK] != 1 || h[W_PGM] >= 0 && (h[W_MFULL] % h[W_MTEXT]) != 0 || h[W_PGN] >= 0 || h[W_PGK] >= 0)
+    const int K = (int)h[W_KTA];
+    if (!stream_desc_fits(h, RSK_NMAX, RSK_KMAX))
       return fail(CTGB_E_VALUE, "descriptor does not fit the long-k row-stream kernel");
     // offset(k) must decompose as chunk_base[k / 8] + in_chunk[k % 8]
     auto koff = [&](long long e) {
@@ -192,13 +202,12 @@ int launch_rowstream_longk(const int64_t* h, const int64_t* d, const void* A, co
     };
     for (long long e = 0; e < K; ++e)
       if (koff(e) != koff(e - e % 8) + koff(e % 8)) return fail(CTGB_E_VALUE, "k offsets do not split into chunks of 8");
-    const unsigned long long M = (unsigned long long)h[W_MTA] * (unsigned long long)h[W_TILES_M];
-    if (M >= (1ull << 32)) return fail(CTGB_E_VALUE, "too many rows for the row-stream kernel");
+    const unsigned long long M = stream_row_count(h);
     unsigned long long blocks = (M + 511) / 512;
     const unsigned long long cap = (unsigned long long)di.sms * 6;
     if (blocks > cap) blocks = cap;
     if (blocks == 0) return CTGB_OK;
-    if (h[W_SCALE_A] != 0 || h[W_FACTOR_C] != 0)
+    if (desc_stripped(h))
       rowstream_longk_kernel<T, true><<<(unsigned)blocks, 256, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C);
     else
       rowstream_longk_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C);
@@ -252,13 +261,10 @@ struct DsLaunch {
 };
 
 int dmmastream_launch_config(const int64_t* h, int sms, DsLaunch& lc) {
-  const int N = (int)h[W_NTA], K = (int)h[W_KTA];
-  if (h[W_DTYPE] != CTGB_C128 || N > 64 || K > (N <= 32 ? DS_KMAX : DS_KMAX_WIDE) || h[W_TILES_N] != 1 ||
-      h[W_TILES_B] != 1 || h[W_STEPS_K] != 1 || h[W_SPLITK] != 1 ||
-      h[W_PGM] >= 0 && (h[W_MFULL] % h[W_MTEXT]) != 0 || h[W_PGN] >= 0 || h[W_PGK] >= 0)
+  const int N = (int)h[W_NTA];
+  if (h[W_DTYPE] != CTGB_C128 || !stream_desc_fits(h, 64, N <= 32 ? DS_KMAX : DS_KMAX_WIDE))
     return fail(CTGB_E_VALUE, "descriptor does not fit the DMMA stream kernel");
-  const unsigned long long M = (unsigned long long)h[W_MTA] * (unsigned long long)h[W_TILES_M];
-  if (M >= (1ull << 32)) return fail(CTGB_E_VALUE, "too many rows for the DMMA stream kernel");
+  const unsigned long long M = stream_row_count(h);
   // 64 accumulator doubles per lane at most: 32-row warp blocks up to N = 32, 16-row ones beyond
   lc.nj = N <= 8 ? 1 : N <= 16 ? 2 : N <= 32 ? 4 : 8;
   lc.rows = lc.nj <= 4 ? 32 : 16;
@@ -282,7 +288,7 @@ int launch_dmmastream(const int64_t* h, const int64_t* d, const void* A, const v
   DsLaunch lc;
   if (int rc = dmmastream_launch_config(h, di.sms, lc)) return rc;
   if (lc.blocks == 0) return CTGB_OK;
-  const bool strip = h[W_SCALE_A] != 0 || h[W_FACTOR_C] != 0;  // fused strip_exponent: separate instantiations
+  const bool strip = desc_stripped(h);
   const double2 *a = (const double2*)A, *b = (const double2*)B;
   double2* c = (double2*)C;
   const unsigned blocks = (unsigned)lc.blocks;

@@ -9,10 +9,11 @@
 // barriers in the loop: the warps of an SM drift apart, so loads, DMMAs and stores of different row blocks overlap by themselves
 // -- which the staged 256x16 policy could not do (all consumer warps share one phase: ncu
 // showed its N=16 K=16 node with compute and HBM time adding up instead of overlapping).
+// The offset tables and the row decoder are in stream_rows.cuh.
 // (included inside namespace ctgb)
 #pragma once
 
-constexpr int DS_KMAX = 64;       // k rows of the s_B copy for NJ <= 4
+constexpr int DS_KMAX = 64;       // k rows of the s.B copy for NJ <= 4
 constexpr int DS_KMAX_WIDE = 32;  // ... for NJ = 8 (64 x 64 complex doubles would be 64 KB of static shared memory)
 
 // NJ = column fragments (N <= 8*NJ), RG = 8-row groups per warp block (4: 32 rows, 2: 16 rows -- one
@@ -26,68 +27,13 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
                   double2* __restrict__ C) {
   static_assert(RG == 2 || RG == 4, "a warp block is one or two m16 fragment pairs");
   constexpr int DS_NMAX = NJ * 8, DS_KB = NJ <= 4 ? DS_KMAX : DS_KMAX_WIDE, ROWS = RG * 8;
-  __shared__ long long s_akoff[DS_KMAX], s_bkoff[DS_KMAX], s_bnoff[DS_NMAX], s_cnoff[DS_NMAX];
-  __shared__ long long s_msA[RS_MAXDIMS], s_msC[RS_MAXDIMS];
-  __shared__ unsigned s_mext[RS_MAXDIMS];
-  __shared__ double2 s_B[DS_KB * DS_NMAX];  // [k][n], zero beyond (K, N); the launcher keeps K <= DS_KB
+  // s.B: [k][n], zero beyond (K, N); the launcher keeps K <= DS_KB
+  STREAM_TABLES(double2, DS_KMAX, DS_NMAX, DS_KB);
   const int tid = threadIdx.x, lane = tid & 31;
-  const int n_tm = (int)D[W_NTM], n_gm = (int)D[W_NGM], n_tk = (int)D[W_NTK], n_tn = (int)D[W_NTN];
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
-  const int n_m = n_tm + n_gm;
-  const bool accumulate = (D[W_FLAGS] & 1) != 0;
-  const bool pair_ok = (D[W_FLAGS] & 2) != 0 && !accumulate;
-  const bool pow2 = (D[W_FLAGS] & 8) != 0;  // every m dim (tile and grid) is a power of two
-  // m dims in enumeration order: tile dims (dim 0 fastest) then grid dims
-  for (int d = tid; d < n_m; d += blockDim.x) {
-    if (d < n_tm) {
-      const int64_t* L = D + OFF_TM + d * 3;
-      s_mext[d] = (unsigned)L[0];
-      s_msA[d] = L[1];
-      s_msC[d] = L[2];
-    } else {
-      const int64_t* G = D + OFF_GM + (d - n_tm) * 4;
-      s_mext[d] = (unsigned)G[0];
-      s_msA[d] = G[2];
-      s_msC[d] = G[3];
-    }
-  }
-  if (tid < DS_KMAX) {
-    long long a = 0, b = 0;
-    if (tid < K) {
-      unsigned e = tid;
-      for (int d = 0; d < n_tk; ++d) {
-        const int64_t* L = D + OFF_TK + d * 3;
-        const unsigned ext = (unsigned)L[0];
-        a += (long long)(e % ext) * L[1];
-        b += (long long)(e % ext) * L[2];
-        e /= ext;
-      }
-    }
-    s_akoff[tid] = a;
-    s_bkoff[tid] = b;
-  }
-  if (tid >= 32 && tid < 32 + DS_NMAX) {
-    const int c = tid - 32;
-    long long b = 0, o = 0;
-    if (c < N) {
-      unsigned e = c;
-      for (int d = 0; d < n_tn; ++d) {
-        const int64_t* L = D + OFF_TN + d * 3;
-        const unsigned ext = (unsigned)L[0];
-        b += (long long)(e % ext) * L[1];
-        o += (long long)(e % ext) * L[2];
-        e /= ext;
-      }
-    }
-    s_bnoff[c] = b;
-    s_cnoff[c] = o;
-  }
-  __syncthreads();
-  for (int i = tid; i < DS_KB * DS_NMAX; i += blockDim.x) {
-    const int kk = i / DS_NMAX, c = i % DS_NMAX;
-    s_B[i] = (kk < K && c < N) ? B[s_bkoff[kk] + s_bnoff[c]] : make_double2(0.0, 0.0);
-  }
-  __syncthreads();
+  const int n_m = s.load(D, B, K, N);
+  // (the flags after the tables: read before them, ptxas gives <8, 2, true> 248 registers, not 244)
+  const StreamFlags f = stream_flags<double2>(D);
 
   [[maybe_unused]] StripCtx sctx;  // fused strip_exponent: its own instantiation (register-bound loop)
   if constexpr (STRIP) sctx = strip_begin(D);
@@ -106,27 +52,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
     for (int i = 0; i < RG; ++i) {
       const unsigned long long m = blk * ROWS + (unsigned)(i * 8 + frow);
       live[i] = m < M;
-      unsigned e = live[i] ? (unsigned)m : 0u;
-      long long xa = 0, xc = 0;
-      if (pow2) {
-        for (int d = 0; d < n_m; ++d) {
-          const unsigned ext = s_mext[d];
-          const unsigned dig = e & (ext - 1);
-          e >>= 31 - __clz(ext);
-          xa += (long long)dig * s_msA[d];
-          xc += (long long)dig * s_msC[d];
-        }
-      } else {
-        for (int d = 0; d < n_m; ++d) {
-          const unsigned ext = s_mext[d];
-          const unsigned dig = e % ext;
-          e /= ext;
-          xa += (long long)dig * s_msA[d];
-          xc += (long long)dig * s_msC[d];
-        }
-      }
-      oa[i] = xa;
-      oc[i] = xc;
+      s.row(n_m, f.pow2, live[i] ? (unsigned)m : 0u, oa[i], oc[i]);
     }
     double re[RG][NJ][2], im[RG][NJ][2];
 #pragma unroll
@@ -142,7 +68,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
 #pragma unroll
       for (int k4 = 0; k4 < 4; ++k4) {
         const int kk = kc * 16 + k4 * 4 + fk;
-        const long long ko = s_akoff[kk & (DS_KMAX - 1)];
+        const long long ko = s.akoff[kk & (DS_KMAX - 1)];
         const bool kin = kk < K;
 #pragma unroll
         for (int i = 0; i < RG; ++i) {
@@ -157,7 +83,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
         // B fragment: lane holds B[k = .. + fk][n = j*8 + frow]
         double2 b[NJ];
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) b[j] = s_B[(kc * 16 + k4 * 4 + fk) * DS_NMAX + j * 8 + frow];
+        for (int j = 0; j < NJ; ++j) b[j] = s.B[(kc * 16 + k4 * 4 + fk) * DS_NMAX + j * 8 + frow];
 #pragma unroll
         for (int i = 0; i < RG; i += 2)
 #pragma unroll
@@ -180,6 +106,8 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
             if (j < n8s) dmma16x8x4(im[i][j], im[i + 1][j], a[i][k4].y, a[i + 1][k4].y, b[j].x);
       }
     }
+    // (not strip_row of stream_rows.cuh: the accumulators are split re / im DMMA fragments, which
+    // it would take as double2 copies, and scaling happens per column pair in the store below)
     if constexpr (STRIP) {
       if (!sctx.scale) {
         // max|C|: integer scan over the accumulators, then (rarely) the values (see gett_ws.cuh)
@@ -218,14 +146,14 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
             if (c + 1 < N) v1 = strip_apply(sctx, v1);
           }
         }
-        if (pair_ok) {
-          store_pair_of(crow + s_cnoff[c], v0, v1);
+        if (f.pair_ok) {
+          store_pair_of(crow + s.cnoff[c], v0, v1);
         } else {
-          double2* p0 = crow + s_cnoff[c];
-          *p0 = accumulate ? add_of(*p0, v0) : v0;
+          double2* p0 = crow + s.cnoff[c];
+          *p0 = f.accumulate ? add_of(*p0, v0) : v0;
           if (c + 1 < N) {
-            double2* p1 = crow + s_cnoff[c + 1];
-            *p1 = accumulate ? add_of(*p1, v1) : v1;
+            double2* p1 = crow + s.cnoff[c + 1];
+            *p1 = f.accumulate ? add_of(*p1, v1) : v1;
           }
         }
       }

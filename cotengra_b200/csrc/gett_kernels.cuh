@@ -653,6 +653,7 @@ struct DmmaPolicy {
 };
 
 #include "tf32_policy.cuh"
+#include "stream_rows.cuh"
 #include "rowstream.cuh"
 #include "dmmastream.cuh"
 #include "dotstream.cuh"
