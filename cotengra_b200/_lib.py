@@ -42,6 +42,7 @@ EXPORTS = (
     "ctgb_probe_fp64_peaks",
     "ctgb_tc05_launch_config",
     "ctgb_dmmastream_launch_config",
+    "ctgb_absorb_root",
 )
 TC05_LAUNCH_FIELDS = ("b_stat", "nb", "sa", "grid", "smem", "tm_rank", "bulk", "chunk_steps", "chunks")
 DMMASTREAM_LAUNCH_FIELDS = ("nj", "rows", "grid")
@@ -125,6 +126,7 @@ def load():
     ]
     lib.ctgb_contract_pair.argtypes = [C.c_void_p] * 5
     lib.ctgb_reduce_single.argtypes = [C.c_void_p] * 4
+    lib.ctgb_absorb_root.argtypes = [C.c_void_p] * 6
     lib.ctgb_plan_create.argtypes = [C.POINTER(CtgbPlanDesc), C.POINTER(C.c_void_p)]
     lib.ctgb_plan_set_chunk_desc.argtypes = [C.c_void_p, C.c_void_p]
     lib.ctgb_plan_set_scale_slots.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]

@@ -205,7 +205,8 @@ class _Executor:
     """
 
     def __init__(self, contractions, inputs, output, size_dict, sliced, dtype, strip_exponent=False, device=None,
-                 vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, accumulate="native", **plan_opts):
+                 vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, accumulate="native", absorb_root=False,
+                 **plan_opts):
         torch = _torch()
         self._ir, self._plan_opts = contractions, plan_opts
         # the program without its slicing: the positional head of ``ExecPlan`` and ``VjpPlan``
@@ -213,7 +214,8 @@ class _Executor:
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
         with torch.cuda.device(self.device):
             self.plan = ExecPlan(*self._program, sliced, dtype=dtype, strip_exponent=strip_exponent,
-                                 precision=precision, accumulate=accumulate, **plan_opts).create()
+                                 precision=precision, accumulate=accumulate, absorb_root=absorb_root,
+                                 **plan_opts).create()
         self.dtype = self.plan.dtype
         self.precision = precision
         self.accumulate = accumulate
@@ -402,7 +404,8 @@ class TreeExecutor(_Executor):
         ir = self.exec_spec.contractions() if contractions is None else contractions
         super().__init__(ir, spec.inputs, spec.output, spec.size_dict, spec.sliced, dtype,
                          strip_exponent=strip_exponent, device=device, vjp_max_bytes=vjp_max_bytes,
-                         precision=precision, stripped_grad=stripped_grad, accumulate=accumulate, **plan_opts)
+                         precision=precision, stripped_grad=stripped_grad, accumulate=accumulate,
+                         absorb_root=bool(fuse) and contractions is None, **plan_opts)
         self._ref_work = None
 
     @property

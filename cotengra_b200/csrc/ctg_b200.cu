@@ -303,6 +303,33 @@ int launch_dmmastream(const int64_t* h, const int64_t* d, const void* A, const v
   return CTGB_OK;
 }
 
+// absorb-root node (absorbdot.cuh): one CTA per SM at most, each taking an even share of the k' units
+int launch_absorb_root(const int64_t* h, const int64_t* d, const void* A, const void* Bs, const void* V, void* C,
+                       cudaStream_t st) {
+  if (h[W_DTYPE] != CTGB_C128) return fail(CTGB_E_VALUE, "the absorb-root kernel is complex128 only");
+  if (h[AB_M] < 1 || h[AB_M] > 32 || h[AB_N] < 1 || h[AB_N] > 32 || h[AB_K] < 1 || h[AB_K] > 16 || h[AB_C] < 1 ||
+      h[AB_C] > h[AB_CCP] || h[AB_CCP] % 32 || h[AB_CCP] > 128 || (h[AB_KL] != 1 && h[AB_KL] != 2) || h[AB_NG] < 0 || h[AB_NG] > AB_MAXG || h[AB_UNITS] < 1 || h[AB_UNITS] >= (1ll << 32) ||
+      h[AB_GRID] < 1 || h[AB_GRID] > h[AB_UNITS] || h[AB_GRID] > (1 << 20))
+    return fail(CTGB_E_VALUE, "absorb-root descriptor out of range");
+  for (int mb = 0; mb < 4; ++mb)
+    if (h[AB_TBCK + mb] < 0 || (h[AB_TBCK + mb] + 1) * h[AB_CCP] > 128)
+      return fail(CTGB_E_VALUE, "absorb-root descriptor out of range");
+  if (!(h[W_FLAGS] & 1)) {
+    if (h[W_CELEMS] <= 0) return fail(CTGB_E_VALUE, "absorb-root into a strided C needs accumulate");
+    CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)h[W_CELEMS] * sizeof(double2), st));
+  }
+  static bool attr = false;
+  if (!attr) {
+    CUDA_TRY(cudaFuncSetAttribute(absorbdot_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AB_SMEM));
+    attr = true;
+  }
+  absorbdot_kernel<<<(unsigned)h[AB_GRID], AB_THREADS, AB_SMEM, st>>>(d, (const double2*)A, (const double2*)Bs,
+                                                                      (const double2*)V, (double2*)C);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  CUDA_TRY(cudaGetLastError());
+  return CTGB_OK;
+}
+
 std::atomic<int64_t> g_tmap_launches{0};
 
 // Tensor map for the A tile of the wgmma kernel.  The tile is described in A's memory order by
@@ -600,6 +627,7 @@ int launch_gett_typed(const int64_t* h, const int64_t* d, const void* A, const v
 
 int launch_gett(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
   if (h[W_MAGIC] != DESC_MAGIC) return fail(CTGB_E_VALUE, "bad pair descriptor magic");
+  if (h[W_VARIANT] == VAR_ABSORB_ROOT) return fail(CTGB_E_VALUE, "an absorb-root node has three operands (ctgb_absorb_root)");
   switch ((int)h[W_DTYPE]) {
     case CTGB_F32: return launch_gett_typed<float>(h, d, A, B, C, st);
     case CTGB_F64: return launch_gett_typed<double>(h, d, A, B, C, st);
@@ -1042,6 +1070,18 @@ int ctgb_contract_pair(const int64_t* desc, const void* A, const void* B, void* 
   return rc;
 }
 
+int ctgb_absorb_root(const int64_t* desc, const void* A, const void* Bs, const void* V, void* C, void* stream) {
+  if (!desc || desc[0] != DESC_MAGIC || desc[W_VARIANT] != VAR_ABSORB_ROOT)
+    return fail(CTGB_E_VALUE, "not an absorb-root descriptor");
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t* d = nullptr;
+  CUDA_TRY(cudaMallocAsync((void**)&d, DESC_WORDS * sizeof(int64_t), st));
+  CUDA_TRY(cudaMemcpyAsync(d, desc, DESC_WORDS * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  int rc = launch_absorb_root(desc, d, A, Bs, V, C, st);
+  cudaFreeAsync(d, st);
+  return rc;
+}
+
 int ctgb_reduce_single(const int64_t* desc, const void* X, void* out, void* stream) {
   if (!desc) return fail(CTGB_E_VALUE, "null descriptor");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1086,6 +1126,10 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     if (n.phase < 0 || n.phase > 3) return refuse("bad node phase");
     auto bad = [&](int t) { return t < 0 || t >= pd->n_tensors; };
     if (bad(n.a) || bad(n.c) || (n.kind == 0 && bad(n.b))) return refuse("node refers to a missing tensor");
+    if (n.kind == 0 && n.desc[W_VARIANT] == VAR_ABSORB_ROOT) {
+      if (bad((int)n.desc[AB_BS_SLOT])) return refuse("node refers to a missing tensor");
+      if (pd->strip_exponent) return refuse("an absorb-root node runs in unstripped plans only");
+    }
     p->backward |= n.phase >= 2;
     if (n.is_root) p->root = i;
     if (n.kind == 0 && (n.desc[W_FLAGS] & FLAG_WIDE_C)) {
@@ -1346,7 +1390,11 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
           return r;
         A = p->d_bscale + (A - base);
       }
-      if (int r = launch_node(n.kind, h, d, A, B, C, st)) return r;
+      if (n.kind == 0 && h[W_VARIANT] == VAR_ABSORB_ROOT) {
+        if (int r = launch_absorb_root(h, d, A, resolve((int)h[AB_BS_SLOT], out_off), B, C, st)) return r;
+      } else if (int r = launch_node(n.kind, h, d, A, B, C, st)) {
+        return r;
+      }
       // contract.py:816-829 strips after every *pairwise* node (single-operand preprocessing
       // steps `continue` before reaching it, :792-796).  The kernels do it in their epilogues
       // (scale by the operands' factors, record max|C|: gett_kernels.cuh StripCtx); only nodes

@@ -92,9 +92,39 @@ enum : int {
   VAR_ROWSTREAM_K = 19,    // N <= 8, 8 < K <= 64, 8-byte and narrower types: the row stream in chunks of 8 k
   VAR_DMMA_32x32 = 18,     // fp64 DMMA, one 32 x 32 tile with split-K over all SMs, two CTAs per SM: a few
                            // peeled stem tails times the other stem (M, N <= 32 over K ~ 2^25)
-  VAR_TF32_32x32 = 20      // its float32 / complex64 counterpart (3xTF32 mma.sync); chosen by VJP plans only,
+  VAR_TF32_32x32 = 20,     // its float32 / complex64 counterpart (3xTF32 mma.sync); chosen by VJP plans only,
                            // for the small-result backward nodes of stem absorptions
+  VAR_ABSORB_ROOT = 21     // complex128: a stem absorption X = A.Bs folded into the DMMA_32x32 product R = X.V
+                           // that is X's only reader (absorbdot.cuh); three operands, its own word layout below
 };
+
+// ---- absorb-root descriptor (VAR_ABSORB_ROOT) --------------------------------
+// R[m,n] (+)= sum_{k',c} (sum_k A[m,k',k] Bs[k,c]) V[k',c,n].  Same size and magic as a pair
+// descriptor; W_DTYPE, W_FLAGS (bit0: accumulate into C), W_VARIANT and W_CELEMS keep their meaning.
+constexpr int AB_MAXG = 32;  // grid k' dims (one lane each)
+enum : int {
+  AB_M = 2, AB_N = 3, AB_K = 4, AB_C = 5,  // row slots, N <= 32, K <= 16, contracted c (CC)
+  AB_KL = 6,                               // extent of the tile k' dim (1 or 2)
+  AB_NG = 7,                               // grid k' dims
+  AB_UNITS = 8,                            // k' units (product of the grid extents)
+  AB_KLA = 9, AB_KLV = 10,                 // strides of the tile k' dim in A and V
+  AB_GRID = 11,                            // CTAs (units split evenly among them)
+  AB_BS_SLOT = 12,                         // in a plan: the tensor slot of Bs (the node's a, b, c are A, V, C)
+  AB_CCP = 13,                             // CC rounded up to 32; Bs column of (ck, cc) is ck * CCP + cc, <= 128
+  // R's row r = mb * 8 + g (8-row block mb) is an A row and a kept column ck(mb) of Bs (one per block)
+  AB_TMA = W_HDR,             // 32: A offset of row r      AB_TMC: C offset of row r (-1: no row)
+  AB_TMC = AB_TMA + 32,
+  AB_TNV = AB_TMC + 32,       // 32: V offset of column n   AB_TNC: C offset of column n
+  AB_TNC = AB_TNV + 32,
+  AB_TKA = AB_TNC + 32,       // 16: A offset of k          AB_TKB: Bs offset of k
+  AB_TKB = AB_TKA + 16,
+  AB_TCB = AB_TKB + 16,       // 128: Bs offset of column ck * CCP + cc (-1: none)   AB_TCV: V offset of cc
+  AB_TCV = AB_TCB + 128,
+  AB_G = AB_TCV + 128,        // AB_MAXG x (ext, div, sA, sV), unit digit = u / div % ext
+  AB_TBCK = AB_G + AB_MAXG * 4,  // 4: ck of row block mb
+  AB_WORDS = AB_TBCK + 4
+};
+static_assert(AB_WORDS <= DESC_WORDS, "absorb-root words fit a pair descriptor");
 
 // ---- single-operand descriptor (cotengra/contract.py:332-361) -------------
 // out[o] = sum_s X[off_o(o) + off_s(s)], out written at its own strides.

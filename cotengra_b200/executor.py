@@ -164,7 +164,7 @@ def layout(sched, reserve=0):
         c = nd["c"]
         if c.first_use is None:
             c.first_use = zero_pos if c.kind == K_HACC else pos
-        for s in (nd["a"], nd["b"]):
+        for s in (nd["a"], nd["b"], nd.get("d")):
             if s is None:
                 continue
             s.last_use = max(s.last_use, pos)
@@ -189,7 +189,7 @@ def layout(sched, reserve=0):
 
 def _slots(sched):
     """The slots of a schedule in order of first appearance."""
-    return list(dict.fromkeys(t for nd in sched if nd is not None for t in (nd["a"], nd["b"], nd["c"])
+    return list(dict.fromkeys(t for nd in sched if nd is not None for t in (nd["a"], nd["b"], nd.get("d"), nd["c"])
                               if t is not None))
 
 
@@ -223,7 +223,9 @@ class _DevicePlan:
                 ct[i].slice_stride = C.cast(st, C.POINTER(C.c_int64))
         cn = (_lib.CtgbNode * max(len(self.nodes), 1))()
         for i, nd in enumerate(self.nodes):
-            words = np.ascontiguousarray(nd["words"], dtype=np.int64)
+            words = np.array(nd["words"], dtype=np.int64)
+            if nd.get("d") is not None:
+                words[lowering.AB_BS_SLOT] = slot[id(nd["d"])]
             keep.append(words)
             cn[i].kind = nd["kind"]
             cn[i].a = slot[id(nd["a"])]
@@ -316,11 +318,15 @@ class ExecPlan(_DevicePlan):
         adds into the output itself, any other root stores its slice densely in the workspace and one
         extra launch folds it in through the chunk descriptor.  For float64 / complex128 it is
         ``"native"``.
+    absorb_root : fold a complex128 stem absorption ``X = A . Bs`` into the ``DMMA_32x32`` product
+        ``R = X . V`` that reads it next (``lowering.build_absorb_desc``), so that X is never stored:
+        one ``VAR_ABSORB_ROOT`` node reads A, Bs and V and writes R.  Off by default: the plan is then
+        node for node the reference's sequence.  Not with ``strip_exponent`` or a forced ``variant``.
     """
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None, precision="3xtf32", accumulate="native"):
+                 variant=None, precision="3xtf32", accumulate="native", absorb_root=False):
         self.dtype = dtype_name(dtype)
         self.precision = check_precision(precision, self.dtype)
         self.esize = DTYPE_SIZES[self.dtype]
@@ -338,6 +344,8 @@ class ExecPlan(_DevicePlan):
             except Exception:
                 sm_count = 132  # H100 SXM
         self.sm_count = sm_count
+        self.absorb_root = bool(absorb_root) and self.dtype == "complex128" and not self.strip_exponent \
+            and variant is None
         self._build(hoist, allow_dmma, variant)
 
     # ------------------------------------------------------------------ build
@@ -447,9 +455,11 @@ class ExecPlan(_DevicePlan):
                         max(math.prod(dims.out_shape), 1) * self.esize, variant=A.variant or Bt.variant)
             a, b = (Bt, A) if plan.swapped else (A, Bt)
             nodes.append(dict(kind=0, a=a, b=b, c=dst, words=plan.words, root=is_root, plan=plan,
-                              sizes=plan.sizes, dims=dims, acc=acc, dense=dense))
+                              sizes=plan.sizes, dims=dims, acc=acc, dense=dense, terms=(A, Bt)))
             tensors.append(dst)
             cur[p] = dst
+            if self.absorb_root:
+                self._absorb(nodes, tensors)
 
         if not nodes:
             raise ValueError("empty contraction program")
@@ -458,7 +468,7 @@ class ExecPlan(_DevicePlan):
             nodes[-1]["c"].kind = K_OUTPUT  # the root writes the output accumulator directly
         # invariance: hoisted results live in the persistent arena
         for nd in nodes:
-            srcs = [nd["a"]] + ([nd["b"]] if nd["b"] is not None else [])
+            srcs = [t for t in (nd["a"], nd["b"], nd.get("d")) if t is not None]
             nd["invariant"] = bool(hoist and not nd["root"] and not any(s.variant for s in srcs))
             nd["phase"] = PHASE_INV_FWD if nd["invariant"] else PHASE_VAR_FWD
             if nd["invariant"]:
@@ -480,9 +490,8 @@ class ExecPlan(_DevicePlan):
         for nd in nodes:
             if nd["kind"] != 0:
                 continue
-            Bn, M, N, K = nd["sizes"]
-            macs = Bn * M * N * K
-            el = math.prod(nd["a"].shape) + math.prod(nd["b"].shape) + math.prod(nd["c"].shape)
+            macs = nd["plan"].macs if nd.get("d") is not None else math.prod(nd["sizes"])
+            el = sum(math.prod(nd[x].shape) for x in ("a", "b", "d", "c") if nd.get(x) is not None)
             if nd["invariant"]:
                 self.macs_invariant += macs
             else:
@@ -497,6 +506,28 @@ class ExecPlan(_DevicePlan):
             dense = row_major_strides(rs)
             odims = [[e, sx, so] for e, sx, so in zip(rs, dense, root_strides) if e != 1]
             self._chunk_words = build_single_desc(odims, [], self.dtype)
+
+    def _absorb(self, nodes, tensors):
+        """Replace the last two pair nodes by one absorb-root node when the last one is a
+        ``DMMA_32x32`` product reading the other's result (``lowering.build_absorb_desc``)."""
+        if len(nodes) < 2:
+            return
+        P, R = nodes[-2], nodes[-1]
+        if P["kind"] != 0 or R["kind"] != 0 or P.get("d") is not None or R["plan"].variant != lowering.VAR_DMMA_32x32:
+            return
+        X = P["c"]
+        if X not in R["terms"]:
+            return
+        ab = lowering.build_absorb_desc(P["dims"], R["dims"], R["terms"][0] is X, accumulate=R["acc"],
+                                        sm_count=self.sm_count, c_dense_elems=R["dense"])
+        if ab is None:
+            return
+        pa, pb = P["terms"]
+        small, big = (pa, pb) if ab.small_is_a else (pb, pa)
+        V = R["terms"][1] if R["terms"][0] is X else R["terms"][0]
+        tensors.remove(X)
+        nodes[-2:] = [dict(kind=0, a=big, b=V, d=small, c=R["c"], words=ab.words, root=R["root"], plan=ab,
+                           sizes=ab.sizes, dims=None, acc=R["acc"], dense=R["dense"], terms=None)]
 
     def _check_root_shape(self, shape):
         if tuple(shape) != tuple(self.root_shape):

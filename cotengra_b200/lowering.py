@@ -62,6 +62,7 @@ VAR_DMMA_256x16, VAR_ROW_128x8, VAR_ROW_256x4, VAR_ROWSTREAM = 5, 6, 7, 8
 VAR_TC05_128x64, VAR_TC05_128x32, VAR_TC05_128x16 = 9, 10, 11
 VAR_DMMA3M_128x32, VAR_DMMA3M_256x16, VAR_DMMASTREAM, VAR_DOTSTREAM, VAR_DOTSTREAM4 = 12, 13, 14, 15, 16
 VAR_DMMA_32x32, VAR_ROWSTREAM_K, VAR_TF32_32x32 = 18, 19, 20
+VAR_ABSORB_ROOT = 21
 # the DMMA stream kernel (csrc/dmmastream.cuh) takes N <= 32 with K <= 64 (32-row warp blocks) and
 # 32 < N <= 64 with K <= 32 (16-row warp blocks)
 DMMASTREAM_KMAX, DMMASTREAM_WIDE_N, DMMASTREAM_WIDE_KMAX = 64, 64, 32
@@ -731,6 +732,124 @@ def _pack(dtype, t, splitk, flags, run_a, lbopad, c_dense_elems):
 # ---------------------------------------------------------------------------
 # single-operand nodes  (contract.py:61-119, 332-361)
 # ---------------------------------------------------------------------------
+
+
+# ---------------------------------------------------------------------------
+# absorb-root nodes (csrc/absorbdot.cuh; word layout in csrc/gett_desc.h)
+# ---------------------------------------------------------------------------
+AB_M, AB_N, AB_K, AB_C, AB_KL, AB_NG, AB_UNITS, AB_KLA, AB_KLV, AB_GRID, AB_BS_SLOT, AB_CCP = range(2, 14)
+AB_MAXG = 32
+AB_TMA = W_HDR
+AB_TMC, AB_TNV, AB_TNC = AB_TMA + 32, AB_TMA + 64, AB_TMA + 96
+AB_TKA = AB_TMA + 128
+AB_TKB = AB_TKA + 16
+AB_TCB = AB_TKB + 16
+AB_TCV = AB_TCB + 128
+AB_G = AB_TCV + 128
+AB_TBCK = AB_G + AB_MAXG * 4
+
+
+@dataclass
+class AbsorbPlan:
+    """An absorb-root node: ``words`` and what the executor needs to wire its operands.
+    ``small_is_a``: the absorption's small operand is its term A (else B)."""
+
+    words: np.ndarray
+    small_is_a: bool
+    sizes: tuple
+    macs: int
+    variant: int = VAR_ABSORB_ROOT
+    swapped: bool = False
+    splitk: int = 1
+    tiles: int = 1
+
+
+def _enum(dims, cols):
+    """Offsets (one list per column of ``cols``) of every point of ``dims`` (first dim fastest)."""
+    out = [[0] for _ in cols]
+    for d in dims:
+        out = [[o + i * d[c] for i in range(d[0]) for o in lst] for lst, c in zip(out, cols)]
+    return out
+
+
+def build_absorb_desc(dp: PairDims, dr: PairDims, x_is_a, accumulate=False, sm_count=132, c_dense_elems=0):
+    """Fold the absorption ``X = P`` (dims ``dp``) into the product ``R`` that reads it (dims ``dr``;
+    X is R's operand A if ``x_is_a``), or None when the absorb-root kernel does not take the pair.
+    One side of P is the small operand Bs: its kept dims are each contracted in R (cc) or kept by R
+    (ck); the other side's kept dims are kept by R (rows) or contracted (k').  The kernel takes
+    N <= 32, K <= 16, 32 * ceil(CC / 32) * CK <= 128 and either CK = 1 with up to 32 rows or CK <= 4
+    with up to 8; no batch, and the dims of P and R must match one to one by their X stride."""
+    if dp.batch or dr.batch:
+        return None
+    xi = 1 if x_is_a else 2  # X's stride column in R's dims
+    vi = 3 - xi
+    r_keep = {d[xi]: (d[0], d[3]) for d in (dr.m if x_is_a else dr.n)}  # X stride -> (ext, sC)
+    v_keep = [[d[0], d[vi], d[3]] for d in (dr.n if x_is_a else dr.m)]
+    r_con = {d[xi]: (d[0], d[vi]) for d in dr.k}  # X stride -> (ext, sV)
+    if len(r_con) != len(dr.k) or len(r_keep) != len(dr.m if x_is_a else dr.n):
+        return None
+    for small_is_a in (False, True):
+        small = dp.m if small_is_a else dp.n   # [ext, sA, sB, sC]: P's side of Bs
+        big = dp.n if small_is_a else dp.m
+        bi, si = (2, 1) if small_is_a else (1, 2)  # columns of the big and the small operand in P
+        xdims = {d[3]: d for d in small + big}
+        if not small or len(xdims) != len(small) + len(big) or set(xdims) != set(r_keep) | set(r_con):
+            continue
+        if any(xdims[x][0] != (r_keep.get(x) or r_con[x])[0] for x in xdims):
+            continue
+        small_x = {d[3] for d in small}
+        rows = [[d[0], d[bi], r_keep[d[3]][1]] for d in big if d[3] in r_keep]
+        ck = [[d[0], d[si], r_keep[d[3]][1]] for d in small if d[3] in r_keep]
+        cc = sorted(([d[0], d[si], r_con[d[3]][1]] for d in small if d[3] in r_con), key=lambda d: d[2])
+        kprime = [[d[0], d[bi], r_con[d[3]][1]] for d in big if d[3] in r_con]
+        MX, CK = math.prod(d[0] for d in rows), math.prod(d[0] for d in ck)
+        N, K, CC = math.prod(d[0] for d in v_keep), math.prod(d[0] for d in dp.k), math.prod(d[0] for d in cc)
+        CCP = -(-CC // 32) * 32
+        rows_per = 8 if CK > 1 else 32
+        if MX > rows_per or CK * rows_per > 32 or N > 32 or K > 16 or CK * CCP > 128 or not small_x:
+            return None
+        kl = min(kprime, key=lambda d: d[2], default=None)
+        if kl is not None and kl[0] == 2:
+            kprime.remove(kl)
+        else:
+            kl = [1, 0, 0]
+        grid = sorted(kprime, key=lambda d: (d[1], d[2]))  # unit u + 1 reads the other half of A's sectors
+        if len(grid) > AB_MAXG:
+            return None
+        units = math.prod(d[0] for d in grid)
+        w = np.zeros(DESC_WORDS, dtype=np.int64)
+        w[0], w[1] = DESC_MAGIC, DTYPE_CODES["complex128"]
+        w[AB_M], w[AB_N], w[AB_K], w[AB_C], w[AB_CCP], w[AB_KL] = CK * rows_per if CK > 1 else MX, N, K, CC, CCP, kl[0]
+        w[AB_NG], w[AB_UNITS], w[AB_KLA], w[AB_KLV] = len(grid), units, kl[1], kl[2]
+        w[AB_GRID] = min(units, sm_count)
+        w[AB_BS_SLOT] = -1
+        w[W_FLAGS] = int(bool(accumulate))
+        w[W_VARIANT] = VAR_ABSORB_ROOT
+        w[W_CELEMS] = c_dense_elems
+        ra, rc = _enum(rows, (1, 2))
+        ckb, ckc = _enum(ck, (1, 2))
+        ma, mc = [-1] * 32, [-1] * 32
+        for j, (ob, oc) in enumerate(zip(ckb, ckc)):
+            for r, (a, c) in enumerate(zip(ra, rc)):
+                ma[j * rows_per + r], mc[j * rows_per + r] = a, c + oc
+        tbck = [min(mb * 8 // rows_per, CK - 1) for mb in range(4)]
+        nv, nc = _enum(v_keep, (1, 2))
+        ka, kb = _enum([[d[0], d[bi], d[si]] for d in dp.k], (1, 2))
+        cb, cv = _enum(cc, (1, 2))
+        tcb = [-1] * 128
+        for j, ob in enumerate(ckb):
+            tcb[j * CCP:j * CCP + CC] = [ob + o for o in cb]
+        for off, vals in ((AB_TMA, ma), (AB_TMC, mc), (AB_TNV, nv), (AB_TNC, nc), (AB_TKA, ka), (AB_TKB, kb),
+                          (AB_TCB, tcb), (AB_TCV, cv), (AB_TBCK, tbck)):
+            w[off:off + len(vals)] = vals
+        div = 1
+        for j, (e, sa, sv) in enumerate(grid):
+            w[AB_G + 4 * j:AB_G + 4 * j + 4] = (e, div, sa, sv)
+            div *= e
+        kp = units * kl[0]
+        M = MX * CK
+        return AbsorbPlan(w, small_is_a, (1, M, N, kp * CC), MX * kp * K * CC * CK + M * N * kp * CC)
+    return None
 
 
 def classify_single(term, shape, out, out_strides=None, strides_x=None):

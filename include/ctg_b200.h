@@ -85,6 +85,13 @@ int ctgb_device_info(int* sm_count, int* cc_major, int* cc_minor,
 int ctgb_contract_pair(const int64_t* desc, const void* A, const void* B,
                        void* C, void* stream);
 
+/* One absorb-root node (variant 21, complex128):
+ * C[m,n] (+)= sum_{k',c} (sum_k A[m,k',k] Bs[k,c]) V[k',c,n], the result of the
+ * absorption A.Bs never formed.  `desc` is a pair-sized word array in the
+ * absorb-root layout (cotengra_b200/csrc/gett_desc.h). */
+int ctgb_absorb_root(const int64_t* desc, const void* A, const void* Bs,
+                     const void* V, void* C, void* stream);
+
 /* One single-operand node: out = diag/sum/transpose of X. */
 int ctgb_reduce_single(const int64_t* desc, const void* X, void* out,
                        void* stream);
