@@ -318,13 +318,23 @@ int launch_absorb_root(const int64_t* h, const int64_t* d, const void* A, const 
     if (h[W_CELEMS] <= 0) return fail(CTGB_E_VALUE, "absorb-root into a strided C needs accumulate");
     CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)h[W_CELEMS] * sizeof(double2), st));
   }
-  static bool attr = false;
-  if (!attr) {
-    CUDA_TRY(cudaFuncSetAttribute(absorbdot_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AB_SMEM));
-    attr = true;
+  // A8: every row is one of the first 8 A rows again (one block per kept Bs column), so a stage
+  // holds 8 A rows; one quarter of c: the Bs fragments stay in registers
+  bool a8 = true;
+  for (int r = 8; r < 32; ++r)
+    if (h[AB_TMC + r] >= 0 && (h[AB_TMC + r % 8] < 0 || h[AB_TMA + r] != h[AB_TMA + r % 8])) a8 = false;
+  const bool breg = h[AB_CCP] == 32;
+  using Kern = void (*)(const int64_t*, const double2*, const double2*, const double2*, double2*);
+  const Kern kern = a8 ? (breg ? absorbdot_kernel<true, true> : absorbdot_kernel<true, false>)
+                    : (breg ? absorbdot_kernel<false, true> : absorbdot_kernel<false, false>);
+  const size_t smem = a8 ? AbRing<true>::SMEM : AbRing<false>::SMEM;
+  static bool attr[4] = {};
+  if (!attr[2 * a8 + breg]) {
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr[2 * a8 + breg] = true;
   }
-  absorbdot_kernel<<<(unsigned)h[AB_GRID], AB_THREADS, AB_SMEM, st>>>(d, (const double2*)A, (const double2*)Bs,
-                                                                      (const double2*)V, (double2*)C);
+  kern<<<(unsigned)h[AB_GRID], AB_THREADS, smem, st>>>(d, (const double2*)A, (const double2*)Bs, (const double2*)V,
+                                                       (double2*)C);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   CUDA_TRY(cudaGetLastError());
   return CTGB_OK;

@@ -657,9 +657,9 @@ struct DmmaPolicy {
 #include "rowstream.cuh"
 #include "dmmastream.cuh"
 #include "dotstream.cuh"
-#include "absorbdot.cuh"
 #include "tc05_policy.cuh"
 #include "gett_ws.cuh"
+#include "absorbdot.cuh"
 #include "tc05_kernel.cuh"
 
 // ------------------------------------------------------------------ single operand
