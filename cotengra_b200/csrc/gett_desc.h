@@ -51,7 +51,8 @@ enum : int {
   // descriptor by ctgb_plan_create; 0 = off.  Device addresses of doubles:
   W_SCALE_A = 36,      //   max|A| of operand A as stored (A is a lazily-normalised intermediate) or 1.0
   W_SCALE_B = 37,      //   same for B; the epilogue multiplies by 1/(fA*fB)
-  W_FACTOR_C = 38,     //   slot receiving max|C| of what this launch stores (atomicMax of the double's bits)
+  W_FACTOR_C = 38,     //   slot receiving max|product| of this launch, as scaled (atomicMax of the double's bits);
+                       //   an accumulating launch adds C0 after it is measured, so it is max|C| only without C0
   W_HDR = 40,
   // arrays
   OFF_TM = W_HDR,                 // MAX_T x (ext, sA, sC)

@@ -36,6 +36,9 @@ MAX_T, MAX_G, MAX_GB, MAX_LD = 12, 40, 12, 24
  W_NTA, W_KTA, W_TILES_M, W_TILES_N, W_TILES_B, W_STEPS_K, W_SPLITK, W_PGM,
  W_MFULL, W_MTEXT, W_MW, W_PGN, W_NFULL, W_NTEXT, W_NW, W_PGK, W_KFULL,
  W_KTEXT, W_KW, W_NLDA, W_NLDB, W_FLAGS, W_VARIANT, W_CELEMS, W_RUNA, W_LBOPAD) = range(36)
+# fused strip_exponent: device addresses of doubles (0 = off) -- the factors fA and fB the product
+# is divided by, and the slot that receives max|product| of the launch (patched in by ctgb_plan_create)
+W_SCALE_A, W_SCALE_B, W_FACTOR_C = 36, 37, 38
 W_HDR = 40
 OFF_TM = W_HDR
 OFF_TN = OFF_TM + MAX_T * 3
