@@ -23,6 +23,7 @@ from .vjp import VjpPlan
 from .contract import (
     B200Contractor,
     TreeExecutor,
+    array_contract_expression,
     benchmark,
     contract_checkpointed,
     contract_distributed,
@@ -40,6 +41,6 @@ from .contract import (
 __all__ = [
     "TreeSpec", "get_symbol", "PairDims", "build_pair_desc", "build_single_desc",
     "classify_pair", "classify_single", "ExecPlan", "VjpPlan", "B200Contractor", "TreeExecutor",
-    "benchmark", "contract_checkpointed", "contract_distributed", "contract_tree", "einsum", "gen_output_chunks", "implementation", "install",
+    "array_contract_expression", "benchmark", "contract_checkpointed", "contract_distributed", "contract_tree", "einsum", "gen_output_chunks", "implementation", "install",
     "make_contractor", "rank_slices", "reduce_partials", "tensordot",
 ]

@@ -202,11 +202,19 @@ class _Executor:
     depends on the result only through ``m 10^e``.  ``vjp`` then takes the forward's ``exponent``.
 
     ``plan_opts`` go to the forward and reverse-mode plans (``ExecPlan`` / ``VjpPlan`` keywords).
+
+    ``resident`` are device tensors the executor holds for the last plan inputs (folded constants,
+    ``TreeExecutor(constants=...)``): every entry point takes only the leading inputs, the
+    *variables*, and the executor appends the resident ones.
     """
+
+    _exp_shift = 0.0         # added to every stripped exponent: the exponents of the folded constants
+    _constant_result = None  # every input constant: the whole result, formed when the executor is built
+    _constant_numpy = False  # ... and whether it is returned as numpy
 
     def __init__(self, contractions, inputs, output, size_dict, sliced, dtype, strip_exponent=False, device=None,
                  vjp_max_bytes=None, precision="3xtf32", stripped_grad=False, accumulate="native", absorb_root=False,
-                 **plan_opts):
+                 resident=(), **plan_opts):
         torch = _torch()
         self._ir, self._plan_opts = contractions, plan_opts
         # the program without its slicing: the positional head of ``ExecPlan`` and ``VjpPlan``
@@ -223,7 +231,8 @@ class _Executor:
         self.strip_exponent = bool(strip_exponent)
         self.stripped_grad = bool(stripped_grad)
         self.vjp_max_bytes = vjp_max_bytes
-        self._shapes = [tuple(size_dict[ix] for ix in term) for term in inputs]
+        self._resident = list(resident)
+        self._shapes = [tuple(size_dict[ix] for ix in term) for term in inputs[:len(inputs) - len(self._resident)]]
         self._ws = None
         self._vjp_plans, self._vjp_ws = {}, None
 
@@ -242,7 +251,8 @@ class _Executor:
     def _check_inputs(self, arrays):
         shapes = self._shapes
         if len(arrays) != len(shapes):
-            raise ValueError(f"expected {len(shapes)} arrays, got {len(arrays)}")
+            what = "variables" if self._resident else "arrays"
+            raise ValueError(f"expected {len(shapes)} {what}, got {len(arrays)}")
         for i, (x, s) in enumerate(zip(arrays, shapes)):
             if tuple(x.shape) != tuple(s):
                 raise ValueError(f"array {i} has shape {tuple(x.shape)}, expected {tuple(s)}")
@@ -254,6 +264,10 @@ class _Executor:
         torch = _torch()
         self._check_inputs(tensors)
         begin, step, count = self._check_slice_range(begin, step, count)
+        if (self._constant_result is not None and out is None and exponent is None
+                and (begin, step, count) == (0, 1, self.nslices)):
+            return tuple(t.clone() for t in self._constant_result) if self.strip_exponent \
+                else self._constant_result.clone()
         tdt = getattr(torch, self.out_dtype)
         with torch.cuda.device(self.device):
             if out is None:
@@ -266,12 +280,17 @@ class _Executor:
                 exponent = torch.full((1,), -math.inf, dtype=torch.float64, device=self.device)
             ws = self.workspace()
             ptrs, _keep = self._input_ptrs(tensors)
+            if self._exp_shift:
+                exponent.sub_(self._exp_shift)  # the plan combines its slices with the exponent it was given
             self.plan.execute(ptrs, out.data_ptr(), exponent.data_ptr() if exponent is not None else None,
                               ws.data_ptr(), ws.numel(), begin, step, count, _stream_ptr())
+            if self._exp_shift:
+                exponent.add_(self._exp_shift)
         return (out, exponent) if self.strip_exponent else out
 
     def _input_ptrs(self, tensors):
-        """Device pointers of the inputs (plus the contiguous copies that must outlive the call)."""
+        """Device pointers of the inputs, then of the resident tensors (plus the contiguous copies
+        that must outlive the call)."""
         ptrs, keep = [], []
         for i, t in enumerate(tensors):
             if dtype_name(t.dtype) != self.dtype:
@@ -283,7 +302,7 @@ class _Executor:
                 t = t.contiguous()
                 keep.append(t)
             ptrs.append(t.data_ptr())
-        return ptrs, keep
+        return ptrs + [t.data_ptr() for t in self._resident], keep
 
     # ------------------------------------------------------------------ gradients
     def vjp_plan(self, wrt=None, max_bytes=None):
@@ -292,6 +311,8 @@ class _Executor:
         from .vjp import VjpPlan
 
         wrt = tuple(range(len(self._shapes))) if wrt is None else tuple(sorted({int(i) for i in wrt}))
+        if self._resident and any(i < 0 or i >= len(self._shapes) for i in wrt):
+            raise ValueError(f"wrt {list(wrt)} names inputs outside the {len(self._shapes)} variables")
         max_bytes = self.vjp_max_bytes if max_bytes is None else max_bytes
         key = wrt if max_bytes is None else (wrt, max_bytes)
         plan = self._vjp_plans.get(key)
@@ -330,6 +351,9 @@ class _Executor:
                 if exponent is None:
                     raise ValueError("a stripped gradient needs the exponent of the forward call (exponent=)")
                 exp = torch.as_tensor(exponent, dtype=torch.float64).to(self.device).reshape(1).contiguous()
+                if self._exp_shift:
+                    exp = exp - self._exp_shift  # the plan's own exponent, without the folded constants'
+
             cot = cotangent.to(device=self.device, dtype=tdt).contiguous()
             grads = [torch.zeros(tuple(t.shape), dtype=tdt, device=self.device) if i in plan.wrt else None
                      for i, t in enumerate(tensors)]
@@ -339,7 +363,8 @@ class _Executor:
             ws = self._vjp_ws
             # (only a stripped plan takes the forward's exponent)
             extra = {} if exp is None else {"exp_ptr": exp.data_ptr()}
-            plan.execute(ptrs, cot.data_ptr(), [g.data_ptr() if g is not None else None for g in grads],
+            gptrs = [g.data_ptr() if g is not None else None for g in grads] + [None] * len(self._resident)
+            plan.execute(ptrs, cot.data_ptr(), gptrs,
                          ws.data_ptr(), ws.numel(), begin, step, count, _stream_ptr(), **extra)
         return grads
 
@@ -361,10 +386,17 @@ class _Executor:
 
     def contract_host(self, arrays, begin=0, step=1, count=None):
         """End-to-end with HOST buffers through ``ctgb_plan_execute_host``:
-        H2D of the inputs, all slices, D2H of the result, synchronised."""
+        H2D of the inputs, all slices, D2H of the result, synchronised.  An executor with resident
+        tensors copies its variables to the device and runs ``contract_device``."""
         torch = _torch()
         self._check_inputs(arrays)
         begin, step, count = self._check_slice_range(begin, step, count)
+        if self._resident:
+            res = self.contract_device([_to_device(np.asarray(a, dtype=self.dtype), self.device)[0] for a in arrays],
+                                       begin, step, count)
+            if self.strip_exponent:
+                return _from_device(res[0], True), float(res[1].item())
+            return _from_device(res, True)
         host = [np.asarray(a, dtype=self.dtype, order="C") for a in arrays]
         out = np.zeros(self.plan.out_shape, dtype=self.out_dtype)
         with torch.cuda.device(self.device):
@@ -381,11 +413,22 @@ class TreeExecutor(_Executor):
     ``TreeSpec.from_cotengra``).  The slice loop, the node loop, the slice
     accumulation and (optionally) exponent stripping all run inside
     ``ctgb_plan_execute``.  The options are those of ``_Executor``.
+
+    ``constants={position: array}`` fixes the inputs at those positions of ``tree.inputs`` (numpy
+    arrays or torch tensors of the input's full shape and the executor's dtype).  Every subtree whose
+    leaves are all constant is contracted once, here, within ``fold_max_bytes`` of folded arrays
+    (default: the unfolded forward plan's ``workspace_bytes``; 0 folds nothing; ``constants.py``), and
+    every entry point then takes only the remaining inputs, the *variables*, in their original order;
+    ``wrt`` counts positions among them.  The constants are copied: changing them afterwards has no
+    effect, and they get no gradient.  ``folded`` lists the folds (``constants.Fold``: SSA id, term,
+    bytes, MACs per call removed) and ``folded_bytes`` their size.  When every input is constant the
+    result is formed here and each full call returns a fresh copy of it: numpy if every constant was
+    numpy, a torch CUDA tensor otherwise.
     """
 
     def __init__(self, tree, dtype="complex128", strip_exponent=False, device=None,
                  contractions=None, fuse=True, vjp_max_bytes=None, precision="3xtf32", stripped_grad=False,
-                 accumulate="native", **plan_opts):
+                 accumulate="native", constants=None, fold_max_bytes=None, **plan_opts):
         check_precision(precision, dtype)
         check_accumulate(accumulate)
         self.spec = spec = tree if isinstance(tree, TreeSpec) else TreeSpec.from_cotengra(tree)
@@ -402,11 +445,70 @@ class TreeExecutor(_Executor):
             opts = fuse if isinstance(fuse, dict) else {}
             self.exec_spec, self.fusion = fuse_stems(spec, dtype_name(dtype), **opts)
         ir = self.exec_spec.contractions() if contractions is None else contractions
-        super().__init__(ir, spec.inputs, spec.output, spec.size_dict, spec.sliced, dtype,
-                         strip_exponent=strip_exponent, device=device, vjp_max_bytes=vjp_max_bytes,
-                         precision=precision, stripped_grad=stripped_grad, accumulate=accumulate,
-                         absorb_root=bool(fuse) and contractions is None, **plan_opts)
+        opts = dict(strip_exponent=strip_exponent, device=device, vjp_max_bytes=vjp_max_bytes, precision=precision,
+                    stripped_grad=stripped_grad, accumulate=accumulate,
+                    absorb_root=bool(fuse) and contractions is None, **plan_opts)
+        self.constants, self.folded, self.folded_bytes, self._const_digest = (), [], 0, None
+        if constants is None:
+            super().__init__(ir, spec.inputs, spec.output, spec.size_dict, spec.sliced, dtype, **opts)
+        else:
+            if contractions is not None:
+                raise ValueError("constants are folded on the tree's own program: not with contractions=")
+            self._init_folded(ir, dtype_name(dtype), constants, fold_max_bytes, opts)
         self._ref_work = None
+
+    def _init_folded(self, ir, dtype, constants, fold_max_bytes, opts):
+        """Fold the constant subtrees (``constants.plan_folds``) on the device and compile what
+        remains, with the folded arrays and the unfolded constant leaves as resident inputs."""
+        from . import constants as K
+
+        torch = _torch()
+        spec = self.spec
+        consts = K.check_constants(constants, spec.shapes(), dtype)
+        self.constants = tuple(sorted(consts))
+        self._const_digest = K.digest(consts, dtype)
+        dev = torch.device("cuda", torch.cuda.current_device() if opts["device"] is None else opts["device"])
+        # the keywords of the plans that form the folded arrays: F is stored in the plan dtype
+        fold_kw = {k: v for k, v in opts.items()
+                   if k not in ("device", "vjp_max_bytes", "stripped_grad", "absorb_root", "accumulate")}
+        with torch.cuda.device(dev):
+            leaves = {}
+            for i, x in consts.items():
+                t, was_numpy = _to_device(x, dev)
+                leaves[i] = t.detach() if was_numpy else t.detach().clone()
+            if len(consts) == len(spec.inputs):
+                terms, ids, resident, runs = list(spec.inputs), None, [leaves[i] for i in range(len(consts))], []
+            else:
+                cost = ExecPlan(ir, spec.inputs, spec.output, spec.size_dict, spec.sliced, dtype=dtype, **fold_kw)
+                fp = K.plan_folds(self.exec_spec, ir, consts, dtype, fold_max_bytes, cost)
+                runs = [self._fold(f, leaves, dtype, fold_kw, dev) for f in fp.folds]
+                resident = [r[0] for r in runs] + [leaves[i] for i in fp.resident_leaves]
+                terms, ids, ir = fp.inputs, fp.input_ids, fp.records
+                self.folded = fp.folds
+                self.folded_bytes = sum(f.bytes for f in fp.folds)
+            del leaves
+            super().__init__(ir, terms, spec.output, spec.size_dict, spec.sliced, dtype, resident=resident,
+                             input_ids=ids, **opts)
+            if len(consts) == len(spec.inputs):
+                self._constant_result = self.contract_device([])
+                self._constant_numpy = all(not isinstance(a, torch.Tensor) for a in consts.values())
+            torch.cuda.synchronize(dev)
+        # the folds' exponents, read once everything has run
+        self._exp_shift = sum(float(r[1].item()) for r in runs if r[1] is not None)
+
+    def _fold(self, f, leaves, dtype, fold_kw, dev):
+        """Start forming ``F`` of the fold ``f`` from its constant leaves, in the plan dtype: returns
+        ``(F, exponent tensor or None, plan, workspace)``, the last two to be kept until it has run."""
+        torch = _torch()
+        plan = ExecPlan(f.records, [self.spec.inputs[i] for i in f.leaves], f.term, self.spec.size_dict, f.sliced,
+                        dtype=dtype, input_ids=f.leaves, **fold_kw).create()
+        out = torch.zeros(plan.out_shape, dtype=getattr(torch, dtype), device=dev)
+        exp = torch.full((1,), -math.inf, dtype=torch.float64, device=dev) if plan.strip_exponent else None
+        ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=dev)
+        plan.execute([leaves[i].data_ptr() for i in f.leaves], out.data_ptr(),
+                     exp.data_ptr() if exp is not None else None, ws.data_ptr(), ws.numel(), 0, 1, plan.nslices,
+                     _stream_ptr())
+        return out, exp, plan, ws
 
     @property
     def reference_work(self):
@@ -425,6 +527,13 @@ class TreeExecutor(_Executor):
     def __call__(self, arrays, **kw):
         return contract_tree(self, arrays, **kw)
 
+    def _numpy_out(self, torch, arrays):
+        """Whether results of a call on ``arrays`` come back as numpy: numpy variables, or, when every
+        input is constant, numpy constants."""
+        if not arrays and self.constants:
+            return self._constant_numpy
+        return all(not isinstance(a, torch.Tensor) for a in arrays)
+
     # ------------------------------------------------------------------ output chunks
     def _chunk_plan(self):
         """A second plan over the same program whose output is ONE chunk: the output term
@@ -434,11 +543,14 @@ class TreeExecutor(_Executor):
             torch = _torch()
             spec = self.exec_spec
             chunk_out, _step, _n = output_chunking(spec)
+            # (with constants: the folded program, whose last inputs are resident)
+            ir, inputs = self._program[:2] if self.constants else (spec.contractions(), spec.inputs)
             with torch.cuda.device(self.device):
-                self._chunk = ExecPlan(spec.contractions(), spec.inputs, chunk_out, spec.size_dict,
+                self._chunk = ExecPlan(ir, inputs, chunk_out, spec.size_dict,
                                        spec.sliced, dtype=self.dtype,
                                        strip_exponent=self.strip_exponent, precision=self.precision,
-                                       accumulate=self.accumulate).create()
+                                       accumulate=self.accumulate,
+                                       input_ids=self._plan_opts.get("input_ids")).create()
         return self._chunk
 
     def gen_output_chunks(self, arrays, with_key=False):
@@ -454,9 +566,9 @@ class TreeExecutor(_Executor):
         spec = self.spec
         _chunk_out, stepsize, nchunks = output_chunking(spec)
         plan = self._chunk_plan()
-        all_numpy = all(not isinstance(a, torch.Tensor) for a in arrays)
+        all_numpy = self._numpy_out(torch, arrays)
         tensors = [_to_device(a, self.device)[0] for a in arrays]
-        ptrs = [t.data_ptr() for t in tensors]
+        ptrs = [t.data_ptr() for t in tensors] + [t.data_ptr() for t in self._resident]
         tdt = getattr(torch, self.out_dtype)
         need = plan.total_bytes
         # a buffer of its own, not ``_ws``: the generator yields between launches, and a
@@ -472,7 +584,7 @@ class TreeExecutor(_Executor):
                              ws.data_ptr(), ws.numel(), o * stepsize, 1, stepsize, _stream_ptr())
             chunk = _from_device(out, all_numpy)
             if self.strip_exponent:
-                chunk = (chunk, float(exp.item()))
+                chunk = (chunk, float(exp.item()) + self._exp_shift)
             if with_key:
                 key = {ix: x for ix, x in spec.slice_key(o * stepsize).items() if ix in spec.output}
                 yield chunk, key
@@ -494,6 +606,8 @@ def contract_tree(tree, arrays, strip_exponent=False, check_zero=False, dtype=No
     ex = _executor_for(tree, arrays, dtype, strip_exponent=strip_exponent, vjp_max_bytes=vjp_max_bytes,
                        precision=precision, stripped_grad=stripped_grad, accumulate=accumulate, **plan_opts)
     slices = (0, 1, None) if slice_ids is None else slice_ids
+    if ex._constant_result is not None and not ex._constant_numpy:
+        return _run_device(ex, arrays, [], slices, check_zero)
     if all(not isinstance(a, torch.Tensor) for a in arrays):
         res = ex.contract_host(arrays, *slices)
         return _finish_stripped(*res, check_zero) if ex.strip_exponent else res
@@ -592,6 +706,70 @@ def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=
     yield from ex.gen_output_chunks(arrays, with_key=with_key)
 
 
+def array_contract_expression(inputs, output=None, size_dict=None, shapes=None, optimize=None, constants=None,
+                              strip_exponent=False, dtype=None, **executor_opts):
+    """``cotengra.array_contract_expression`` (interface.py:673-768) on the tree executor: a callable
+    ``expr(*variables, backend=None)`` that contracts the inputs not in ``constants`` (``{position:
+    array}``, folded once, ``TreeExecutor(constants=...)``) along the tree ``optimize``, a
+    ``TreeSpec`` or a live cotengra ``ContractionTree`` whose inputs, output and index sizes match
+    the arguments (``ValueError`` otherwise; path search stays in cotengra).  ``size_dict`` or
+    ``shapes`` give the sizes, default the tree's; ``output`` defaults to the tree's.  ``dtype``
+    defaults to the constants' common dtype, or without constants to that of the first call's arrays.
+    Results as ``contract_tree``: ``(mantissa, exponent)`` with ``strip_exponent``, numpy for numpy
+    variables.  ``executor_opts`` are ``TreeExecutor``'s."""
+    if optimize is None:
+        raise ValueError("optimize must be a TreeSpec or a cotengra ContractionTree (path search stays in cotengra)")
+    try:
+        spec = optimize if isinstance(optimize, TreeSpec) else TreeSpec.from_cotengra(optimize)
+    except AttributeError:
+        raise ValueError(f"optimize must be a TreeSpec or a cotengra ContractionTree, got {type(optimize)}") from None
+    inputs = tuple(tuple(t) for t in inputs)
+    if shapes is not None:
+        if len(shapes) != len(inputs):
+            raise ValueError(f"{len(shapes)} shapes for {len(inputs)} inputs")
+        size_dict = {}
+        for term, shp in zip(inputs, shapes):
+            if len(term) != len(shp):
+                raise ValueError(f"input {term} has {len(shp)} dimensions")
+            for ix, d in zip(term, shp):
+                if size_dict.setdefault(ix, int(d)) != int(d):
+                    raise ValueError(f"index {ix!r} has two sizes")
+    if inputs != spec.inputs:
+        raise ValueError("the tree's inputs differ from the expression's")
+    if output is not None and tuple(output) != spec.output:
+        raise ValueError(f"the tree's output {''.join(map(str, spec.output))!r} differs from the expression's")
+    if size_dict is not None and any(int(size_dict.get(ix, -1)) != d for ix, d in spec.size_dict.items()
+                                     if any(ix in t for t in inputs)):
+        raise ValueError("the tree's index sizes differ from the expression's")
+    if constants is not None:
+        from .constants import check_constants
+
+        constants = check_constants(constants, spec.shapes())
+        if dtype is None and constants:
+            names = {dtype_name(a.dtype) for a in constants.values()}
+            if len(names) != 1:
+                raise TypeError(f"constants of several dtypes {sorted(names)}: give dtype=")
+            dtype = names.pop()
+    return _Expression(spec, constants, dict(executor_opts, strip_exponent=strip_exponent), dtype)
+
+
+class _Expression:
+    """``expr(*variables, backend=None)`` of ``array_contract_expression``: one ``TreeExecutor``,
+    built on the first call when the dtype comes from the arrays."""
+
+    def __init__(self, spec, constants, opts, dtype):
+        self.spec, self.constants, self.opts = spec, constants, opts
+        self.executor = None if dtype is None else TreeExecutor(spec, dtype=dtype, constants=constants, **opts)
+
+    def __call__(self, *arrays, backend=None):
+        if self.executor is None:
+            if not arrays:
+                raise ValueError("the expression's dtype comes from its arrays: call it with its variables")
+            self.executor = TreeExecutor(self.spec, dtype=dtype_name(arrays[0].dtype), constants=self.constants,
+                                         **self.opts)
+        return contract_tree(self.executor, list(arrays))
+
+
 def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warmup=True,
               executor=None, precision="3xtf32", accumulate="native", **plan_opts):
     """``tree.benchmark(dtype, max_time, min_reps, max_reps, warmup)`` (cotengra/core.py:
@@ -611,7 +789,7 @@ def benchmark(tree, dtype="float64", max_time=60, min_reps=3, max_reps=100, warm
     gen = torch.Generator(device=ex.device)
     gen.manual_seed(0)
     tensors = []
-    for shp in ex.spec.shapes():
+    for shp in ex._shapes:  # (the variables of an executor with constants)
         t = torch.empty(tuple(shp), dtype=tdt, device=ex.device)
         (torch.view_as_real(t) if t.is_complex() else t).normal_(generator=gen)
         tensors.append(t / max(1.0, float(t.numel()) ** 0.5))
@@ -694,6 +872,8 @@ def contract_checkpointed(tree, arrays, checkpoint, every=1024, strip_exponent=F
     for a in host:
         h.update(str(a.shape).encode())
         h.update(a.tobytes())
+    if getattr(ex, "constants", ()):  # (executors without constants hash as before)
+        h.update(f"|constants={list(ex.constants)}|{ex._const_digest}".encode())
     tag = h.hexdigest()
     nslices = int(ex.nslices)
     every = max(1, int(every))

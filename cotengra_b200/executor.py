@@ -322,11 +322,14 @@ class ExecPlan(_DevicePlan):
         ``R = X . V`` that reads it next (``lowering.build_absorb_desc``), so that X is never stored:
         one ``VAR_ABSORB_ROOT`` node reads A, Bs and V and writes R.  Off by default: the plan is then
         node for node the reference's sequence.  Not with ``strip_exponent`` or a forced ``variant``.
+    input_ids : the SSA id each plan input stands for (default ``range(len(inputs))``), so that a plan
+        input may be an intermediate node formed elsewhere (a folded constant subtree,
+        ``constants.py``); the records keep their own SSA ids.
     """
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None, precision="3xtf32", accumulate="native", absorb_root=False):
+                 variant=None, precision="3xtf32", accumulate="native", absorb_root=False, input_ids=None):
         self.dtype = dtype_name(dtype)
         self.precision = check_precision(precision, self.dtype)
         self.esize = DTYPE_SIZES[self.dtype]
@@ -334,6 +337,9 @@ class ExecPlan(_DevicePlan):
         self.wide = self.acc_dtype != self.dtype
         self.contractions = tuple(contractions)
         self.inputs = [tuple(t) for t in inputs]
+        self.input_ids = tuple(range(len(self.inputs))) if input_ids is None else tuple(int(i) for i in input_ids)
+        if len(self.input_ids) != len(self.inputs):
+            raise ValueError(f"{len(self.input_ids)} input_ids for {len(self.inputs)} inputs")
         self.output = tuple(output)
         self.size_dict = dict(size_dict)
         self.sliced = [(i, int(s), None if p is None else int(p)) for i, s, p in sliced]
@@ -383,11 +389,12 @@ class ExecPlan(_DevicePlan):
             keep = [k for k, ix in enumerate(term) if ix not in sliced_pos]
             cut = [k for k, ix in enumerate(term) if ix in sliced_pos]
             # (nbytes: the whole unsliced array, which strip_exponent copies scaled)
-            cur[i] = _Slot([full_shape[k] for k in keep], [fs[k] for k in keep], K_INPUT, self.input_nbytes[-1],
-                           i, [sliced_pos[term[k]] for k in cut], [fs[k] for k in cut], variant=bool(cut))
-        self.sliced_shapes = [cur[i].shape for i in range(len(self.inputs))]
-
+            cur[self.input_ids[i]] = _Slot([full_shape[k] for k in keep], [fs[k] for k in keep], K_INPUT,
+                                           self.input_nbytes[-1], i, [sliced_pos[term[k]] for k in cut],
+                                           [fs[k] for k in cut], variant=bool(cut))
         tensors = list(cur.values())
+        self.sliced_shapes = [t.shape for t in tensors]
+
         nodes = []  # dicts
         # does the root write (accumulate into) the output itself?  Not with strip_exponent, and in a
         # wide plan only a dot-stream root (decided where the root is lowered)

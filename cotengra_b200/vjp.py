@@ -170,7 +170,7 @@ def vjp_single_dims(h, t):
 class VjpPlan(_DevicePlan):
     """Compile the VJP of ``contractions`` (the executed IR, stem fusion included) for fixed
     input shapes and dtype.  Same arguments as ``ExecPlan`` plus ``wrt``, the inputs that need a
-    gradient (default: all).  ``variant`` forces the kernel of every backward pairwise node.
+    gradient (default: all; positions among the plan's inputs, as ``input_index``).  ``variant`` forces the kernel of every backward pairwise node.
 
     ``max_bytes`` bounds ``workspace_bytes + persistent_bytes`` by recomputing per-slice forward
     values in phase 2.  ``None``, or a budget at or above the plan's own size, gives the plan
@@ -185,7 +185,7 @@ class VjpPlan(_DevicePlan):
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128",
                  wrt=None, strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None,
-                 variant=None, max_bytes=None, precision="3xtf32", stripped_grad=False):
+                 variant=None, max_bytes=None, precision="3xtf32", stripped_grad=False, input_ids=None):
         if max_bytes is not None and (isinstance(max_bytes, bool) or not isinstance(max_bytes, numbers.Integral)
                                       or max_bytes <= 0):
             raise ValueError(f"max_bytes must be a positive integer, got {max_bytes!r}")
@@ -194,7 +194,7 @@ class VjpPlan(_DevicePlan):
                                       "stripped_grad=True (the exponent held constant)")
         self.strip_exponent = bool(strip_exponent)
         fwd = ExecPlan(contractions, inputs, output, size_dict, sliced, dtype=dtype, hoist=hoist,
-                       allow_dmma=allow_dmma, sm_count=sm_count, precision=precision)
+                       allow_dmma=allow_dmma, sm_count=sm_count, precision=precision, input_ids=input_ids)
         self.fwd = fwd
         self.dtype, self.esize, self.sm_count, self.precision = fwd.dtype, fwd.esize, fwd.sm_count, fwd.precision
         self.inputs, self.output, self.sliced = fwd.inputs, fwd.output, fwd.sliced
