@@ -19,6 +19,7 @@ from .lowering import (
     classify_single,
 )
 from .executor import ExecPlan
+from .jvp import JvpPlan
 from .vjp import VjpPlan
 from .contract import (
     B200Contractor,
@@ -40,7 +41,7 @@ from .contract import (
 
 __all__ = [
     "TreeSpec", "get_symbol", "PairDims", "build_pair_desc", "build_single_desc",
-    "classify_pair", "classify_single", "ExecPlan", "VjpPlan", "B200Contractor", "TreeExecutor",
+    "classify_pair", "classify_single", "ExecPlan", "VjpPlan", "JvpPlan", "B200Contractor", "TreeExecutor",
     "array_contract_expression", "benchmark", "contract_checkpointed", "contract_distributed", "contract_tree", "einsum", "gen_output_chunks", "implementation", "install",
     "make_contractor", "rank_slices", "reduce_partials", "tensordot",
 ]

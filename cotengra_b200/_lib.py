@@ -43,6 +43,8 @@ EXPORTS = (
     "ctgb_tc05_launch_config",
     "ctgb_dmmastream_launch_config",
     "ctgb_absorb_root",
+    "ctgb_contract_pair2",
+    "ctgb_plan_execute_jvp",
 )
 TC05_LAUNCH_FIELDS = ("b_stat", "nb", "sa", "grid", "smem", "tm_rank", "bulk", "chunk_steps", "chunks")
 DMMASTREAM_LAUNCH_FIELDS = ("nj", "rows", "grid")
@@ -127,6 +129,11 @@ def load():
     lib.ctgb_contract_pair.argtypes = [C.c_void_p] * 5
     lib.ctgb_reduce_single.argtypes = [C.c_void_p] * 4
     lib.ctgb_absorb_root.argtypes = [C.c_void_p] * 6
+    lib.ctgb_contract_pair2.argtypes = [C.c_void_p] * 7
+    lib.ctgb_plan_execute_jvp.argtypes = [
+        C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p,
+        C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
+    ]
     lib.ctgb_plan_create.argtypes = [C.POINTER(CtgbPlanDesc), C.POINTER(C.c_void_p)]
     lib.ctgb_plan_set_chunk_desc.argtypes = [C.c_void_p, C.c_void_p]
     lib.ctgb_plan_set_scale_slots.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]

@@ -235,6 +235,7 @@ class _Executor:
         self._shapes = [tuple(size_dict[ix] for ix in term) for term in inputs[:len(inputs) - len(self._resident)]]
         self._ws = None
         self._vjp_plans, self._vjp_ws = {}, None
+        self._jvp_plans, self._jvp_ws = {}, None
 
     @property
     def nslices(self):
@@ -367,6 +368,65 @@ class _Executor:
             plan.execute(ptrs, cot.data_ptr(), gptrs,
                          ws.data_ptr(), ws.numel(), begin, step, count, _stream_ptr(), **extra)
         return grads
+
+    def jvp_plan(self, wrt=None, _two_term=True):
+        """The (cached) ``JvpPlan`` of the executed program for the inputs ``wrt`` (default all; positions
+        among the variables).  ``strip_exponent`` executors raise ``NotImplementedError``."""
+        from .jvp import JvpPlan
+
+        if self.strip_exponent:
+            raise NotImplementedError("forward-mode derivatives of strip_exponent results are not supported")
+        wrt = tuple(range(len(self._shapes))) if wrt is None else tuple(sorted({int(i) for i in wrt}))
+        if any(i < 0 or i >= len(self._shapes) for i in wrt):
+            raise ValueError(f"wrt {list(wrt)} names inputs outside the {len(self._shapes)} variables")
+        key = (wrt, bool(_two_term))
+        plan = self._jvp_plans.get(key)
+        if plan is None:
+            torch = _torch()
+            with torch.cuda.device(self.device):
+                plan = JvpPlan(*self._program, self._sliced, dtype=self.dtype, wrt=wrt, precision=self.precision,
+                               accumulate=self.accumulate, absorb_root=self.plan.absorb_root, _two_term=_two_term,
+                               **self._plan_opts).create()
+            self._jvp_plans[key] = plan
+        return plan
+
+    def jvp(self, tensors, tangents, begin=0, step=1, count=None, wrt=None, primal=True, _two_term=True):
+        """Forward mode over slices ``begin, begin+step, ...`` (``count`` of them): the tangent of their
+        sum for the input tangents ``tangents``, one tensor per input in ``wrt`` (default: all), each of
+        its input's shape.  Returns ``(out, tangent_out)``, or ``tangent_out`` alone with
+        ``primal=False``; both have the output's shape and the accumulator dtype.  Asynchronous on the
+        current stream.  Tangents are additive over slices, so one call per rank over
+        ``rank_slices(...)`` followed by an all-reduce gives the JVP of the whole tree.  Folded
+        constants carry no tangent.  ``strip_exponent`` executors raise ``NotImplementedError``."""
+        torch = _torch()
+        self._check_inputs(tensors)
+        begin, step, count = self._check_slice_range(begin, step, count)
+        plan = self.jvp_plan(wrt, _two_term)
+        if len(tangents) != len(plan.wrt):
+            raise ValueError(f"expected {len(plan.wrt)} tangents (one per input in wrt), got {len(tangents)}")
+        tdt, odt = getattr(torch, self.dtype), getattr(torch, self.out_dtype)
+        with torch.cuda.device(self.device):
+            ptrs, _keep = self._input_ptrs(tensors)
+            tans, tptrs = [], [None] * len(ptrs)
+            for i, t in zip(plan.wrt, tangents):
+                if tuple(t.shape) != tuple(self._shapes[i]):
+                    raise ValueError(f"tangent of input {i} has shape {tuple(t.shape)}, expected {self._shapes[i]}")
+                t = t.to(device=self.device, dtype=tdt).contiguous()
+                tans.append(t)
+                tptrs[i] = t.data_ptr()
+            out = torch.zeros(plan.out_shape, dtype=odt, device=self.device) if primal else None
+            tout = torch.zeros(plan.out_shape, dtype=odt, device=self.device)
+            if not plan.tangent_nodes:  # nothing to differentiate: the tangent is zero
+                if primal:
+                    self.contract_device(tensors, begin, step, count, out=out)
+                return (out, tout) if primal else tout
+            if self._jvp_ws is None or self._jvp_ws.numel() < plan.total_bytes:
+                self._jvp_ws = None
+                self._jvp_ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
+            ws = self._jvp_ws
+            plan.execute(ptrs, tptrs, out.data_ptr() if primal else None, tout.data_ptr(), ws.data_ptr(), ws.numel(),
+                         begin, step, count, _stream_ptr())
+        return (out, tout) if primal else tout
 
     def _check_slice_range(self, begin, step, count):
         """Slice ids ``begin, begin+step, ...`` must all lie in ``[0, nslices)``: the device
@@ -625,15 +685,22 @@ def _executor_for(tree, arrays, dtype=None, **opts):
 
 def _run_device(ex, arrays, tensors, slices, check_zero=False, max_bytes=None, as_numpy=False):
     """``ex.contract_device`` of the device ``tensors`` (made from the caller's ``arrays``) over the
-    slices ``(begin, step, count)``: one torch autograd node when ``_records_grad`` says so, whose
-    backward is ``ex.vjp`` over the same slices within ``max_bytes``; a plain run otherwise.  The
-    result comes back as numpy with ``as_numpy``, and a stripped one as ``(mantissa, float exponent)``."""
+    slices ``(begin, step, count)``: one torch autograd node when ``_records_grad`` says so or some
+    array carries a forward-mode tangent (``_tangent_inputs``), whose backward is ``ex.vjp`` over the
+    same slices within ``max_bytes`` and whose forward-mode rule is ``ex.jvp`` over them; a plain run
+    otherwise.  The result comes back as numpy with ``as_numpy``, and a stripped one as
+    ``(mantissa, float exponent)``."""
     torch = _torch()
     begin, step, count = slices
-    if _records_grad(torch, arrays, ex.strip_exponent, ex.stripped_grad):
+    dual = _tangent_inputs(torch, arrays, ex.strip_exponent)
+    if _records_grad(torch, arrays, ex.strip_exponent, ex.stripped_grad) or dual:
+        jvp = None
+        if dual:
+            def jvp(ts, tans):
+                return ex.jvp(ts, [tans[i] for i in dual], begin, step, count, wrt=dual, primal=False)
         res = _differentiable(torch, lambda ts: ex.contract_device(ts, begin, step, count),
                               lambda ts, g, wrt, e=None: ex.vjp(ts, g, begin, step, count, wrt=wrt,
-                                                                max_bytes=max_bytes, exponent=e), tensors)
+                                                                max_bytes=max_bytes, exponent=e), tensors, jvp)
     else:
         res = ex.contract_device(tensors, begin, step, count)
     if ex.strip_exponent:
@@ -657,22 +724,39 @@ def _records_grad(torch, arrays, strip_exponent, stripped_grad=False):
     return True
 
 
+def _tangent_inputs(torch, arrays, strip_exponent):
+    """Positions of the arrays that carry a ``torch.autograd.forward_ad`` tangent (all must be torch
+    tensors).  ``strip_exponent`` results get no tangent: a warning says so and the list is empty."""
+    if not arrays or not all(isinstance(a, torch.Tensor) for a in arrays):
+        return []
+    from torch.autograd import forward_ad
+
+    dual = [i for i, a in enumerate(arrays) if forward_ad.unpack_dual(a).tangent is not None]
+    if dual and strip_exponent:
+        warnings.warn("strip_exponent=True: no forward-mode tangent is recorded for the (mantissa, exponent) "
+                      "result", UserWarning, stacklevel=4)
+        return []
+    return dual
+
+
 _GRAD_FN = None
 
 
-def _differentiable(torch, run, vjp, tensors):
+def _differentiable(torch, run, vjp, tensors, jvp=None):
     """``run(tensors)`` as one torch autograd node whose backward is ``vjp(tensors, grad, wrt)``
-    (a ``VjpPlan`` on the device; ``wrt`` from ``ctx.needs_input_grad``).  A stripped ``run``
+    (a ``VjpPlan`` on the device; ``wrt`` from ``ctx.needs_input_grad``) and whose forward-mode rule
+    is ``jvp(tensors, tangents)`` (a ``JvpPlan``; ``tangents`` has one entry per tensor, zeros where
+    torch has none, and ``jvp`` reads those of the inputs it was made for).  A stripped ``run``
     returns ``(m, e)``: ``e`` is not differentiable, and the backward is
-    ``vjp(tensors, grad_m, wrt, e)``."""
+    ``vjp(tensors, grad_m, wrt, e)``; it has no forward-mode rule (``jvp`` is None)."""
     global _GRAD_FN
     if _GRAD_FN is None:
         from torch.autograd.function import once_differentiable
 
         class _Contract(torch.autograd.Function):
             @staticmethod
-            def forward(ctx, run, vjp, *tensors):
-                ctx.vjp = vjp
+            def forward(ctx, run, vjp, jvp, *tensors):
+                ctx.vjp, ctx.jvp_fn = vjp, jvp
                 res = run(list(tensors))
                 ctx.stripped = isinstance(res, tuple)
                 if ctx.stripped:
@@ -680,21 +764,29 @@ def _differentiable(torch, run, vjp, tensors):
                     ctx.save_for_backward(*tensors, res[1])
                 else:
                     ctx.save_for_backward(*tensors)
+                    if jvp is not None:
+                        ctx.save_for_forward(*tensors)
                 return res
 
             @staticmethod
             @once_differentiable
             def backward(ctx, grad, *_grad_e):
-                wrt = [i for i, need in enumerate(ctx.needs_input_grad[2:]) if need]
+                wrt = [i for i, need in enumerate(ctx.needs_input_grad[3:]) if need]
                 saved = list(ctx.saved_tensors)
                 if ctx.stripped:
                     grads = ctx.vjp(saved[:-1], grad, wrt, saved[-1])
                 else:
                     grads = ctx.vjp(saved, grad, wrt)
-                return (None, None, *grads)
+                return (None, None, None, *grads)
+
+            @staticmethod
+            def jvp(ctx, _run_t, _vjp_t, _jvp_t, *tangents):
+                if ctx.jvp_fn is None:
+                    return (None, None) if ctx.stripped else None
+                return ctx.jvp_fn(list(ctx.saved_tensors), list(tangents))
 
         _GRAD_FN = _Contract
-    return _GRAD_FN.apply(run, vjp, *tensors)
+    return _GRAD_FN.apply(run, vjp, jvp, *tensors)
 
 
 def gen_output_chunks(tree, arrays, with_key=False, strip_exponent=False, dtype=None, precision="3xtf32",

@@ -151,8 +151,10 @@ bool stream_desc_fits(const int64_t* h, int nmax, int kmax) {
 // fused strip_exponent (scale the product or measure C's factor): the STRIP instantiations
 bool desc_stripped(const int64_t* h) { return h[W_SCALE_A] != 0 || h[W_FACTOR_C] != 0; }
 
+// A2, B2 non-null: the two-term form C (+)= A.B + A2.B2 (stream_rows.cuh)
 template <typename T>
-int launch_rowstream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
+int launch_rowstream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st,
+                     const void* A2 = nullptr, const void* B2 = nullptr) {
   DevInfo& di = devinfo();
   if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
   const int N = (int)h[W_NTA], K = (int)h[W_KTA];
@@ -166,15 +168,21 @@ int launch_rowstream(const int64_t* h, const int64_t* d, const void* A, const vo
   const T* b = (const T*)B;
   T* c = (T*)C;
   const bool strip = desc_stripped(h);
-  if (N <= 4 && K <= 4) {
-    if (strip) rowstream_kernel<T, 4, 4, true, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
-    else rowstream_kernel<T, 4, 4, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
+  if (A2) {
+    const T* a2 = (const T*)A2;
+    const T* b2 = (const T*)B2;
+    if (N <= 4 && K <= 4) rowstream_kernel<T, 4, 4, false, false, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, a2, b2);
+    else if (N <= 2) rowstream_kernel<T, 2, 8, false, false, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, a2, b2);
+    else rowstream_kernel<T, 8, 8, false, false, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, a2, b2);
+  } else if (N <= 4 && K <= 4) {
+    if (strip) rowstream_kernel<T, 4, 4, true, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, nullptr, nullptr);
+    else rowstream_kernel<T, 4, 4, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, nullptr, nullptr);
   } else if (N <= 2) {  // (B from shared memory: in registers it costs 154 registers = one block / SM)
-    if (strip) rowstream_kernel<T, 2, 8, sizeof(T) < 16, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
-    else rowstream_kernel<T, 2, 8, sizeof(T) < 16><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
+    if (strip) rowstream_kernel<T, 2, 8, sizeof(T) < 16, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, nullptr, nullptr);
+    else rowstream_kernel<T, 2, 8, sizeof(T) < 16><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, nullptr, nullptr);
   } else {
-    if (strip) rowstream_kernel<T, 8, 8, false, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
-    else rowstream_kernel<T, 8, 8, false><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c);
+    if (strip) rowstream_kernel<T, 8, 8, false, true><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, nullptr, nullptr);
+    else rowstream_kernel<T, 8, 8, false><<<(unsigned)blocks, 256, 0, st>>>(d, a, b, c, nullptr, nullptr);
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   CUDA_TRY(cudaGetLastError());
@@ -182,7 +190,8 @@ int launch_rowstream(const int64_t* h, const int64_t* d, const void* A, const vo
 }
 
 template <typename T>
-int launch_rowstream_longk(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
+int launch_rowstream_longk(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st,
+                           const void* A2 = nullptr, const void* B2 = nullptr) {
   DevInfo& di = devinfo();
   if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
   if constexpr (sizeof(T) > 8) {
@@ -207,10 +216,14 @@ int launch_rowstream_longk(const int64_t* h, const int64_t* d, const void* A, co
     const unsigned long long cap = (unsigned long long)di.sms * 6;
     if (blocks > cap) blocks = cap;
     if (blocks == 0) return CTGB_OK;
-    if (desc_stripped(h))
-      rowstream_longk_kernel<T, true><<<(unsigned)blocks, 256, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C);
+    if (A2)
+      rowstream_longk_kernel<T, false, true><<<(unsigned)blocks, 256, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C,
+                                                                             (const T*)A2, (const T*)B2);
+    else if (desc_stripped(h))
+      rowstream_longk_kernel<T, true><<<(unsigned)blocks, 256, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C, nullptr,
+                                                                       nullptr);
     else
-      rowstream_longk_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C);
+      rowstream_longk_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(d, (const T*)A, (const T*)B, (T*)C, nullptr, nullptr);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     CUDA_TRY(cudaGetLastError());
     return CTGB_OK;
@@ -260,13 +273,16 @@ struct DsLaunch {
   unsigned long long blocks = 0;    // CTAs (0: nothing to launch)
 };
 
-int dmmastream_launch_config(const int64_t* h, int sms, DsLaunch& lc) {
+// (two: the two-term form, whose k range is ds_two_kb)
+int dmmastream_launch_config(const int64_t* h, int sms, DsLaunch& lc, bool two = false) {
   const int N = (int)h[W_NTA];
-  if (h[W_DTYPE] != CTGB_C128 || !stream_desc_fits(h, 64, N <= 32 ? DS_KMAX : DS_KMAX_WIDE))
-    return fail(CTGB_E_VALUE, "descriptor does not fit the DMMA stream kernel");
-  const unsigned long long M = stream_row_count(h);
   // 64 accumulator doubles per lane at most: 32-row warp blocks up to N = 32, 16-row ones beyond
   lc.nj = N <= 8 ? 1 : N <= 16 ? 2 : N <= 32 ? 4 : 8;
+  const int kmax = two ? ds_two_kb(lc.nj) : N <= 32 ? DS_KMAX : DS_KMAX_WIDE;
+  if (h[W_DTYPE] != CTGB_C128 || !stream_desc_fits(h, 64, kmax))
+    return fail(CTGB_E_VALUE, two ? "descriptor does not fit the two-term DMMA stream kernel"
+                                  : "descriptor does not fit the DMMA stream kernel");
+  const unsigned long long M = stream_row_count(h);
   lc.rows = lc.nj <= 4 ? 32 : 16;
   const unsigned long long per = 4ull * lc.rows;  // 4 warps per block and pass
   lc.blocks = (M + per - 1) / per;
@@ -277,26 +293,28 @@ int dmmastream_launch_config(const int64_t* h, int sms, DsLaunch& lc) {
 
 template <int NJ, int RG>
 void dmmastream_launch(bool strip, unsigned blocks, const int64_t* d, const double2* a, const double2* b, double2* c,
-                       cudaStream_t st) {
-  if (strip) dmmastream_kernel<NJ, RG, true><<<blocks, 128, 0, st>>>(d, a, b, c);
-  else dmmastream_kernel<NJ, RG><<<blocks, 128, 0, st>>>(d, a, b, c);
+                       const double2* a2, const double2* b2, cudaStream_t st) {
+  if (a2) dmmastream_kernel<NJ, RG, false, true><<<blocks, 128, 0, st>>>(d, a, b, c, a2, b2);
+  else if (strip) dmmastream_kernel<NJ, RG, true><<<blocks, 128, 0, st>>>(d, a, b, c, nullptr, nullptr);
+  else dmmastream_kernel<NJ, RG><<<blocks, 128, 0, st>>>(d, a, b, c, nullptr, nullptr);
 }
 
-int launch_dmmastream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st) {
+int launch_dmmastream(const int64_t* h, const int64_t* d, const void* A, const void* B, void* C, cudaStream_t st,
+                      const void* A2 = nullptr, const void* B2 = nullptr) {
   DevInfo& di = devinfo();
   if (!di.ok) return fail(CTGB_E_CUDA, "no CUDA device");
   DsLaunch lc;
-  if (int rc = dmmastream_launch_config(h, di.sms, lc)) return rc;
+  if (int rc = dmmastream_launch_config(h, di.sms, lc, A2 != nullptr)) return rc;
   if (lc.blocks == 0) return CTGB_OK;
   const bool strip = desc_stripped(h);
-  const double2 *a = (const double2*)A, *b = (const double2*)B;
+  const double2 *a = (const double2*)A, *b = (const double2*)B, *a2 = (const double2*)A2, *b2 = (const double2*)B2;
   double2* c = (double2*)C;
   const unsigned blocks = (unsigned)lc.blocks;
   switch (lc.nj) {
-    case 1: dmmastream_launch<1, 4>(strip, blocks, d, a, b, c, st); break;
-    case 2: dmmastream_launch<2, 4>(strip, blocks, d, a, b, c, st); break;
-    case 4: dmmastream_launch<4, 4>(strip, blocks, d, a, b, c, st); break;
-    default: dmmastream_launch<8, 2>(strip, blocks, d, a, b, c, st); break;
+    case 1: dmmastream_launch<1, 4>(strip, blocks, d, a, b, c, a2, b2, st); break;
+    case 2: dmmastream_launch<2, 4>(strip, blocks, d, a, b, c, a2, b2, st); break;
+    case 4: dmmastream_launch<4, 4>(strip, blocks, d, a, b, c, a2, b2, st); break;
+    default: dmmastream_launch<8, 2>(strip, blocks, d, a, b, c, a2, b2, st); break;
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   CUDA_TRY(cudaGetLastError());
@@ -647,6 +665,33 @@ int launch_gett(const int64_t* h, const int64_t* d, const void* A, const void* B
   return fail(CTGB_E_VALUE, "bad dtype");
 }
 
+// The two-term node C (+)= A.B + A2.B2 (A2 laid out as A, B2 as B) in one launch: the row-stream and
+// DMMA stream kernels only, unstripped and with C of the plan dtype
+template <typename T>
+int launch_gett2_typed(const int64_t* h, const int64_t* d, const void* A, const void* B, const void* A2,
+                       const void* B2, void* C, cudaStream_t st) {
+  const int variant = (int)h[W_VARIANT];
+  if (variant == VAR_ROWSTREAM) return launch_rowstream<T>(h, d, A, B, C, st, A2, B2);
+  if (variant == VAR_ROWSTREAM_K) return launch_rowstream_longk<T>(h, d, A, B, C, st, A2, B2);
+  if (variant == VAR_DMMASTREAM) return launch_dmmastream(h, d, A, B, C, st, A2, B2);
+  return fail(CTGB_E_VALUE, "the two-term form runs on the row-stream and DMMA stream kernels only");
+}
+
+int launch_gett2(const int64_t* h, const int64_t* d, const void* A, const void* B, const void* A2, const void* B2,
+                 void* C, cudaStream_t st) {
+  if (h[W_MAGIC] != DESC_MAGIC) return fail(CTGB_E_VALUE, "bad pair descriptor magic");
+  if (!A2 || !B2) return fail(CTGB_E_VALUE, "the two-term form needs both A2 and B2");
+  if (desc_stripped(h)) return fail(CTGB_E_VALUE, "the two-term form takes unstripped descriptors");
+  if (h[W_FLAGS] & FLAG_WIDE_C) return fail(CTGB_E_VALUE, "the two-term form has no wide C");
+  switch ((int)h[W_DTYPE]) {
+    case CTGB_F32: return launch_gett2_typed<float>(h, d, A, B, A2, B2, C, st);
+    case CTGB_F64: return launch_gett2_typed<double>(h, d, A, B, A2, B2, C, st);
+    case CTGB_C64: return launch_gett2_typed<float2>(h, d, A, B, A2, B2, C, st);
+    case CTGB_C128: return launch_gett2_typed<double2>(h, d, A, B, A2, B2, C, st);
+  }
+  return fail(CTGB_E_VALUE, "bad dtype");
+}
+
 template <typename T>
 int launch_single_typed(const int64_t* h, const int64_t* d, const void* X, void* out, cudaStream_t st) {
   long long n = h[S_OUT_ELEMS];
@@ -792,6 +837,8 @@ struct ctgb_tensor_rec {
 struct ctgb_slice_mem {
   const void* const* inputs = nullptr;  // kind 0
   void* const* grads = nullptr;         // kind 5
+  const void* const* tangents = nullptr;  // kind 7
+  char* tout = nullptr;                 // kind 8
   char* persistent = nullptr;           // kinds 2, 6
   char* scratch = nullptr;              // kind 1
   char* out = nullptr;                  // kind 3
@@ -814,6 +861,8 @@ static char* resolve_tensor(const ctgb_tensor_rec& q, const ctgb_slice_mem& m, i
     case 6: return m.persistent + q.offset;
     case 4: return (char*)m.cot + out_off * (int64_t)m.es;
     case 5: return sliced(m.grads[q.input_index]);
+    case 7: return sliced(m.tangents[q.input_index]);
+    case 8: return m.tout + out_off * (int64_t)m.out_es;
     default: return m.out + out_off * (int64_t)m.out_es;
   }
 }
@@ -850,7 +899,7 @@ static int copy_tensors(const ctgb_tensor* ts, int n, int n_inputs, int n_sliced
     q.input_index = t.input_index;
     q.offset = t.offset;
     q.nbytes = t.nbytes;
-    if ((t.kind == 0 || t.kind == 5) && (t.input_index < 0 || t.input_index >= n_inputs))
+    if ((t.kind == 0 || t.kind == 5 || t.kind == 7) && (t.input_index < 0 || t.input_index >= n_inputs))
       return fail(CTGB_E_VALUE, "tensor refers to a missing input");
     for (int j = 0; j < t.n_sliced; ++j) {
       if (t.slice_pos[j] < 0 || t.slice_pos[j] >= n_sliced) return fail(CTGB_E_VALUE, "slice position out of range");
@@ -871,6 +920,7 @@ struct ctgb_plan {
   using Tensor = ctgb_tensor_rec;
   struct Node {
     int kind, a, b, c, phase, zero_fill, is_root;
+    int a2 = -1, b2 = -1;  // two-term node (kind 2): the slots of A' and B'
     size_t desc_off;  // word offset into descs
     int64_t c_elems;  // dense elements of the result (strip_exponent)
     int measure_after = 0;  // strip_exponent: max|C| needs its own pass (split-K / block partial sums)
@@ -892,6 +942,10 @@ struct ctgb_plan {
   bool wide_desc = false;           // a descriptor carries FLAG_WIDE_C: runs only with a wide accumulator
   int root = -1;                    // the node that writes the output
   bool backward = false;            // phase 2/3 nodes: needs a cotangent and the gradient buffers
+  // forward-mode plans (tangent slots, two-term nodes): run by ctgb_plan_execute_jvp
+  bool jvp = false;
+  int troot = -1;                   // a node that writes the root's tangent (is_root = 2)
+  std::vector<char> needs_tangent;  // per input: a kind-7 slot reads its tangent
   int64_t cot_offset = -1;          // conjugated cotangent copy in the persistent arena
   std::vector<int64_t> grad_elems;  // per input: elements of its gradient (0: not differentiated)
   int64_t launches_per_slice = 0;
@@ -1080,6 +1134,18 @@ int ctgb_contract_pair(const int64_t* desc, const void* A, const void* B, void* 
   return rc;
 }
 
+int ctgb_contract_pair2(const int64_t* desc, const void* A, const void* B, const void* A2, const void* B2, void* C,
+                        void* stream) {
+  if (!desc) return fail(CTGB_E_VALUE, "null descriptor");
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t* d = nullptr;
+  CUDA_TRY(cudaMallocAsync((void**)&d, DESC_WORDS * sizeof(int64_t), st));
+  CUDA_TRY(cudaMemcpyAsync(d, desc, DESC_WORDS * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  int rc = launch_gett2(desc, d, A, B, A2, B2, C, st);
+  cudaFreeAsync(d, st);
+  return rc;
+}
+
 int ctgb_absorb_root(const int64_t* desc, const void* A, const void* Bs, const void* V, void* C, void* stream) {
   if (!desc || desc[0] != DESC_MAGIC || desc[W_VARIANT] != VAR_ABSORB_ROOT)
     return fail(CTGB_E_VALUE, "not an absorb-root descriptor");
@@ -1130,18 +1196,30 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     q.phase = n.phase;
     q.zero_fill = n.zero_fill;
     q.is_root = n.is_root;
-    const int words = n.kind == 0 ? (int)DESC_WORDS : (int)SDESC_WORDS;
-    const int64_t magic = n.kind == 0 ? DESC_MAGIC : SDESC_MAGIC;
-    if (n.kind < 0 || n.kind > 1 || !n.desc || n.desc[0] != magic) return refuse("bad node descriptor");
+    // (a two-term node: the pair words, then the slots of A' and B')
+    const int words = n.kind == 0 ? (int)DESC_WORDS : n.kind == 2 ? (int)DESC_WORDS + 2 : (int)SDESC_WORDS;
+    const int64_t magic = n.kind == 1 ? SDESC_MAGIC : DESC_MAGIC;
+    if (n.kind < 0 || n.kind > 2 || !n.desc || n.desc[0] != magic) return refuse("bad node descriptor");
     if (n.phase < 0 || n.phase > 3) return refuse("bad node phase");
+    if (n.is_root < 0 || n.is_root > 2) return refuse("bad node root mark");
     auto bad = [&](int t) { return t < 0 || t >= pd->n_tensors; };
-    if (bad(n.a) || bad(n.c) || (n.kind == 0 && bad(n.b))) return refuse("node refers to a missing tensor");
+    if (bad(n.a) || bad(n.c) || (n.kind != 1 && bad(n.b))) return refuse("node refers to a missing tensor");
+    if (n.kind == 2) {
+      const int64_t v = n.desc[W_VARIANT];
+      if (v != VAR_ROWSTREAM && v != VAR_ROWSTREAM_K && v != VAR_DMMASTREAM)
+        return refuse("a two-term node runs on the row-stream and DMMA stream kernels only");
+      if (bad((int)n.desc[DESC_WORDS]) || bad((int)n.desc[DESC_WORDS + 1])) return refuse("node refers to a missing tensor");
+      q.a2 = (int)n.desc[DESC_WORDS];
+      q.b2 = (int)n.desc[DESC_WORDS + 1];
+    }
+    p->jvp |= n.kind == 2 || n.is_root == 2;
     if (n.kind == 0 && n.desc[W_VARIANT] == VAR_ABSORB_ROOT) {
       if (bad((int)n.desc[AB_BS_SLOT])) return refuse("node refers to a missing tensor");
       if (pd->strip_exponent) return refuse("an absorb-root node runs in unstripped plans only");
     }
     p->backward |= n.phase >= 2;
-    if (n.is_root) p->root = i;
+    if (n.is_root == 1) p->root = i;
+    if (n.is_root == 2) p->troot = i;
     if (n.kind == 0 && (n.desc[W_FLAGS] & FLAG_WIDE_C)) {
       if (!n.is_root || pd->strip_exponent) return refuse("a wide C belongs to the root of an unstripped plan");
       p->wide_desc = true;
@@ -1166,10 +1244,15 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
   // kind 3 (the output) belongs to forward plans, kinds 4-6 (cotangent, gradients, H accumulators) to
   // reverse-mode ones: execute checks exactly the buffers the plan's kind needs
   p->grad_elems.assign(pd->n_inputs, 0);
+  p->needs_tangent.assign(pd->n_inputs, 0);
+  for (const auto& q : p->tensors) p->jvp |= q.kind >= 7;
+  if (p->jvp && (p->backward || pd->strip_exponent)) return refuse("a forward-mode plan has phases 0 and 1, unstripped");
   for (const auto& q : p->tensors) {
-    if (q.kind < 0 || q.kind > 6 || (q.kind == 3 && p->backward) || (q.kind >= 4 && !p->backward))
+    const bool rev = q.kind >= 4 && q.kind <= 6, fwd = q.kind >= 7;
+    if (q.kind < 0 || q.kind > 8 || (q.kind == 3 && p->backward) || (rev && !p->backward) || (fwd && !p->jvp))
       return refuse("bad tensor kind for the plan's phases");
     if (q.kind == 5) p->grad_elems[q.input_index] = q.nbytes / (int64_t)es;
+    if (q.kind == 7) p->needs_tangent[q.input_index] = 1;
   }
   const bool cplx = pd->dtype == CTGB_C64 || pd->dtype == CTGB_C128;
   if (cplx && p->backward && pd->cotangent_offset < 0)
@@ -1286,7 +1369,7 @@ int ctgb_plan_set_accumulator(ctgb_plan* p, int32_t dtype) {
     if (p->root < 0) return fail(CTGB_E_VALUE, "plan has no root node");
     const int ckind = p->tensors[p->nodes[p->root].c].kind;
     if (ckind != (p->wide_desc ? 3 : 1)) return fail(CTGB_E_VALUE, "root slot does not match the wide accumulator");
-    if (!p->wide_desc && p->acc_dtype == p->dtype) p->launches_per_slice += 1;
+    if (!p->wide_desc && p->acc_dtype == p->dtype) p->launches_per_slice += p->troot >= 0 ? 2 : 1;
   } else if (p->wide_desc) {
     return fail(CTGB_E_VALUE, "the plan's root descriptor needs a wide accumulator");
   }
@@ -1313,10 +1396,14 @@ int ctgb_plan_set_scale_slots(ctgb_plan* p, const int32_t* slot_a, const int32_t
   return CTGB_OK;
 }
 
-int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double* exponent_dev,
-                      const void* cotangent, void* const* grads, void* workspace, size_t workspace_bytes,
-                      int64_t slice_begin, int64_t slice_step, int64_t slice_count, void* stream) {
-  if (!p) return fail(CTGB_E_VALUE, "null plan");
+}  // extern "C"
+
+// ctgb_plan_execute and ctgb_plan_execute_jvp: `tangents` and `tangent_out` belong to forward-mode
+// plans, whose primal root is skipped when `out` is null
+static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* tangents, void* out,
+                    void* tangent_out, double* exponent_dev, const void* cotangent, void* const* grads,
+                    void* workspace, size_t workspace_bytes, int64_t slice_begin, int64_t slice_step,
+                    int64_t slice_count, void* stream) {
   if (workspace_bytes < (size_t)(p->workspace_bytes + p->persistent_bytes))
     return fail(CTGB_E_MEMORY, "workspace too small");
   if (!inputs) return fail(CTGB_E_VALUE, "null inputs");
@@ -1334,6 +1421,10 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   for (int i = 0; i < p->n_inputs; ++i)
     if (p->grad_elems[i] > 0 && (!grads || !grads[i]))
       return fail(CTGB_E_VALUE, "missing gradient buffer of a differentiated input");
+  for (int i = 0; i < p->n_inputs; ++i)
+    if (p->needs_tangent[i] && (!tangents || !tangents[i]))
+      return fail(CTGB_E_VALUE, "missing tangent of an input the plan differentiates");
+  if (p->jvp && !tangent_out) return fail(CTGB_E_VALUE, "a forward-mode plan needs a tangent output");
   cudaStream_t st = (cudaStream_t)stream;
   const size_t es = elem_size(p->dtype);
   char* persistent = (char*)workspace;
@@ -1346,6 +1437,8 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   ctgb_slice_mem mem;
   mem.inputs = inputs;
   mem.grads = grads;
+  mem.tangents = tangents;
+  mem.tout = (char*)tangent_out;
   mem.persistent = persistent;
   mem.scratch = scratch;
   mem.out = (char*)out;
@@ -1368,11 +1461,12 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
     for (size_t ni = 0; ni < p->nodes.size(); ++ni) {
       const auto& n = p->nodes[ni];
       if (n.phase != phase) continue;
+      if (n.is_root == 1 && p->jvp && !out) continue;  // forward mode without the primal
       if (p->profile) cudaEventRecord(p->ev0[ni], st);
       const int64_t* h = p->descs.data() + n.desc_off;
       const int64_t* d = p->d_descs + n.desc_off;
       char* A = resolve(n.a, out_off);
-      char* B = n.kind == 0 ? resolve(n.b, out_off) : nullptr;
+      char* B = n.kind != 1 ? resolve(n.b, out_off) : nullptr;  // (pairwise and two-term nodes)
       char* C = resolve(n.c, out_off);
       if (n.zero_fill) CUDA_TRY(cudaMemsetAsync(C, 0, (size_t)p->tensors[n.c].nbytes, st));
       // the whole underlying buffer of an operand (a sliced input, or the cotangent's slice view,
@@ -1400,7 +1494,9 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
           return r;
         A = p->d_bscale + (A - base);
       }
-      if (n.kind == 0 && h[W_VARIANT] == VAR_ABSORB_ROOT) {
+      if (n.kind == 2) {
+        if (int r = launch_gett2(h, d, A, B, resolve(n.a2, out_off), resolve(n.b2, out_off), C, st)) return r;
+      } else if (n.kind == 0 && h[W_VARIANT] == VAR_ABSORB_ROOT) {
         if (int r = launch_absorb_root(h, d, A, resolve((int)h[AB_BS_SLOT], out_off), B, C, st)) return r;
       } else if (int r = launch_node(n.kind, h, d, A, B, C, st)) {
         return r;
@@ -1463,9 +1559,15 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
                           froot, st);
       if (rc) return rc;
     }
-    if (wide_fold) {
+    if (wide_fold && out) {
       rc = add_chunk_wide(p->dtype, p->d_chunk_desc, p->chunk_desc.data(), (char*)out + out_off * (int64_t)mem.out_es,
                           resolve(p->nodes[p->root].c, 0), st);
+      if (rc) return rc;
+    }
+    if (wide_fold && p->troot >= 0) {
+      // the root's tangent, stored densely as the root is, into its chunk of the tangent output
+      rc = add_chunk_wide(p->dtype, p->d_chunk_desc, p->chunk_desc.data(),
+                          (char*)tangent_out + out_off * (int64_t)mem.out_es, resolve(p->nodes[p->troot].c, 0), st);
       if (rc) return rc;
     }
   }
@@ -1475,6 +1577,26 @@ int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double
   for (int i = 0; i < p->n_inputs; ++i)
     if (p->grad_elems[i] > 0 && (rc = conj_inplace(p->dtype, grads[i], p->grad_elems[i], st))) return rc;
   return CTGB_OK;
+}
+
+extern "C" {
+
+int ctgb_plan_execute(ctgb_plan* p, const void* const* inputs, void* out, double* exponent_dev,
+                      const void* cotangent, void* const* grads, void* workspace, size_t workspace_bytes,
+                      int64_t slice_begin, int64_t slice_step, int64_t slice_count, void* stream) {
+  if (!p) return fail(CTGB_E_VALUE, "null plan");
+  if (p->jvp) return fail(CTGB_E_VALUE, "a forward-mode plan runs through ctgb_plan_execute_jvp");
+  return plan_run(p, inputs, nullptr, out, nullptr, exponent_dev, cotangent, grads, workspace, workspace_bytes,
+                  slice_begin, slice_step, slice_count, stream);
+}
+
+int ctgb_plan_execute_jvp(ctgb_plan* p, const void* const* inputs, const void* const* tangents, void* out,
+                          void* tangent_out, void* workspace, size_t workspace_bytes, int64_t slice_begin,
+                          int64_t slice_step, int64_t slice_count, void* stream) {
+  if (!p) return fail(CTGB_E_VALUE, "null plan");
+  if (!p->jvp) return fail(CTGB_E_VALUE, "not a forward-mode plan");
+  return plan_run(p, inputs, tangents, out, tangent_out, nullptr, nullptr, nullptr, workspace, workspace_bytes,
+                  slice_begin, slice_step, slice_count, stream);
 }
 
 int ctgb_plan_execute_host(ctgb_plan* p, const void* const* host_inputs, const int64_t* input_nbytes, void* host_out,

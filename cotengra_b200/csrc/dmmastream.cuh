@@ -21,17 +21,25 @@ constexpr int DS_KMAX_WIDE = 32;  // ... for NJ = 8 (64 x 64 complex doubles wou
 // NJ = 8 at 16 rows: both 64 accumulator doubles per lane).  NJ = 1 serves skinny nodes
 // whose contracted space is too long for the row-stream kernel (N <= 8, 8 < K <= 64: the staged
 // row policy ran the M = 2^22, N = 8, K = 64 node of the Sycamore slice at 0.57 of its roofline)
-template <int NJ, int RG, bool STRIP = false>
+// The two-term form (TWO: C (+)= A.B + A2.B2) holds copies of B and B2: with both within the 48 KB of
+// static shared memory its k range is shorter for the wide instantiations (ds_two_kb)
+__host__ __device__ constexpr int ds_two_kb(int nj) { return nj <= 2 ? DS_KMAX : nj == 4 ? 32 : 16; }
+
+template <int NJ, int RG, bool STRIP = false, bool TWO = false>
 __global__ void __launch_bounds__(128, NJ <= 2 ? 3 : 2)
 dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, const double2* __restrict__ B,
-                  double2* __restrict__ C) {
+                  double2* __restrict__ C, const double2* __restrict__ A2, const double2* __restrict__ B2) {
   static_assert(RG == 2 || RG == 4, "a warp block is one or two m16 fragment pairs");
-  constexpr int DS_NMAX = NJ * 8, DS_KB = NJ <= 4 ? DS_KMAX : DS_KMAX_WIDE, ROWS = RG * 8;
+  static_assert(!TWO || !STRIP, "the two-term form is unstripped");
+  constexpr int DS_NMAX = NJ * 8, ROWS = RG * 8;
+  constexpr int DS_KB = TWO ? ds_two_kb(NJ) : NJ <= 4 ? DS_KMAX : DS_KMAX_WIDE;
   // s.B: [k][n], zero beyond (K, N); the launcher keeps K <= DS_KB
   STREAM_TABLES(double2, DS_KMAX, DS_NMAX, DS_KB);
+  __shared__ double2 s_B2[TWO ? DS_KB * DS_NMAX : 1];
   const int tid = threadIdx.x, lane = tid & 31;
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
   const int n_m = s.load(D, B, K, N);
+  if constexpr (TWO) s.copy_b(B2, s_B2, K, N);
   // (the flags after the tables: read before them, ptxas gives <8, 2, true> 248 registers, not 244)
   const StreamFlags f = stream_flags<double2>(D);
 
@@ -59,7 +67,12 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
     for (int i = 0; i < RG; ++i)
 #pragma unroll
       for (int j = 0; j < NJ; ++j) re[i][j][0] = re[i][j][1] = im[i][j][0] = im[i][j][1] = 0.0;
-    for (int kc = 0; kc < kchunks; ++kc) {
+    // (TWO: the k chunks of A2.B2 follow those of A.B into the same accumulators)
+    for (int kt = 0; kt < (TWO ? 2 : 1) * kchunks; ++kt) {
+      const bool second = TWO && kt >= kchunks;
+      const int kc = second ? kt - kchunks : kt;
+      const double2* __restrict__ At = second ? A2 : A;
+      const double2* Bt = second ? s_B2 : s.B;
       // 8*RG independent 64-bit loads per lane: element (row i*8 + frow, k = kc*16 + k4*4 + fk).
       // Not one 128-bit load per element: an m16n8k4 A operand is the real (or imaginary)
       // parts of two rows in adjacent registers, and 128-bit loads make ptxas copy them
@@ -72,7 +85,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
         const bool kin = kk < K;
 #pragma unroll
         for (int i = 0; i < RG; ++i) {
-          const double* pa = reinterpret_cast<const double*>(A + oa[i] + ko);
+          const double* pa = reinterpret_cast<const double*>(At + oa[i] + ko);
           a[i][k4].x = kin ? __ldg(pa) : 0.0;
           a[i][k4].y = kin ? __ldg(pa + 1) : 0.0;
         }
@@ -83,7 +96,7 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
         // B fragment: lane holds B[k = .. + fk][n = j*8 + frow]
         double2 b[NJ];
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) b[j] = s.B[(kc * 16 + k4 * 4 + fk) * DS_NMAX + j * 8 + frow];
+        for (int j = 0; j < NJ; ++j) b[j] = Bt[(kc * 16 + k4 * 4 + fk) * DS_NMAX + j * 8 + frow];
 #pragma unroll
         for (int i = 0; i < RG; i += 2)
 #pragma unroll

@@ -12,14 +12,20 @@
 
 // STRIP: fused strip_exponent (a separate instantiation: its few live registers would spill
 // inside the row loop of the register-bound variants otherwise)
-template <typename T, int NMAX, int KMAX, bool BREG, bool STRIP = false>
-__global__ void __launch_bounds__(256, BREG ? 2 : 3)
-rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B, T* __restrict__ C) {
+// TWO: C (+)= A.B + A2.B2 (stream_rows.cuh), B2 from shared memory, two blocks per SM (the A2 row
+// doubles the operand registers); not with BREG or STRIP
+template <typename T, int NMAX, int KMAX, bool BREG, bool STRIP = false, bool TWO = false>
+__global__ void __launch_bounds__(256, (BREG || TWO) ? 2 : 3)
+rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B, T* __restrict__ C,
+                 const T* __restrict__ A2, const T* __restrict__ B2) {
+  static_assert(!TWO || (!BREG && !STRIP), "the two-term form reads B' from shared memory, unstripped");
   STREAM_TABLES(T, KMAX, NMAX, KMAX);
+  __shared__ T s_B2[TWO ? KMAX * NMAX : 1];
   const int tid = threadIdx.x;
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
   const StreamFlags f = stream_flags<T>(D);
   const int n_m = s.load(D, B, K, N);
+  if constexpr (TWO) s.copy_b(B2, s_B2, K, N);
   [[maybe_unused]] T breg[BREG ? KMAX : 1][BREG ? NMAX : 1];
   if constexpr (BREG) {
 #pragma unroll
@@ -48,11 +54,15 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
       s.row(n_m, f.pow2, live[i] ? (unsigned)m : 0u, oa[i], oc[i]);
     }
     T a[R][KMAX];
+    [[maybe_unused]] T a2[TWO ? R : 1][TWO ? KMAX : 1];
 #pragma unroll
     for (int i = 0; i < R; ++i)
 #pragma unroll
       for (int kk = 0; kk < KMAX; ++kk)
-        if (kk < K) a[i][kk] = A[oa[i] + akoff[kk]];
+        if (kk < K) {
+          a[i][kk] = A[oa[i] + akoff[kk]];
+          if constexpr (TWO) a2[i][kk] = A2[oa[i] + akoff[kk]];
+        }
     // 16-byte types read s.B afresh for every row: through an index the compiler cannot see
     // through, which keeps it from hoisting all KMAX x NMAX reads out of the row loop (for N = K = 8,
     // 64 complex128 values = 256 registers: ptxas spilled them to a 984-byte stack frame and the
@@ -86,6 +96,15 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
             }
           }
         }
+        if constexpr (TWO) {
+#pragma unroll
+          for (int kk = 0; kk < KMAX; ++kk)
+            if (kk < K) {
+#pragma unroll
+              for (int c = 0; c < CH; ++c)
+                if (c0 + c < N) mac(acc[c], a2[i][kk], s_B2[sb0 + kk * NMAX + c0 + c]);
+            }
+        }
         if constexpr (STRIP) strip_row(sctx, acc, c0, N);
         store_row<true>(pc, s.cnoff, acc, c0, N, f);
       }
@@ -103,15 +122,19 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
 // memory, the 8 accumulators of a row stay in registers across the chunks.
 constexpr int RSK_KMAX = 64, RSK_NMAX = 8;
 
-template <typename T, bool STRIP = false>
+// TWO: C (+)= A.B + A2.B2, the chunks of A2 after those of A into the same accumulators
+template <typename T, bool STRIP = false, bool TWO = false>
 __global__ void __launch_bounds__(256, 3)
 rowstream_longk_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B,
-                       T* __restrict__ C) {
+                       T* __restrict__ C, const T* __restrict__ A2, const T* __restrict__ B2) {
+  static_assert(!TWO || !STRIP, "the two-term form is unstripped");
   STREAM_TABLES(T, RSK_KMAX, RSK_NMAX, RSK_KMAX);
+  __shared__ T s_B2[TWO ? RSK_KMAX * RSK_NMAX : 1];
   const int tid = threadIdx.x;
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
   const StreamFlags f = stream_flags<T>(D);
   const int n_m = s.load(D, B, K, N);
+  if constexpr (TWO) s.copy_b(B2, s_B2, K, N);
   long long inoff[8];  // offsets inside a chunk of 8 k
 #pragma unroll
   for (int kk = 0; kk < 8; ++kk) inoff[kk] = s.akoff[kk];
@@ -135,18 +158,22 @@ rowstream_longk_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, c
     for (int i = 0; i < R; ++i)
 #pragma unroll
       for (int c = 0; c < RSK_NMAX; ++c) acc[i][c] = zero_of<T>();
-    for (int kc = 0; kc < nchunks; ++kc) {
+    for (int kt = 0; kt < (TWO ? 2 : 1) * nchunks; ++kt) {
+      const bool second = TWO && kt >= nchunks;
+      const int kc = second ? kt - nchunks : kt;
+      const T* __restrict__ At = second ? A2 : A;
+      const T* Bt = second ? s_B2 : s.B;
       const long long cb = s.akoff[kc * 8];  // chunk base (in_chunk[0] is 0)
       T a[R][8];
 #pragma unroll
       for (int i = 0; i < R; ++i)
 #pragma unroll
-        for (int kk = 0; kk < 8; ++kk) a[i][kk] = (kc * 8 + kk < K) ? A[oa[i] + cb + inoff[kk]] : zero_of<T>();
+        for (int kk = 0; kk < 8; ++kk) a[i][kk] = (kc * 8 + kk < K) ? At[oa[i] + cb + inoff[kk]] : zero_of<T>();
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk)
 #pragma unroll
         for (int c = 0; c < RSK_NMAX; ++c) {
-          const T b = s.B[(kc * 8 + kk) * RSK_NMAX + c];
+          const T b = Bt[(kc * 8 + kk) * RSK_NMAX + c];
 #pragma unroll
           for (int i = 0; i < R; ++i) mac(acc[i][c], a[i][kk], b);
         }

@@ -3,6 +3,8 @@
 // zero-padded copy of B, the row decoder, and the FMA kernels' fused strip_exponent scan and
 // row store.  Each kernel keeps its own main loop: their register budgets differ (80 to 255
 // registers for two or three blocks per SM) and a shared loop would move the allocation.
+// The two-term instantiations (TWO) form C (+)= A.B + A'.B' for A' laid out as A and B' as B: both
+// products go into the same accumulators before the one row store, so C is written once.
 // (included inside namespace ctgb)
 #pragma once
 
@@ -97,12 +99,18 @@ struct StreamTables {
       cnoff[c] = o;
     }
     __syncthreads();
-    for (int i = tid; i < KB * NMAX; i += blockDim.x) {
+    copy_b(Bg, B, K, N);
+    return n_m;
+  }
+
+  // A zero-padded [KB][NMAX] copy of an operand laid out as B (offsets bkoff, bnoff) into dst; the
+  // two-term kernels make a second one of B'
+  __device__ __forceinline__ void copy_b(const T* __restrict__ Bg, T* dst, int K, int N) const {
+    for (int i = threadIdx.x; i < KB * NMAX; i += blockDim.x) {
       const int kk = i / NMAX, c = i % NMAX;
-      B[i] = (kk < K && c < N) ? Bg[bkoff[kk] + bnoff[c]] : zero_of<T>();
+      dst[i] = (kk < K && c < N) ? Bg[bkoff[kk] + bnoff[c]] : zero_of<T>();
     }
     __syncthreads();
-    return n_m;
   }
 
   // offsets in A and C of row e: its mixed-radix digits over the m dims, by shift and mask when

@@ -19,7 +19,8 @@ Planning is host-side integer work:
 
 Every node carries the phase it runs in: 0 (invariant forward, once per call)
 and 1 (variant forward, per slice) here; a reverse-mode plan (``vjp.py``) adds
-2 (variant backward) and 3 (invariant backward).  Both plan kinds are one
+2 (variant backward) and 3 (invariant backward); a forward-mode plan (``jvp.py``)
+adds tangent records to phases 0 and 1.  All plan kinds are one
 ``ctgb_plan`` type, laid out by ``layout`` and marshalled and uploaded by
 ``_DevicePlan``.
 """
@@ -53,6 +54,7 @@ ALIGN = 256
 PHASE_INV_FWD, PHASE_VAR_FWD, PHASE_VAR_BWD, PHASE_INV_BWD = 0, 1, 2, 3
 LOOP_PHASES = (PHASE_VAR_FWD, PHASE_VAR_BWD)  # run once per slice
 K_INPUT, K_SCRATCH, K_PERSISTENT, K_OUTPUT, K_COT, K_GRAD, K_HACC = 0, 1, 2, 3, 4, 5, 6
+K_TANGENT, K_TOUT = 7, 8  # forward mode (jvp.py): an input's tangent, the output's tangent
 
 
 def _align(x):
@@ -164,7 +166,7 @@ def layout(sched, reserve=0):
         c = nd["c"]
         if c.first_use is None:
             c.first_use = zero_pos if c.kind == K_HACC else pos
-        for s in (nd["a"], nd["b"], nd.get("d")):
+        for s in (nd["a"], nd["b"], nd.get("d"), nd.get("a2"), nd.get("b2")):
             if s is None:
                 continue
             s.last_use = max(s.last_use, pos)
@@ -189,7 +191,8 @@ def layout(sched, reserve=0):
 
 def _slots(sched):
     """The slots of a schedule in order of first appearance."""
-    return list(dict.fromkeys(t for nd in sched if nd is not None for t in (nd["a"], nd["b"], nd.get("d"), nd["c"])
+    return list(dict.fromkeys(t for nd in sched if nd is not None
+                              for t in (nd["a"], nd["b"], nd.get("d"), nd.get("a2"), nd.get("b2"), nd["c"])
                               if t is not None))
 
 
@@ -226,6 +229,8 @@ class _DevicePlan:
             words = np.array(nd["words"], dtype=np.int64)
             if nd.get("d") is not None:
                 words[lowering.AB_BS_SLOT] = slot[id(nd["d"])]
+            if nd["kind"] == 2:  # a two-term node: the pair words, then the slots of A' and B'
+                words = np.append(words, [slot[id(nd["a2"])], slot[id(nd["b2"])]]).astype(np.int64)
             keep.append(words)
             cn[i].kind = nd["kind"]
             cn[i].a = slot[id(nd["a"])]

@@ -85,6 +85,16 @@ int ctgb_device_info(int* sm_count, int* cc_major, int* cc_minor,
 int ctgb_contract_pair(const int64_t* desc, const void* A, const void* B,
                        void* C, void* stream);
 
+/* The two-term form of one pairwise node: C (+)= A.B + A2.B2 in one launch, where
+ * A2 has A's index structure and strides and B2 has B's, so the same descriptor
+ * describes both products and C is stored once (accumulated when the descriptor
+ * says so).  Runs on the row-stream and DMMA stream kernels (variants 8, 19 and
+ * 14) with unstripped descriptors; any other descriptor fails with CTGB_E_VALUE.
+ * The DMMA stream kernel's two-term form takes K <= 64 for N <= 16, K <= 32 for
+ * N <= 32 and K <= 16 beyond. */
+int ctgb_contract_pair2(const int64_t* desc, const void* A, const void* B,
+                        const void* A2, const void* B2, void* C, void* stream);
+
 /* One absorb-root node (variant 21, complex128):
  * C[m,n] (+)= sum_{k',c} (sum_k A[m,k',k] Bs[k,c]) V[k',c,n], the result of the
  * absorption A.Bs never formed.  `desc` is a pair-sized word array in the
@@ -110,8 +120,11 @@ typedef struct ctgb_plan ctgb_plan;
  *   4 = the cotangent's view of the slice (element offset as kind 3),
  *   5 = the gradient of network input `input_index` (slice offset as kind 0),
  *   6 = a persistent accumulator at byte offset `offset` of the persistent
- *       arena, zeroed before the slice loop (H of a slice-invariant tensor).
- * Kinds 4-6 belong to reverse-mode plans, kind 3 to forward ones. */
+ *       arena, zeroed before the slice loop (H of a slice-invariant tensor),
+ *   7 = the tangent of network input `input_index` (slice offset as kind 0),
+ *   8 = the tangent output accumulator (at the slice's view, as kind 3).
+ * Kinds 4-6 belong to reverse-mode plans, kind 3 to forward ones, and kinds 7-8
+ * to forward-mode plans (ctgb_plan_execute_jvp), which may also hold kind 3. */
 typedef struct {
   int32_t kind;
   int32_t input_index;
@@ -130,12 +143,15 @@ typedef struct {
  * per-slice values there, right before the backward steps that read them.
  * Each phase runs its nodes in list order, so this needs nothing new here. */
 typedef struct {
-  int32_t kind;       /* 0 = pairwise (desc = pair words), 1 = single-operand   */
+  int32_t kind;       /* 0 = pairwise (desc = pair words), 1 = single-operand,
+                         2 = two-term pairwise (desc = pair words followed by the
+                         slots of A2 and B2: ctgb_contract_pair2's form)        */
   int32_t a, b, c;    /* tensor slots (b unused for kind 1)                     */
   int32_t phase;      /* 0 invariant forward (once), 1 variant forward, 2 variant
                          backward (per slice), 3 invariant backward (once, last) */
   int32_t zero_fill;  /* 1: zero tensor c (nbytes) before the launch           */
-  int32_t is_root;    /* 1: writes the output (accumulated over slices)         */
+  int32_t is_root;    /* 1: writes the output (accumulated over slices); 2: writes
+                         the tangent of the output (forward-mode plans)         */
   const int64_t* desc;
 } ctgb_node;
 
@@ -241,6 +257,21 @@ int ctgb_plan_execute(ctgb_plan* plan, const void* const* inputs, void* out,
                       void* const* grads, void* workspace,
                       size_t workspace_bytes, int64_t slice_begin,
                       int64_t slice_step, int64_t slice_count, void* stream);
+
+/* Forward mode: a plan with tangent slots (kinds 7, 8) forms, for the slices
+ * slice_begin, slice_begin + slice_step, ... (slice_count of them), the tangent
+ * of the sum of the slices for the input tangents `tangents` (a host array of
+ * n_inputs device pointers laid out as the inputs, null for inputs the plan does
+ * not differentiate) and accumulates it into `tangent_out` (device, out_elements
+ * of the accumulator dtype, zeroed by the caller).  `out` receives the primal
+ * result as ctgb_plan_execute does; it may be null, and the primal root is then
+ * not run.  The workspace rules are ctgb_plan_execute's.  Asynchronous. */
+int ctgb_plan_execute_jvp(ctgb_plan* plan, const void* const* inputs,
+                          const void* const* tangents, void* out,
+                          void* tangent_out, void* workspace,
+                          size_t workspace_bytes, int64_t slice_begin,
+                          int64_t slice_step, int64_t slice_count,
+                          void* stream);
 
 /* Same job for a forward plan with HOST buffers: copies the inputs
  * host->device, runs the slices, copies the accumulated output (out_elements of the
