@@ -45,6 +45,8 @@ EXPORTS = (
     "ctgb_absorb_root",
     "ctgb_contract_pair2",
     "ctgb_plan_execute_jvp",
+    "ctgb_plan_execute_jvp_stripped",
+    "ctgb_plan_set_tangent_scale_slots",
 )
 TC05_LAUNCH_FIELDS = ("b_stat", "nb", "sa", "grid", "smem", "tm_rank", "bulk", "chunk_steps", "chunks")
 DMMASTREAM_LAUNCH_FIELDS = ("nj", "rows", "grid")
@@ -134,6 +136,12 @@ def load():
         C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p,
         C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
     ]
+    lib.ctgb_plan_execute_jvp_stripped.argtypes = [
+        C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p,
+        C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
+    ]
+    lib.ctgb_plan_set_tangent_scale_slots.argtypes = [
+        C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]
     lib.ctgb_plan_create.argtypes = [C.POINTER(CtgbPlanDesc), C.POINTER(C.c_void_p)]
     lib.ctgb_plan_set_chunk_desc.argtypes = [C.c_void_p, C.c_void_p]
     lib.ctgb_plan_set_scale_slots.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]

@@ -199,7 +199,8 @@ class _Executor:
 
     ``stripped_grad=True`` (with ``strip_exponent``) differentiates the mantissa ``m`` of a result
     ``(m, e)`` with the exponent held constant, ``dm/dx = 10^-e damp/dx``: exact for every loss that
-    depends on the result only through ``m 10^e``.  ``vjp`` then takes the forward's ``exponent``.
+    depends on the result only through ``m 10^e``.  ``vjp`` then takes the forward's ``exponent``, and
+    ``jvp`` returns ``((m, e), dm)`` or, given the forward's ``exponent``, ``dm`` alone.
 
     ``plan_opts`` go to the forward and reverse-mode plans (``ExecPlan`` / ``VjpPlan`` keywords).
 
@@ -371,11 +372,13 @@ class _Executor:
 
     def jvp_plan(self, wrt=None, _two_term=True):
         """The (cached) ``JvpPlan`` of the executed program for the inputs ``wrt`` (default all; positions
-        among the variables).  ``strip_exponent`` executors raise ``NotImplementedError``."""
+        among the variables).  ``strip_exponent`` executors without ``stripped_grad`` raise
+        ``NotImplementedError``."""
         from .jvp import JvpPlan
 
-        if self.strip_exponent:
-            raise NotImplementedError("forward-mode derivatives of strip_exponent results are not supported")
+        if self.strip_exponent and not self.stripped_grad:
+            raise NotImplementedError("forward-mode derivatives of strip_exponent results are only defined with "
+                                      "stripped_grad=True (the exponent held constant)")
         wrt = tuple(range(len(self._shapes))) if wrt is None else tuple(sorted({int(i) for i in wrt}))
         if any(i < 0 or i >= len(self._shapes) for i in wrt):
             raise ValueError(f"wrt {list(wrt)} names inputs outside the {len(self._shapes)} variables")
@@ -385,35 +388,43 @@ class _Executor:
             torch = _torch()
             with torch.cuda.device(self.device):
                 plan = JvpPlan(*self._program, self._sliced, dtype=self.dtype, wrt=wrt, precision=self.precision,
-                               accumulate=self.accumulate, absorb_root=self.plan.absorb_root, _two_term=_two_term,
-                               **self._plan_opts).create()
+                               accumulate=self.accumulate, absorb_root=self.plan.absorb_root,
+                               strip_exponent=self.strip_exponent, stripped_grad=self.stripped_grad,
+                               _two_term=_two_term, **self._plan_opts).create()
             self._jvp_plans[key] = plan
         return plan
 
-    def jvp(self, tensors, tangents, begin=0, step=1, count=None, wrt=None, primal=True, _two_term=True):
+    def jvp(self, tensors, tangents, begin=0, step=1, count=None, wrt=None, primal=True, exponent=None,
+            _two_term=True):
         """Forward mode over slices ``begin, begin+step, ...`` (``count`` of them): the tangent of their
         sum for the input tangents ``tangents``, one tensor per input in ``wrt`` (default: all), each of
         its input's shape.  Returns ``(out, tangent_out)``, or ``tangent_out`` alone with
         ``primal=False``; both have the output's shape and the accumulator dtype.  Asynchronous on the
         current stream.  Tangents are additive over slices, so one call per rank over
         ``rank_slices(...)`` followed by an all-reduce gives the JVP of the whole tree.  Folded
-        constants carry no tangent.  ``strip_exponent`` executors raise ``NotImplementedError``."""
+        constants carry no tangent.
+
+        With ``strip_exponent`` and ``stripped_grad`` it returns ``((m, e), dm)``: ``(m, e)`` as
+        ``contract_device`` returns it and ``dm = 10^-e d(amp)``, the tangent of the mantissa with the
+        exponent held constant.  ``primal=False`` needs ``exponent`` (a float or a one-element tensor),
+        the ``e`` of the forward call over the same slices, and returns ``dm`` relative to it: the plan
+        runs as with the primal and the tangent is rescaled by ``10^(e_run - exponent)``.  A zero result
+        gives a zero ``dm``.  ``exponent`` belongs to that call only: given with ``primal=True``, or to an
+        executor without ``strip_exponent``, it raises ``ValueError``.  ``strip_exponent`` executors
+        without ``stripped_grad`` raise ``NotImplementedError``."""
         torch = _torch()
+        if exponent is not None and (primal or not self.strip_exponent):
+            raise ValueError("exponent= is the forward's e for a stripped tangent without the primal "
+                             "(strip_exponent executors, primal=False)")
         self._check_inputs(tensors)
         begin, step, count = self._check_slice_range(begin, step, count)
         plan = self.jvp_plan(wrt, _two_term)
-        if len(tangents) != len(plan.wrt):
-            raise ValueError(f"expected {len(plan.wrt)} tangents (one per input in wrt), got {len(tangents)}")
-        tdt, odt = getattr(torch, self.dtype), getattr(torch, self.out_dtype)
+        if plan.strip_exponent:
+            return self._jvp_stripped(plan, tensors, tangents, begin, step, count, primal, exponent)
+        odt = getattr(torch, self.out_dtype)
         with torch.cuda.device(self.device):
             ptrs, _keep = self._input_ptrs(tensors)
-            tans, tptrs = [], [None] * len(ptrs)
-            for i, t in zip(plan.wrt, tangents):
-                if tuple(t.shape) != tuple(self._shapes[i]):
-                    raise ValueError(f"tangent of input {i} has shape {tuple(t.shape)}, expected {self._shapes[i]}")
-                t = t.to(device=self.device, dtype=tdt).contiguous()
-                tans.append(t)
-                tptrs[i] = t.data_ptr()
+            tans, tptrs = self._jvp_tangents(plan, tangents, len(tensors))
             out = torch.zeros(plan.out_shape, dtype=odt, device=self.device) if primal else None
             tout = torch.zeros(plan.out_shape, dtype=odt, device=self.device)
             if not plan.tangent_nodes:  # nothing to differentiate: the tangent is zero
@@ -427,6 +438,53 @@ class _Executor:
             plan.execute(ptrs, tptrs, out.data_ptr() if primal else None, tout.data_ptr(), ws.data_ptr(), ws.numel(),
                          begin, step, count, _stream_ptr())
         return (out, tout) if primal else tout
+
+    def _jvp_stripped(self, plan, tensors, tangents, begin, step, count, primal, exponent):
+        torch = _torch()
+        if not primal and exponent is None:
+            raise ValueError("a stripped tangent without the primal needs the exponent of the forward call "
+                             "(exponent=)")
+        odt = getattr(torch, self.out_dtype)
+        with torch.cuda.device(self.device):
+            ptrs, _keep = self._input_ptrs(tensors)
+            tans, tptrs = self._jvp_tangents(plan, tangents, len(tensors))
+            out = torch.zeros(plan.out_shape, dtype=odt, device=self.device)
+            tout = torch.zeros(plan.out_shape, dtype=odt, device=self.device)
+            if not plan.tangent_nodes:  # nothing to differentiate: the tangent is zero
+                m, e = self.contract_device(tensors, begin, step, count, out=out)
+                return ((m, e), tout) if primal else tout
+            e = torch.full((1,), -math.inf, dtype=torch.float64, device=self.device)
+            if self._jvp_ws is None or self._jvp_ws.numel() < plan.total_bytes:
+                self._jvp_ws = None
+                self._jvp_ws = torch.empty(max(plan.total_bytes, 1), dtype=torch.uint8, device=self.device)
+            ws = self._jvp_ws
+            plan.execute(ptrs, tptrs, out.data_ptr(), tout.data_ptr(), ws.data_ptr(), ws.numel(), begin, step,
+                         count, _stream_ptr(), exp_ptr=e.data_ptr())
+            if self._exp_shift:
+                e.add_(self._exp_shift)  # (the folds' exponents scale m and dm alike)
+            if primal:
+                return (out, e), tout
+            # dm relative to the caller's exponent: 10^(e - exponent), 1 where both are -inf
+            want = torch.as_tensor(exponent, dtype=torch.float64).to(self.device).reshape(1)
+            scale = torch.where(e == want, torch.ones_like(e), torch.pow(10.0, e - want))
+            tout.mul_(scale.reshape(()).to(tout.dtype))
+        return tout
+
+    def _jvp_tangents(self, plan, tangents, n_ptrs):
+        """The tangents of ``plan.wrt`` as contiguous device tensors, and one pointer per plan input
+        (``None`` outside ``wrt``)."""
+        torch = _torch()
+        if len(tangents) != len(plan.wrt):
+            raise ValueError(f"expected {len(plan.wrt)} tangents (one per input in wrt), got {len(tangents)}")
+        tdt = getattr(torch, self.dtype)
+        tans, tptrs = [], [None] * (n_ptrs + len(self._resident))
+        for i, t in zip(plan.wrt, tangents):
+            if tuple(t.shape) != tuple(self._shapes[i]):
+                raise ValueError(f"tangent of input {i} has shape {tuple(t.shape)}, expected {self._shapes[i]}")
+            t = t.to(device=self.device, dtype=tdt).contiguous()
+            tans.append(t)
+            tptrs[i] = t.data_ptr()
+        return tans, tptrs
 
     def _check_slice_range(self, begin, step, count):
         """Slice ids ``begin, begin+step, ...`` must all lie in ``[0, nslices)``: the device
@@ -692,12 +750,12 @@ def _run_device(ex, arrays, tensors, slices, check_zero=False, max_bytes=None, a
     ``(mantissa, float exponent)``."""
     torch = _torch()
     begin, step, count = slices
-    dual = _tangent_inputs(torch, arrays, ex.strip_exponent)
+    dual = _tangent_inputs(torch, arrays, ex.strip_exponent, ex.stripped_grad)
     if _records_grad(torch, arrays, ex.strip_exponent, ex.stripped_grad) or dual:
         jvp = None
         if dual:
-            def jvp(ts, tans):
-                return ex.jvp(ts, [tans[i] for i in dual], begin, step, count, wrt=dual, primal=False)
+            def jvp(ts, tans, e=None):
+                return ex.jvp(ts, [tans[i] for i in dual], begin, step, count, wrt=dual, primal=False, exponent=e)
         res = _differentiable(torch, lambda ts: ex.contract_device(ts, begin, step, count),
                               lambda ts, g, wrt, e=None: ex.vjp(ts, g, begin, step, count, wrt=wrt,
                                                                 max_bytes=max_bytes, exponent=e), tensors, jvp)
@@ -724,15 +782,16 @@ def _records_grad(torch, arrays, strip_exponent, stripped_grad=False):
     return True
 
 
-def _tangent_inputs(torch, arrays, strip_exponent):
+def _tangent_inputs(torch, arrays, strip_exponent, stripped_grad=False):
     """Positions of the arrays that carry a ``torch.autograd.forward_ad`` tangent (all must be torch
-    tensors).  ``strip_exponent`` results get no tangent: a warning says so and the list is empty."""
+    tensors).  ``strip_exponent`` results get no tangent (a warning says so and the list is empty)
+    unless ``stripped_grad`` asks for the mantissa's, with the exponent held constant."""
     if not arrays or not all(isinstance(a, torch.Tensor) for a in arrays):
         return []
     from torch.autograd import forward_ad
 
     dual = [i for i, a in enumerate(arrays) if forward_ad.unpack_dual(a).tangent is not None]
-    if dual and strip_exponent:
+    if dual and strip_exponent and not stripped_grad:
         warnings.warn("strip_exponent=True: no forward-mode tangent is recorded for the (mantissa, exponent) "
                       "result", UserWarning, stacklevel=4)
         return []
@@ -747,8 +806,8 @@ def _differentiable(torch, run, vjp, tensors, jvp=None):
     (a ``VjpPlan`` on the device; ``wrt`` from ``ctx.needs_input_grad``) and whose forward-mode rule
     is ``jvp(tensors, tangents)`` (a ``JvpPlan``; ``tangents`` has one entry per tensor, zeros where
     torch has none, and ``jvp`` reads those of the inputs it was made for).  A stripped ``run``
-    returns ``(m, e)``: ``e`` is not differentiable, and the backward is
-    ``vjp(tensors, grad_m, wrt, e)``; it has no forward-mode rule (``jvp`` is None)."""
+    returns ``(m, e)``: ``e`` is not differentiable, the backward is ``vjp(tensors, grad_m, wrt, e)``
+    and the forward-mode rule, if any, ``jvp(tensors, tangents, e)``, the tangent of ``m``."""
     global _GRAD_FN
     if _GRAD_FN is None:
         from torch.autograd.function import once_differentiable
@@ -762,6 +821,8 @@ def _differentiable(torch, run, vjp, tensors, jvp=None):
                 if ctx.stripped:
                     ctx.mark_non_differentiable(res[1])
                     ctx.save_for_backward(*tensors, res[1])
+                    if jvp is not None:
+                        ctx.save_for_forward(*tensors, res[1])  # (dm is relative to this e)
                 else:
                     ctx.save_for_backward(*tensors)
                     if jvp is not None:
@@ -783,7 +844,10 @@ def _differentiable(torch, run, vjp, tensors, jvp=None):
             def jvp(ctx, _run_t, _vjp_t, _jvp_t, *tangents):
                 if ctx.jvp_fn is None:
                     return (None, None) if ctx.stripped else None
-                return ctx.jvp_fn(list(ctx.saved_tensors), list(tangents))
+                saved = list(ctx.saved_tensors)
+                if ctx.stripped:
+                    return ctx.jvp_fn(saved[:-1], list(tangents), saved[-1]), None
+                return ctx.jvp_fn(saved, list(tangents))
 
         _GRAD_FN = _Contract
     return _GRAD_FN.apply(run, vjp, jvp, *tensors)

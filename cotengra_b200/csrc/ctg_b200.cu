@@ -666,7 +666,8 @@ int launch_gett(const int64_t* h, const int64_t* d, const void* A, const void* B
 }
 
 // The two-term node C (+)= A.B + A2.B2 (A2 laid out as A, B2 as B) in one launch: the row-stream and
-// DMMA stream kernels only, unstripped and with C of the plan dtype
+// DMMA stream kernels only, with C of the plan dtype.  Scale words (W_SCALE_A / W_SCALE_B, both) make
+// it C (+)= (A.B + A2.B2) / (fA fB), B and B2 scaled as they are staged; it never measures a factor
 template <typename T>
 int launch_gett2_typed(const int64_t* h, const int64_t* d, const void* A, const void* B, const void* A2,
                        const void* B2, void* C, cudaStream_t st) {
@@ -681,7 +682,9 @@ int launch_gett2(const int64_t* h, const int64_t* d, const void* A, const void* 
                  void* C, cudaStream_t st) {
   if (h[W_MAGIC] != DESC_MAGIC) return fail(CTGB_E_VALUE, "bad pair descriptor magic");
   if (!A2 || !B2) return fail(CTGB_E_VALUE, "the two-term form needs both A2 and B2");
-  if (desc_stripped(h)) return fail(CTGB_E_VALUE, "the two-term form takes unstripped descriptors");
+  if (h[W_FACTOR_C] != 0) return fail(CTGB_E_VALUE, "the two-term form measures no factor of C (W_FACTOR_C)");
+  if ((h[W_SCALE_A] == 0) != (h[W_SCALE_B] == 0))
+    return fail(CTGB_E_VALUE, "the two-term form takes both scale words or neither");
   if (h[W_FLAGS] & FLAG_WIDE_C) return fail(CTGB_E_VALUE, "the two-term form has no wide C");
   switch ((int)h[W_DTYPE]) {
     case CTGB_F32: return launch_gett2_typed<float>(h, d, A, B, A2, B2, C, st);
@@ -765,31 +768,63 @@ int absmax_into(int dtype, const void* p, long long n, unsigned long long* slot,
 
 int wide_dtype(int dtype) { return dtype == CTGB_F32 ? CTGB_F64 : dtype == CTGB_C64 ? CTGB_C128 : dtype; }
 
-// (O: the type of the output accumulator, T or WideOf<T>)
+// The root's tangent of a stripped forward-mode plan rides along (StripTangent: the tangent output,
+// its chunk, the dense raw tangent root, the tangent's running exponent Et and e'_s, the slice exponent
+// without the root's factor); the same three launches fold both.  (O: the type of the output
+// accumulator, T or WideOf<T>)
+struct StripTangent {
+  void* tout = nullptr;
+  void* tchunk = nullptr;
+  const void* tm = nullptr;
+  double* Et = nullptr;
+  const double* es_t = nullptr;
+};
 template <typename T, typename O>
 int accum_stripped_typed(const int64_t* dchunk, const int64_t* hchunk, void* out, void* chunk, long long out_elems,
-                         const void* m, double* E, const double* es, const double* froot, cudaStream_t st) {
-  rescale_out_kernel<T, O><<<flat_grid(out_elems), 256, 0, st>>>((O*)out, out_elems, E, es);
-  add_chunk_kernel<T, O><<<flat_grid(hchunk[S_OUT_ELEMS]), 256, 0, st>>>(dchunk, (O*)chunk, (const T*)m, E, es, froot);
-  commit_exponent_kernel<<<1, 1, 0, st>>>(E, es);
+                         const void* m, double* E, const double* es, const double* froot, const StripTangent& tg,
+                         cudaStream_t st) {
+  rescale_out_kernel<T, O><<<flat_grid(out_elems), 256, 0, st>>>((O*)out, out_elems, E, es, (O*)tg.tout, tg.Et,
+                                                                  tg.es_t);
+  add_chunk_kernel<T, O><<<flat_grid(hchunk[S_OUT_ELEMS]), 256, 0, st>>>(dchunk, (O*)chunk, (const T*)m, E, es, froot,
+                                                                         (O*)tg.tchunk, (const T*)tg.tm, tg.Et,
+                                                                         tg.es_t);
+  commit_exponent_kernel<<<1, 1, 0, st>>>(E, es, tg.Et, tg.es_t);
   g_launches.fetch_add(3, std::memory_order_relaxed);
   CUDA_TRY(cudaGetLastError());
   return CTGB_OK;
 }
 int accum_stripped(int dtype, bool wide, const int64_t* dchunk, const int64_t* hchunk, void* out, void* chunk,
                    long long out_elems, const void* m, double* E, const double* es, const double* froot,
-                   cudaStream_t st) {
+                   const StripTangent& tg, cudaStream_t st) {
   switch (dtype) {
     case CTGB_F32:
-      return wide ? accum_stripped_typed<float, double>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st)
-                  : accum_stripped_typed<float, float>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
-    case CTGB_F64: return accum_stripped_typed<double, double>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
+      return wide ? accum_stripped_typed<float, double>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, tg, st)
+                  : accum_stripped_typed<float, float>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, tg, st);
+    case CTGB_F64:
+      return accum_stripped_typed<double, double>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, tg, st);
     case CTGB_C64:
-      return wide ? accum_stripped_typed<float2, double2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st)
-                  : accum_stripped_typed<float2, float2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
-    case CTGB_C128: return accum_stripped_typed<double2, double2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, st);
+      return wide ? accum_stripped_typed<float2, double2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, tg, st)
+                  : accum_stripped_typed<float2, float2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, tg, st);
+    case CTGB_C128:
+      return accum_stripped_typed<double2, double2>(dchunk, hchunk, out, chunk, out_elems, m, E, es, froot, tg, st);
   }
   return fail(CTGB_E_VALUE, "bad dtype");
+}
+
+// stripped forward mode, once per call: the tangent output from its own running exponent to the
+// mantissa's (tangent_to_exponent_kernel); `dtype` is the accumulator's
+int tangent_to_exponent(int dtype, void* tout, long long n, const double* Et, const double* E, cudaStream_t st) {
+  const unsigned grid = flat_grid(n);
+  switch (dtype) {
+    case CTGB_F32: tangent_to_exponent_kernel<float><<<grid, 256, 0, st>>>((float*)tout, n, Et, E); break;
+    case CTGB_F64: tangent_to_exponent_kernel<double><<<grid, 256, 0, st>>>((double*)tout, n, Et, E); break;
+    case CTGB_C64: tangent_to_exponent_kernel<float2><<<grid, 256, 0, st>>>((float2*)tout, n, Et, E); break;
+    case CTGB_C128: tangent_to_exponent_kernel<double2><<<grid, 256, 0, st>>>((double2*)tout, n, Et, E); break;
+    default: return fail(CTGB_E_VALUE, "bad dtype");
+  }
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  CUDA_TRY(cudaGetLastError());
+  return CTGB_OK;
 }
 
 // the dense float32 / complex64 root result of one slice, added into its chunk of the double output
@@ -927,6 +962,8 @@ struct ctgb_plan {
     int prescale_b = 0;     // strip_exponent: the small operand is copied, scaled by 1/(fA fB), first
     int prescale_a = 0;     // stripped reverse mode: a single-operand node reads a copy of A scaled by 1/fA
     int fa = -1, fb = -1;   // strip_exponent: the factor slots fA, fB it divides by (-1: 1.0)
+    int tangent = 0;        // stripped forward mode: a tangent record (divides by fA, fB, measures nothing)
+    int bscale_reuse = 0;   // ... whose small operand's scaled copy the node before it has just made
   };
   std::vector<Tensor> tensors;
   std::vector<Node> nodes;
@@ -978,8 +1015,12 @@ struct ctgb_plan {
 // nodes measure max|C| into their own slot as the forward does; a recomputed forward node (phase 2)
 // divides by the phase-1 factors of the values it recomputes and measures nothing, so that it forms
 // the same quotient as phase 1; a backward node divides by f_p and f_r (the seed at the root) and
-// measures nothing.
-static cudaError_t strip_setup(ctgb_plan* p, const int32_t* slot_a, const int32_t* slot_b) {
+// measures nothing.  A stripped forward-mode plan (ctgb_plan_set_tangent_scale_slots) marks its
+// tangent records (`tangent`): each divides by its primal node's two factor slots and measures nothing,
+// a two-term one through its scale words (the kernel scales B and B' as it stages them), and a
+// one-term one whose small operand the node before it has just copied, scaled alike, reads that copy.
+static cudaError_t strip_setup(ctgb_plan* p, const int32_t* slot_a, const int32_t* slot_b,
+                               const int32_t* tangent = nullptr) {
   const size_t nt = p->tensors.size();
   std::vector<double> ones(nt + 2, 1.0);
   cudaError_t e = cudaMalloc((void**)&p->d_factors, (nt + 2) * sizeof(double));
@@ -989,7 +1030,14 @@ static cudaError_t strip_setup(ctgb_plan* p, const int32_t* slot_a, const int32_
     auto& n = p->nodes[i];
     n.fa = slot_a ? slot_a[i] : n.a;
     n.fb = slot_b ? slot_b[i] : n.b;
-    const bool measures = n.phase <= 1;
+    n.tangent = tangent != nullptr && tangent[i] != 0;
+    const bool measures = n.phase <= 1 && !n.tangent;
+    if (n.kind == 2) {
+      int64_t* w = p->descs.data() + n.desc_off;
+      w[W_SCALE_A] = (int64_t)(uintptr_t)(p->d_factors + n.fa);
+      w[W_SCALE_B] = (int64_t)(uintptr_t)(p->d_factors + n.fb);
+      continue;
+    }
     if (n.kind != 0) {
       // (a reverse-mode plan whose root is a single-operand node: its adjoint reads the seeded cotangent)
       n.prescale_a = slot_a != nullptr && n.fa >= 0;
@@ -1002,6 +1050,11 @@ static cudaError_t strip_setup(ctgb_plan* p, const int32_t* slot_a, const int32_
     // output element; otherwise the epilogue multiplies by 1/(fA fB)
     const int64_t bbytes = p->tensors[n.b].nbytes;
     n.prescale_b = bbytes > 0 && bbytes <= (16ll << 20) && p->tensors[n.b].kind != 3;
+    if (n.prescale_b && n.tangent && i > 0) {
+      const auto& prev = p->nodes[i - 1];
+      n.bscale_reuse = prev.kind == 0 && prev.prescale_b && prev.b == n.b && prev.fa == n.fa && prev.fb == n.fb &&
+                       prev.phase == n.phase;
+    }
     if (n.prescale_b) {
       if ((size_t)bbytes > p->bscale_bytes) p->bscale_bytes = (size_t)bbytes;
     } else {
@@ -1240,13 +1293,15 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     }
     if (n.phase == 1 || n.phase == 2) per_slice += 1 + q.measure_after + (pd->strip_exponent && n.kind == 0 ? 1 : 0);
   }
-  p->scale_pending = pd->strip_exponent && p->backward;
   // kind 3 (the output) belongs to forward plans, kinds 4-6 (cotangent, gradients, H accumulators) to
   // reverse-mode ones: execute checks exactly the buffers the plan's kind needs
+  for (const auto& q : p->tensors) p->jvp |= q.kind >= 7;
+  // (stripped derivative plans get their factor slots from ctgb_plan_set_scale_slots or, forward
+  // mode, ctgb_plan_set_tangent_scale_slots)
+  p->scale_pending = pd->strip_exponent && (p->backward || p->jvp);
   p->grad_elems.assign(pd->n_inputs, 0);
   p->needs_tangent.assign(pd->n_inputs, 0);
-  for (const auto& q : p->tensors) p->jvp |= q.kind >= 7;
-  if (p->jvp && (p->backward || pd->strip_exponent)) return refuse("a forward-mode plan has phases 0 and 1, unstripped");
+  if (p->jvp && p->backward) return refuse("a forward-mode plan has phases 0 and 1");
   for (const auto& q : p->tensors) {
     const bool rev = q.kind >= 4 && q.kind <= 6, fwd = q.kind >= 7;
     if (q.kind < 0 || q.kind > 8 || (q.kind == 3 && p->backward) || (rev && !p->backward) || (fwd && !p->jvp))
@@ -1279,8 +1334,8 @@ int ctgb_plan_create(const ctgb_plan_desc* pd, ctgb_plan** out) {
     e = cudaMemcpy(p->d_descs, p->descs.data(), p->descs.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMalloc((void**)&p->d_scalars, 8 * sizeof(double));
   if (e == cudaSuccess) e = cudaMemset(p->d_scalars, 0, 8 * sizeof(double));
-  // (a stripped reverse-mode plan gets its factor slots from ctgb_plan_set_scale_slots)
-  if (e == cudaSuccess && p->strip_exponent && !p->backward) e = strip_setup(p, nullptr, nullptr);
+  // (stripped derivative plans get their factor slots from a setter)
+  if (e == cudaSuccess && p->strip_exponent && !p->scale_pending) e = strip_setup(p, nullptr, nullptr);
   if (e != cudaSuccess) {
     std::string msg = cudaGetErrorString(e);
     ctgb_plan_destroy(p);
@@ -1379,7 +1434,7 @@ int ctgb_plan_set_accumulator(ctgb_plan* p, int32_t dtype) {
 
 int ctgb_plan_set_scale_slots(ctgb_plan* p, const int32_t* slot_a, const int32_t* slot_b, int n) {
   if (!p || !slot_a || !slot_b) return fail(CTGB_E_VALUE, "null argument");
-  if (!p->scale_pending) return fail(CTGB_E_VALUE, "scale slots belong to stripped reverse-mode plans, once");
+  if (!p->scale_pending || p->jvp) return fail(CTGB_E_VALUE, "scale slots belong to stripped reverse-mode plans, once");
   if (n != (int)p->nodes.size()) return fail(CTGB_E_VALUE, "node count mismatch");
   const int seed = (int)p->tensors.size();
   for (int i = 0; i < n; ++i) {
@@ -1392,6 +1447,36 @@ int ctgb_plan_set_scale_slots(ctgb_plan* p, const int32_t* slot_a, const int32_t
   int64_t per_slice = 3;  // reset slots, sum of logs, seed
   for (const auto& q : p->nodes)
     if (q.phase == 1 || q.phase == 2) per_slice += 1 + q.measure_after + q.prescale_b + q.prescale_a;
+  p->launches_per_slice = per_slice;
+  return CTGB_OK;
+}
+
+int ctgb_plan_set_tangent_scale_slots(ctgb_plan* p, const int32_t* slot_a, const int32_t* slot_b,
+                                      const int32_t* tangent, int n) {
+  if (!p || !slot_a || !slot_b || !tangent) return fail(CTGB_E_VALUE, "null argument");
+  if (!p->scale_pending || !p->jvp)
+    return fail(CTGB_E_VALUE, "tangent scale slots belong to stripped forward-mode plans, once");
+  if (n != (int)p->nodes.size()) return fail(CTGB_E_VALUE, "node count mismatch");
+  const int nt = (int)p->tensors.size();
+  for (int i = 0; i < n; ++i) {
+    const auto& q = p->nodes[i];
+    if (tangent[i] != 0 && tangent[i] != 1) return fail(CTGB_E_VALUE, "tangent marks are 0 or 1");
+    if (q.kind == 1) {
+      if (slot_a[i] != -1 || slot_b[i] != -1) return fail(CTGB_E_VALUE, "a single-operand node divides by nothing");
+      continue;
+    }
+    if (slot_a[i] < 0 || slot_a[i] >= nt || slot_b[i] < 0 || slot_b[i] >= nt)
+      return fail(CTGB_E_VALUE, "scale slot out of range");
+    // (a primal record is the forward plan's node: it divides by its own operands' factors)
+    if (!tangent[i] && (q.kind != 0 || slot_a[i] != q.a || slot_b[i] != q.b))
+      return fail(CTGB_E_VALUE, "a primal record divides by its own operands' factor slots");
+    if (tangent[i] && q.is_root == 1) return fail(CTGB_E_VALUE, "the primal root is not a tangent record");
+  }
+  CUDA_TRY(strip_setup(p, slot_a, slot_b, tangent));
+  p->scale_pending = false;
+  int64_t per_slice = 5;  // reset slots, sum of logs, rescale / add / commit
+  for (const auto& q : p->nodes)
+    if (q.phase == 1) per_slice += 1 + q.measure_after + (q.prescale_b && !q.bscale_reuse);
   p->launches_per_slice = per_slice;
   return CTGB_OK;
 }
@@ -1417,6 +1502,9 @@ static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* 
   // a stripped reverse-mode plan reads the exponent of the forward call it differentiates
   if (p->strip_exponent && p->backward && (!exponent_dev || p->scale_pending))
     return fail(CTGB_E_VALUE, "a stripped reverse-mode plan needs the forward's exponent and its scale slots");
+  // a stripped forward-mode plan always runs its primal root: its factor sets the slice exponent
+  if (p->strip_exponent && p->jvp && (p->scale_pending || !out || p->troot < 0))
+    return fail(CTGB_E_VALUE, "a stripped forward-mode plan needs its scale slots, the output and a tangent root");
   if ((p->backward || p->cot_offset >= 0) && !cotangent) return fail(CTGB_E_VALUE, "the plan needs a cotangent");
   for (int i = 0; i < p->n_inputs; ++i)
     if (p->grad_elems[i] > 0 && (!grads || !grads[i]))
@@ -1433,6 +1521,10 @@ static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* 
 
   double* d_slice_exp = p->d_scalars + 1;
   double* d_inv_exp = p->d_scalars + 2;
+  double* d_slice_exp_t = p->d_scalars + 3;  // stripped forward mode: e'_s, without the root's factor
+  double* d_tangent_exp = p->d_scalars + 4;  // ... and the tangent's running exponent Et
+  // (stripped forward mode: the slot of the root's factor, kept out of e'_s; -1 for a single-operand root)
+  const int root_slot = p->strip_exponent && p->jvp && p->nodes[p->root].kind == 0 ? p->nodes[p->root].c : -1;
 
   ctgb_slice_mem mem;
   mem.inputs = inputs;
@@ -1473,16 +1565,20 @@ static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* 
       // keeps its base offset into a copy)
       auto under = [&](const ctgb_plan::Tensor& t) -> char* {
         if (t.kind == 0) return (char*)inputs[t.input_index];
+        if (t.kind == 7) return (char*)tangents[t.input_index];
         if (t.kind == 4) return (char*)mem.cot;
         return (t.kind == 1 ? scratch : persistent) + t.offset;
       };
       if (n.prescale_b) {
-        // the small operand, scaled by 1/(fA fB) read from the factor slots on the device
+        // the small operand, scaled by 1/(fA fB) read from the factor slots on the device (a tangent
+        // record right after its primal node may find that copy made already)
         const ctgb_plan::Tensor& tb = p->tensors[n.b];
         char* base = under(tb);
-        if (int r = scale_copy(p->dtype, base, p->d_bscale, tb.nbytes / (int64_t)es, p->d_factors + n.fa,
-                               p->d_factors + n.fb, st))
-          return r;
+        if (!n.bscale_reuse) {
+          if (int r = scale_copy(p->dtype, base, p->d_bscale, tb.nbytes / (int64_t)es, p->d_factors + n.fa,
+                                 p->d_factors + n.fb, st))
+            return r;
+        }
         B = p->d_bscale + (B - base);
       }
       if (n.prescale_a) {
@@ -1513,6 +1609,11 @@ static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* 
     return CTGB_OK;
   };
 
+  // stripped forward mode: the tangent output holds the tangent relative to the entry exponent, so its
+  // running exponent starts there
+  const bool strip_jvp = p->strip_exponent && p->jvp;
+  if (strip_jvp)
+    CUDA_TRY(cudaMemcpyAsync(d_tangent_exp, exponent_dev, sizeof(double), cudaMemcpyDeviceToDevice, st));
   // slice-invariant subtrees: once per execute call, kept in the persistent arena
   if (p->strip_exponent && p->n_inv_slots > 0) {
     reset_slots_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists + p->n_var_slots, p->n_inv_slots);
@@ -1537,7 +1638,8 @@ static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* 
     }
     if ((rc = run_phase(1, out_off))) return rc;
     if (p->strip_exponent) {
-      sum_log_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists, p->n_var_slots, d_slice_exp, d_inv_exp);
+      sum_log_kernel<<<1, 256, 0, st>>>(p->d_factors, p->d_slot_lists, p->n_var_slots, d_slice_exp, d_inv_exp,
+                                        p->jvp ? d_slice_exp_t : nullptr, root_slot);
       g_launches.fetch_add(1, std::memory_order_relaxed);
     }
     if (p->strip_exponent && p->backward) {
@@ -1554,9 +1656,18 @@ static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* 
       char* m = resolve(root.c, 0);
       // (the stored root is the raw product: its own factor divides it here)
       const double* froot = root.kind == 0 ? p->d_factors + root.c : nullptr;
+      StripTangent tg;
+      if (p->jvp) {
+        // the raw tangent root, stored densely as the root is, follows into the tangent output
+        tg.tout = tangent_out;
+        tg.tchunk = (char*)tangent_out + out_off * (int64_t)mem.out_es;
+        tg.tm = resolve(p->nodes[p->troot].c, 0);
+        tg.Et = d_tangent_exp;
+        tg.es_t = d_slice_exp_t;
+      }
       rc = accum_stripped(p->dtype, wide, p->d_chunk_desc, p->chunk_desc.data(), out,
                           (char*)out + out_off * (int64_t)mem.out_es, p->out_elements, m, exponent_dev, d_slice_exp,
-                          froot, st);
+                          froot, tg, st);
       if (rc) return rc;
     }
     if (wide_fold && out) {
@@ -1571,6 +1682,8 @@ static int plan_run(ctgb_plan* p, const void* const* inputs, const void* const* 
       if (rc) return rc;
     }
   }
+  if (strip_jvp && (rc = tangent_to_exponent(p->acc_dtype, tangent_out, p->out_elements, d_tangent_exp, exponent_dev, st)))
+    return rc;
   // the invariant subtrees are differentiated once, from the accumulated H
   std::fill(digits.begin(), digits.end(), 0);
   if ((rc = run_phase(3, 0))) return rc;
@@ -1596,6 +1709,15 @@ int ctgb_plan_execute_jvp(ctgb_plan* p, const void* const* inputs, const void* c
   if (!p) return fail(CTGB_E_VALUE, "null plan");
   if (!p->jvp) return fail(CTGB_E_VALUE, "not a forward-mode plan");
   return plan_run(p, inputs, tangents, out, tangent_out, nullptr, nullptr, nullptr, workspace, workspace_bytes,
+                  slice_begin, slice_step, slice_count, stream);
+}
+
+int ctgb_plan_execute_jvp_stripped(ctgb_plan* p, const void* const* inputs, const void* const* tangents, void* out,
+                                   void* tangent_out, double* exponent_dev, void* workspace, size_t workspace_bytes,
+                                   int64_t slice_begin, int64_t slice_step, int64_t slice_count, void* stream) {
+  if (!p) return fail(CTGB_E_VALUE, "null plan");
+  if (!p->jvp || !p->strip_exponent) return fail(CTGB_E_VALUE, "not a stripped forward-mode plan");
+  return plan_run(p, inputs, tangents, out, tangent_out, exponent_dev, nullptr, nullptr, workspace, workspace_bytes,
                   slice_begin, slice_step, slice_count, stream);
 }
 

@@ -38,8 +38,9 @@ dmmastream_kernel(const int64_t* __restrict__ D, const double2* __restrict__ A, 
   __shared__ double2 s_B2[TWO ? DS_KB * DS_NMAX : 1];
   const int tid = threadIdx.x, lane = tid & 31;
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
-  const int n_m = s.load(D, B, K, N);
-  if constexpr (TWO) s.copy_b(B2, s_B2, K, N);
+  // (a stripped two-term node: both copies / (fA fB))
+  const int n_m = s.template load<TWO>(D, B, K, N);
+  if constexpr (TWO) s.template copy_b<true>(B2, s_B2, K, N, D);
   // (the flags after the tables: read before them, ptxas gives <8, 2, true> 248 registers, not 244)
   const StreamFlags f = stream_flags<double2>(D);
 

@@ -652,6 +652,17 @@ struct DmmaPolicy {
   }
 };
 
+// strip_exponent scaling of a staged or copied operand (scale_copy_kernel, the two-term stream kernels):
+// v * sa * sb with the intermediate kept in double (sa alone may leave the float range)
+__device__ __forceinline__ float scale2_of(float v, double sa, double sb) { return (float)((double)v * sa * sb); }
+__device__ __forceinline__ double scale2_of(double v, double sa, double sb) { return v * sa * sb; }
+__device__ __forceinline__ float2 scale2_of(float2 v, double sa, double sb) {
+  return make_float2((float)((double)v.x * sa * sb), (float)((double)v.y * sa * sb));
+}
+__device__ __forceinline__ double2 scale2_of(double2 v, double sa, double sb) {
+  return make_double2(v.x * sa * sb, v.y * sa * sb);
+}
+
 #include "tf32_policy.cuh"
 #include "stream_rows.cuh"
 #include "rowstream.cuh"
@@ -786,24 +797,49 @@ __device__ __forceinline__ O mulr_as(T v, double s) {
   else if constexpr (std::is_same<T, float>::value) return (double)v * s;
   else return make_double2((double)v.x * s, (double)v.y * s);
 }
+// Stripped forward-mode plans fold the root's tangent along (tout, its chunk tchunk, the dense raw
+// tangent root tm) against a running exponent of its own, Et: per slice Et' = max(Et, e'_s), tout is
+// rescaled by 10^(Et - Et') and the slice adds tm * 10^(e'_s - Et'), e'_s (es_t) being the slice
+// exponent without the root's factor.  e'_s is finite whenever the factors below the root are, so a
+// slice whose amplitude is exactly zero keeps its tangent whatever its place in the slice order; a
+// slice with a zero factor below its root adds nothing.  tangent_to_exponent_kernel then brings tout
+// to the mantissa's exponent once per call.  A NaN exponent makes the tangent NaN.
 template <typename T, typename O = T>
 __global__ void rescale_out_kernel(O* __restrict__ out, long long n, const double* __restrict__ E,
-                                   const double* __restrict__ es) {
+                                   const double* __restrict__ es, O* __restrict__ tout = nullptr,
+                                   const double* __restrict__ Et = nullptr, const double* __restrict__ es_t = nullptr) {
   const double e = exponent_max(*E, *es);
   const double so = (*E == e) ? 1.0 : pow(10.0, *E - e);
-  if (so == 1.0) return;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    out[i] = mulr_of(out[i], so);
+  if (tout == nullptr) {
+    if (so == 1.0) return;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+      out[i] = mulr_of(out[i], so);
+    return;
+  }
+  const double et = exponent_max(*Et, *es_t);
+  const double so_t = (*Et == et) ? 1.0 : pow(10.0, *Et - et);
+  if (so == 1.0 && so_t == 1.0) return;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (so != 1.0) out[i] = mulr_of(out[i], so);
+    if (so_t != 1.0) tout[i] = mulr_of(tout[i], so_t);
+  }
 }
 template <typename T, typename O = T>
 __global__ void add_chunk_kernel(const int64_t* __restrict__ D, O* __restrict__ out, const T* __restrict__ m,
                                  const double* __restrict__ E, const double* __restrict__ es,
-                                 const double* __restrict__ froot) {
+                                 const double* __restrict__ froot, O* __restrict__ tchunk = nullptr,
+                                 const T* __restrict__ tm = nullptr, const double* __restrict__ Et = nullptr,
+                                 const double* __restrict__ es_t = nullptr) {
   // D: single-operand descriptor mapping the dense slice result onto the chunk
   // froot: the root's own factor max|m| -- the stored root is not normalised yet (lazy scaling)
   const double e = exponent_max(*E, *es);
   double sn = (*es == e) ? 1.0 : pow(10.0, *es - e);
   if (froot != nullptr) sn = (*froot != 0.0) ? sn / *froot : 0.0;
+  double st = 0.0;
+  if (tchunk != nullptr) {
+    const double et = exponent_max(*Et, *es_t);
+    st = et == -CUDART_INF ? 0.0 : (*es_t == et) ? 1.0 : pow(10.0, *es_t - et);
+  }
   const int n_o = (int)D[S_NO];
   const long long n = D[S_OUT_ELEMS];
   for (long long o = blockIdx.x * (long long)blockDim.x + threadIdx.x; o < n; o += (long long)gridDim.x * blockDim.x) {
@@ -816,7 +852,20 @@ __global__ void add_chunk_kernel(const int64_t* __restrict__ D, O* __restrict__ 
       oo += dig * L[2];
     }
     out[oo] = add_of(out[oo], mulr_as<O>(m[xo], sn));
+    if (tchunk != nullptr) tchunk[oo] = add_of(tchunk[oo], mulr_as<O>(tm[xo], st));
   }
+}
+// once per call, after the slices: tout from its own exponent Et to the mantissa's E, tout * 10^(Et - E);
+// zero when E is -inf (a zero result has a zero tangent), NaN when either exponent is
+template <typename O>
+__global__ void tangent_to_exponent_kernel(O* __restrict__ tout, long long n, const double* __restrict__ Et,
+                                           const double* __restrict__ E) {
+  const double a = *Et, b = *E;
+  const double s = (a != a || b != b) ? __longlong_as_double(0x7ff8000000000000LL)
+                   : b == -CUDART_INF ? 0.0 : a == b ? 1.0 : pow(10.0, a - b);
+  if (s == 1.0) return;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    tout[i] = s == 0.0 ? O{} : mulr_of(tout[i], s);
 }
 // accumulate="double" plans whose root is not a dot-stream node: the root stores its slice result
 // densely in the plan dtype, and this folds it into its chunk of the double output (D as above) --
@@ -837,22 +886,15 @@ __global__ void add_chunk_wide_kernel(const int64_t* __restrict__ D, Wide* __res
     out[oo] = add_of(out[oo], mulr_as<Wide>(m[xo], 1.0));
   }
 }
-__global__ void commit_exponent_kernel(double* __restrict__ E, const double* __restrict__ es) {
+__global__ void commit_exponent_kernel(double* __restrict__ E, const double* __restrict__ es,
+                                       double* __restrict__ Et = nullptr, const double* __restrict__ es_t = nullptr) {
   *E = exponent_max(*E, *es);
+  if (Et != nullptr) *Et = exponent_max(*Et, *es_t);
 }
 // strip_exponent, small operand pre-scaled: dst = src / (fA fB) over the whole underlying buffer of
 // the node's small operand (a few KB on a contraction stem), so that the big kernel's epilogue
 // only has to track max|C| -- two multiplies per output element of a 16 GiB result are not free
 // on the fp64 pipe the DMMAs run on.
-// v * sa * sb with the intermediate kept in double (sa alone may leave the float range)
-__device__ __forceinline__ float scale2_of(float v, double sa, double sb) { return (float)((double)v * sa * sb); }
-__device__ __forceinline__ double scale2_of(double v, double sa, double sb) { return v * sa * sb; }
-__device__ __forceinline__ float2 scale2_of(float2 v, double sa, double sb) {
-  return make_float2((float)((double)v.x * sa * sb), (float)((double)v.y * sa * sb));
-}
-__device__ __forceinline__ double2 scale2_of(double2 v, double sa, double sb) {
-  return make_double2(v.x * sa * sb, v.y * sa * sb);
-}
 template <typename T>
 __global__ void scale_copy_kernel(const T* __restrict__ src, T* __restrict__ dst, long long n,
                                   const double* __restrict__ fa, const double* __restrict__ fb) {
@@ -866,23 +908,38 @@ __global__ void scale_copy_kernel(const T* __restrict__ src, T* __restrict__ dst
 __global__ void reset_slots_kernel(double* __restrict__ f, const int* __restrict__ list, int n) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) f[list[i]] = 0.0;
 }
-// exponent = base + sum_i log10(factor[list[i]])   (-inf as soon as one factor is zero; one block)
+// exponent = base + sum_i log10(factor[list[i]])   (-inf as soon as one factor is zero; one block).
+// without (stripped forward mode): the same sum without the entries naming slot `skip` (the root's
+// factor), summed apart so that a zero root factor leaves it finite
 __global__ void sum_log_kernel(const double* __restrict__ f, const int* __restrict__ list, int n,
-                               double* __restrict__ exponent, const double* __restrict__ base) {
-  __shared__ double part[8];
-  double acc = 0.0;
+                               double* __restrict__ exponent, const double* __restrict__ base,
+                               double* __restrict__ without = nullptr, int skip = -1) {
+  __shared__ double part[8], part_w[8];
+  double acc = 0.0, acc_w = 0.0;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const double v = f[list[i]];
-    acc += (v != 0.0) ? log10(v) : -CUDART_INF;
+    const double l = (v != 0.0) ? log10(v) : -CUDART_INF;
+    acc += l;
+    if (list[i] != skip) acc_w += l;
   }
 #pragma unroll
-  for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+  for (int d = 16; d > 0; d >>= 1) {
+    acc += __shfl_xor_sync(0xffffffffu, acc, d);
+    acc_w += __shfl_xor_sync(0xffffffffu, acc_w, d);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    part[threadIdx.x >> 5] = acc;
+    part_w[threadIdx.x >> 5] = acc_w;
+  }
   __syncthreads();
   if (threadIdx.x == 0) {
-    double t = base ? *base : 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += part[w];
+    double t = base ? *base : 0.0, tw = t;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) {
+      t += part[w];
+      tw += part_w[w];
+    }
     *exponent = t;
+    if (without != nullptr) *without = tw;
   }
 }
 // stripped reverse mode, once per slice after its forward phase: the divisor 10^(e - e'_s) that

@@ -13,7 +13,8 @@
 // STRIP: fused strip_exponent (a separate instantiation: its few live registers would spill
 // inside the row loop of the register-bound variants otherwise)
 // TWO: C (+)= A.B + A2.B2 (stream_rows.cuh), B2 from shared memory, two blocks per SM (the A2 row
-// doubles the operand registers); not with BREG or STRIP
+// doubles the operand registers); not with BREG or STRIP.  A stripped two-term node scales the staged
+// B and B2 instead (copy_b<true>: a runtime branch in the prologue)
 template <typename T, int NMAX, int KMAX, bool BREG, bool STRIP = false, bool TWO = false>
 __global__ void __launch_bounds__(256, (BREG || TWO) ? 2 : 3)
 rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B, T* __restrict__ C,
@@ -24,8 +25,8 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
   const int tid = threadIdx.x;
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
   const StreamFlags f = stream_flags<T>(D);
-  const int n_m = s.load(D, B, K, N);
-  if constexpr (TWO) s.copy_b(B2, s_B2, K, N);
+  const int n_m = s.template load<TWO>(D, B, K, N);
+  if constexpr (TWO) s.template copy_b<true>(B2, s_B2, K, N, D);
   [[maybe_unused]] T breg[BREG ? KMAX : 1][BREG ? NMAX : 1];
   if constexpr (BREG) {
 #pragma unroll
@@ -122,7 +123,8 @@ rowstream_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T
 // memory, the 8 accumulators of a row stay in registers across the chunks.
 constexpr int RSK_KMAX = 64, RSK_NMAX = 8;
 
-// TWO: C (+)= A.B + A2.B2, the chunks of A2 after those of A into the same accumulators
+// TWO: C (+)= A.B + A2.B2, the chunks of A2 after those of A into the same accumulators (stripped:
+// the staged B and B2 scaled, as above)
 template <typename T, bool STRIP = false, bool TWO = false>
 __global__ void __launch_bounds__(256, 3)
 rowstream_longk_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, const T* __restrict__ B,
@@ -133,8 +135,8 @@ rowstream_longk_kernel(const int64_t* __restrict__ D, const T* __restrict__ A, c
   const int tid = threadIdx.x;
   const int K = (int)D[W_KTA], N = (int)D[W_NTA];
   const StreamFlags f = stream_flags<T>(D);
-  const int n_m = s.load(D, B, K, N);
-  if constexpr (TWO) s.copy_b(B2, s_B2, K, N);
+  const int n_m = s.template load<TWO>(D, B, K, N);
+  if constexpr (TWO) s.template copy_b<true>(B2, s_B2, K, N, D);
   long long inoff[8];  // offsets inside a chunk of 8 k
 #pragma unroll
   for (int kk = 0; kk < 8; ++kk) inoff[kk] = s.akoff[kk];

@@ -4,7 +4,8 @@
 // row store.  Each kernel keeps its own main loop: their register budgets differ (80 to 255
 // registers for two or three blocks per SM) and a shared loop would move the allocation.
 // The two-term instantiations (TWO) form C (+)= A.B + A'.B' for A' laid out as A and B' as B: both
-// products go into the same accumulators before the one row store, so C is written once.
+// products go into the same accumulators before the one row store, so C is written once.  With scale
+// words (and no factor slot of C) they scale both copies of B as they stage them (copy_b<true>).
 // (included inside namespace ctgb)
 #pragma once
 
@@ -48,7 +49,8 @@ struct StreamTables {
   T* B;
 
   // Every thread of the CTA (at least 128) calls this once; K <= KB and N <= NMAX.  Returns the
-  // number of m dims.
+  // number of m dims.  (SCALED: copy_b's)
+  template <bool SCALED = false>
   __device__ __forceinline__ int load(const int64_t* __restrict__ D, const T* __restrict__ Bg, int K, int N) const {
     const int tid = threadIdx.x;
     const int n_tm = (int)D[W_NTM], n_gm = (int)D[W_NGM], n_tk = (int)D[W_NTK], n_tn = (int)D[W_NTN];
@@ -99,16 +101,35 @@ struct StreamTables {
       cnoff[c] = o;
     }
     __syncthreads();
-    copy_b(Bg, B, K, N);
+    copy_b<SCALED>(Bg, B, K, N, D);
     return n_m;
   }
 
   // A zero-padded [KB][NMAX] copy of an operand laid out as B (offsets bkoff, bnoff) into dst; the
-  // two-term kernels make a second one of B'
-  __device__ __forceinline__ void copy_b(const T* __restrict__ Bg, T* dst, int K, int N) const {
+  // two-term kernels make a second one of B'.  SCALED (the two-term kernels): a descriptor with scale
+  // words (W_SCALE_A / W_SCALE_B, a stripped two-term node: C (+)= (A.B + A'.B') / (fA fB)) scales the
+  // copy by 1/(fA fB) as it is staged, a zero factor by 0 as strip_begin; a runtime branch
+  template <bool SCALED = false>
+  __device__ __forceinline__ void copy_b(const T* __restrict__ Bg, T* dst, int K, int N,
+                                         [[maybe_unused]] const int64_t* __restrict__ D = nullptr) const {
+    [[maybe_unused]] double sa = 1.0, sb = 1.0;
+    [[maybe_unused]] bool scaled = false;
+    if constexpr (SCALED) {
+      const double* pa = reinterpret_cast<const double*>(D[W_SCALE_A]);
+      scaled = pa != nullptr;  // (uniform over the CTA)
+      if (scaled) {
+        const double fa = *pa, fb = *reinterpret_cast<const double*>(D[W_SCALE_B]);
+        sa = fa != 0.0 ? 1.0 / fa : 0.0;
+        sb = fb != 0.0 ? 1.0 / fb : 0.0;
+      }
+    }
     for (int i = threadIdx.x; i < KB * NMAX; i += blockDim.x) {
       const int kk = i / NMAX, c = i % NMAX;
-      dst[i] = (kk < K && c < N) ? Bg[bkoff[kk] + bnoff[c]] : zero_of<T>();
+      T v = (kk < K && c < N) ? Bg[bkoff[kk] + bnoff[c]] : zero_of<T>();
+      if constexpr (SCALED) {
+        if (scaled) v = scale2_of(v, sa, sb);
+      }
+      dst[i] = v;
     }
     __syncthreads();
   }

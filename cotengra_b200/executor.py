@@ -206,7 +206,18 @@ class _DevicePlan:
     cotangent_offset = -1
     acc_dtype = None     # forward plans that sum their slices in double: ctgb_plan_set_accumulator
     _chunk_words = None  # forward plans whose root stores its slice densely: ctgb_plan_set_chunk_desc
-    scale_slots = None   # stripped reverse-mode plans: ctgb_plan_set_scale_slots, ([slot_a], [slot_b])
+    scale_slots = None   # stripped derivative plans: ([slot_a], [slot_b]), from each node's "scale" (_scale_slots)
+    tangent_marks = None  # stripped forward-mode plans: 1 per tangent record (ctgb_plan_set_tangent_scale_slots)
+
+    def _scale_slots(self):
+        """``scale_slots`` of a stripped derivative plan: the factor slots every node of ``self.nodes``
+        divides by, from its ``"scale"`` entry (the operand tensors; ``None`` for the root's seed, slot
+        ``n_tensors``); -1 where a node has none."""
+        slot = {id(t): i for i, t in enumerate(self.tensors)}
+        seed = len(self.tensors)
+        scale = [nd.get("scale", ()) for nd in self.nodes]
+        self.scale_slots = tuple([-1 if len(s) <= k else seed if s[k] is None else slot[id(s[k])] for s in scale]
+                                 for k in (0, 1))
 
     def _marshal(self):
         keep = self._keep = []
@@ -279,7 +290,11 @@ class _DevicePlan:
         if self.scale_slots is not None:
             n = len(self.nodes)
             sa, sb = ((C.c_int32 * max(n, 1))(*s) for s in self.scale_slots)
-            _lib.check(lib.ctgb_plan_set_scale_slots(h, sa, sb, n))
+            if self.tangent_marks is None:
+                _lib.check(lib.ctgb_plan_set_scale_slots(h, sa, sb, n))
+            else:
+                marks = (C.c_int32 * max(n, 1))(*self.tangent_marks)
+                _lib.check(lib.ctgb_plan_set_tangent_scale_slots(h, sa, sb, marks, n))
         return self
 
     def destroy(self):

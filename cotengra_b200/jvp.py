@@ -25,6 +25,27 @@ tangent uses the root's descriptor and accumulates over the slices into the tang
 8, the output's slice view), so ``accumulate="double"``, sliced output indices and the chunk
 descriptor of a dense root apply to it unchanged.  Both arenas are laid out by liveness
 (``executor.layout``).
+
+With ``strip_exponent`` and ``stripped_grad`` the plan forms the tangent of the mantissa ``m`` of a
+stripped result ``(m, e)`` with the exponent held constant, ``dm = 10^-e d(amp)``.  The primal
+records are the stripped forward plan's, descriptor for descriptor: a pairwise value is stored raw,
+``S_p = (S_l/f_l)(S_r/f_r)``, and records ``f_p = max|S_p|``.  Each tangent is defined with the same
+factors,
+
+    T_p = (T_l S_r + S_l T_r) / (f_l f_r)
+
+one scale shared by both terms, the one its primal node uses; a tangent record divides by its
+primal node's two factor slots and records no factor of its own (``tangent_marks``,
+``ctgb_plan_set_tangent_scale_slots``).  A one-term record takes the forward's stripped launch path
+(a pre-scaled small operand, reusing the copy its primal node has just made, or epilogue scaling); a
+two-term record scales B and B' as the kernel stages them.  The primal root always runs, since its
+factor sets the slice exponent ``e_s``.  The raw tangent root ``T_s`` is folded against a running
+exponent of its own, ``Et' = max(Et, e'_s)``: ``tout <- tout 10^(Et - Et') + T_s 10^(e'_s - Et')``,
+``e'_s`` being the slice exponent without the root's factor, and after the slices ``tout`` is brought
+to the mantissa's exponent ``E`` once.  ``e'_s`` is finite whenever the factors below the root are,
+so a slice whose amplitude is exactly zero keeps its tangent in any slice order.  A slice with a zero
+factor below its root adds nothing, a zero result (``E = -inf``) gives a zero tangent, and a NaN
+exponent gives NaN.
 """
 
 from __future__ import annotations
@@ -84,18 +105,23 @@ class JvpPlan(_DevicePlan):
     """Compile the JVP of ``contractions`` (the executed IR, stem fusion included) for fixed input
     shapes and dtype.  Same arguments as ``ExecPlan`` plus ``wrt``, the inputs that carry a tangent
     (default: all; positions among the plan's inputs).  ``precision``, ``accumulate`` and
-    ``absorb_root`` apply to the tangent nodes as to the values.  ``strip_exponent`` raises
-    ``NotImplementedError``: a stripped result has no tangent here.
+    ``absorb_root`` apply to the tangent nodes as to the values.  ``strip_exponent=True`` needs
+    ``stripped_grad=True``: the plan then forms the tangent of the mantissa with the exponent held
+    constant (see the module notes; ``absorb_root`` stays off) and ``execute`` takes an exponent
+    buffer.  Without ``stripped_grad`` it raises ``NotImplementedError``.
 
     ``_two_term=False`` runs every two-term node as two launches (for measuring the two forms)."""
 
     def __init__(self, contractions, inputs, output, size_dict, sliced=(), dtype="complex128", wrt=None,
                  strip_exponent=False, hoist=True, allow_dmma=True, sm_count=None, variant=None,
-                 precision="3xtf32", accumulate="native", absorb_root=False, input_ids=None, _two_term=True):
-        if strip_exponent:
-            raise NotImplementedError("forward-mode derivatives of strip_exponent results are not supported")
-        fwd = ExecPlan(contractions, inputs, output, size_dict, sliced, dtype=dtype, hoist=hoist,
-                       allow_dmma=allow_dmma, sm_count=sm_count, variant=variant, precision=precision,
+                 precision="3xtf32", accumulate="native", absorb_root=False, input_ids=None, stripped_grad=False,
+                 _two_term=True):
+        if strip_exponent and not stripped_grad:
+            raise NotImplementedError("forward-mode derivatives of strip_exponent results are only defined with "
+                                      "stripped_grad=True (the exponent held constant)")
+        self.strip_exponent = bool(strip_exponent)
+        fwd = ExecPlan(contractions, inputs, output, size_dict, sliced, dtype=dtype, strip_exponent=strip_exponent,
+                       hoist=hoist, allow_dmma=allow_dmma, sm_count=sm_count, variant=variant, precision=precision,
                        accumulate=accumulate, absorb_root=absorb_root, input_ids=input_ids)
         self.fwd = fwd
         for k in ("dtype", "esize", "sm_count", "precision", "acc_dtype", "wide", "inputs", "output", "sliced",
@@ -110,6 +136,7 @@ class JvpPlan(_DevicePlan):
 
     def _build(self, two_term):
         fwd = self.fwd
+        strip = self.strip_exponent
         tan = {}
         for nd in fwd.nodes:
             for t in (nd["a"], nd["b"], nd.get("d")):
@@ -122,6 +149,8 @@ class JvpPlan(_DevicePlan):
             rec = {k: nd[k] for k in ("kind", "a", "b", "c", "words", "phase", "root")}
             if nd.get("d") is not None:
                 rec["d"] = nd["d"]
+            if strip and nd["kind"] == 0:
+                rec["scale"] = (nd["a"], nd["b"])  # (the forward's own: its operands' factors)
             phases[nd["phase"]].append(rec)
             a, b, d, c = nd["a"], nd["b"], nd.get("d"), nd["c"]
             ta, tb, td = (tan.get(id(t)) if t is not None else None for t in (a, b, d))
@@ -151,6 +180,8 @@ class JvpPlan(_DevicePlan):
                 trec = dict(kind=nd["kind"], c=tc, words=words, phase=nd["phase"], root=2 if nd["root"] else 0,
                             fwd_index=i)
                 trec.update(t)  # (a two-term record sets kind 2)
+                if strip and nd["kind"] == 0:
+                    trec["scale"] = (a, b)  # the primal node's factors; a tangent records none
                 phases[nd["phase"]].append(trec)
                 self.tangent_nodes.append(trec)
         sched = phases[0] + [None] + phases[1]
@@ -158,6 +189,9 @@ class JvpPlan(_DevicePlan):
         self.tensors = _slots(sched)
         self.workspace_bytes, self.persistent_bytes, _ = layout(sched)
         self.differentiated = sorted({nd["fwd_index"] for nd in self.tangent_nodes})
+        if strip:
+            self._scale_slots()
+            self.tangent_marks = [int("fwd_index" in nd) for nd in self.nodes]
         self._marshal()
 
     def variants(self):
@@ -166,12 +200,18 @@ class JvpPlan(_DevicePlan):
 
     # ------------------------------------------------------------------ device side
     def execute(self, input_ptrs, tangent_ptrs, out_ptr, tangent_out_ptr, ws_ptr, ws_bytes, begin, step, count,
-                stream=0):
+                stream=0, exp_ptr=None):
         """``tangent_ptrs``: one device pointer per plan input, ``None`` outside ``wrt``; ``out_ptr``
-        may be ``None`` (the primal root is then not run)."""
+        may be ``None`` (the primal root is then not run).  A stripped plan needs ``out_ptr`` and
+        ``exp_ptr``, the device double of the running exponent (``ctgb_plan_execute_jvp_stripped``)."""
         lib = _lib.load()
         arr = (C.c_void_p * len(input_ptrs))(*input_ptrs)
         tans = (C.c_void_p * len(tangent_ptrs))(*tangent_ptrs)
+        if self.strip_exponent:
+            _lib.check(lib.ctgb_plan_execute_jvp_stripped(self.handle, arr, tans, out_ptr, tangent_out_ptr, exp_ptr,
+                                                          ws_ptr, ws_bytes, int(begin), int(step), int(count),
+                                                          stream))
+            return
         _lib.check(lib.ctgb_plan_execute_jvp(self.handle, arr, tans, out_ptr, tangent_out_ptr, ws_ptr, ws_bytes,
                                              int(begin), int(step), int(count), stream))
 

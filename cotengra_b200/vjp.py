@@ -373,11 +373,7 @@ class VjpPlan(_DevicePlan):
         self.workspace_bytes, self.persistent_bytes, self.cotangent_offset = sizes
         if self.strip_exponent:
             # factor slot of every operand a node divides by: a tensor slot, or the seed (n_tensors)
-            slot = {id(t): i for i, t in enumerate(self.tensors)}
-            seed = len(self.tensors)
-            scale = [nd.get("scale", ()) for nd in self.nodes]
-            self.scale_slots = tuple([-1 if len(s) <= k else seed if s[k] is None else slot[id(s[k])] for s in scale]
-                                     for k in (0, 1))
+            self._scale_slots()
         self._marshal()
 
     # ------------------------------------------------------------------ recomputation

@@ -89,7 +89,10 @@ int ctgb_contract_pair(const int64_t* desc, const void* A, const void* B,
  * A2 has A's index structure and strides and B2 has B's, so the same descriptor
  * describes both products and C is stored once (accumulated when the descriptor
  * says so).  Runs on the row-stream and DMMA stream kernels (variants 8, 19 and
- * 14) with unstripped descriptors; any other descriptor fails with CTGB_E_VALUE.
+ * 14).  A descriptor with both scale words (W_SCALE_A, W_SCALE_B: device doubles
+ * fA, fB) forms C (+)= (A.B + A2.B2) / (fA fB), a zero factor scaling by 0; one
+ * with a factor slot of C (W_FACTOR_C), one scale word alone, a wide C or any
+ * other variant fails with CTGB_E_VALUE before any launch.
  * The DMMA stream kernel's two-term form takes K <= 64 for N <= 16, K <= 32 for
  * N <= 32 and K <= 16 beyond. */
 int ctgb_contract_pair2(const int64_t* desc, const void* A, const void* B,
@@ -183,7 +186,9 @@ typedef struct {
 } ctgb_plan_desc;
 
 /* strip_exponent together with phase 2/3 nodes makes a stripped reverse-mode
- * plan, which runs only after ctgb_plan_set_scale_slots. */
+ * plan, which runs only after ctgb_plan_set_scale_slots; together with tangent
+ * slots (kinds 7, 8) a stripped forward-mode plan, which runs only after
+ * ctgb_plan_set_tangent_scale_slots. */
 int ctgb_plan_create(const ctgb_plan_desc* desc, ctgb_plan** plan);
 /* strip_exponent plans, and plans with a wide accumulator whose root is not a
  * dot-stream node: the single-operand descriptor (ctgb_single_desc_words()
@@ -203,6 +208,16 @@ int ctgb_plan_set_chunk_desc(ctgb_plan* plan, const int64_t* desc);
  * record nothing.  The gradient is that of m = amp * 10^-e with e held constant. */
 int ctgb_plan_set_scale_slots(ctgb_plan* plan, const int32_t* slot_a,
                               const int32_t* slot_b, int n);
+/* Stripped forward-mode plans, once before the first execute: tangent[i] = 1 marks
+ * the tangent records among the n (= n_nodes) nodes.  A primal record (0) is the
+ * forward plan's node and divides by its own operands' factors (slot_a[i], slot_b[i]
+ * = its a and b; -1, -1 for a single-operand node).  A pairwise or two-term tangent
+ * record divides by the two tensor slots named (its primal node's operands) and
+ * records no factor: T_p = (T_l S_r + S_l T_r) / (f_l f_r), the scale of the primal
+ * value S_p, so that tangents of intermediates are never normalised on their own. */
+int ctgb_plan_set_tangent_scale_slots(ctgb_plan* plan, const int32_t* slot_a,
+                                      const int32_t* slot_b,
+                                      const int32_t* tangent, int n);
 /* Forward plans, once after ctgb_plan_create: the dtype of the output accumulator,
  * the plan's dtype (the default) or its double counterpart (CTGB_F64 for CTGB_F32,
  * CTGB_C128 for CTGB_C64); anything else fails with CTGB_E_VALUE.  With the double
@@ -272,6 +287,24 @@ int ctgb_plan_execute_jvp(ctgb_plan* plan, const void* const* inputs,
                           size_t workspace_bytes, int64_t slice_begin,
                           int64_t slice_step, int64_t slice_count,
                           void* stream);
+/* Forward mode of a strip_exponent plan: `out` and exponent_dev[0] receive the
+ * stripped result (m, e) as ctgb_plan_execute does (neither may be null: the
+ * primal root always runs, its factor sets each slice's exponent), and
+ * `tangent_out` the tangent of the mantissa with the exponent held constant,
+ * dm = 10^-e d(amp); on entry `tangent_out` holds a tangent relative to
+ * exponent_dev[0] as `out` does (zeros with -inf).  The root's raw tangent is
+ * folded against a running exponent of its own, Et' = max(Et, e'_s):
+ * tout = tout 10^(Et - Et') + T_s 10^(e'_s - Et'), e'_s being the slice's
+ * exponent without the root's factor, and one launch after the slices brings
+ * tout to the final e.  So a slice whose amplitude is exactly zero keeps its
+ * tangent in any slice order.  A slice with a zero factor below its root adds
+ * nothing; a zero result (e = -inf) gives a zero tangent; a NaN exponent, NaN. */
+int ctgb_plan_execute_jvp_stripped(ctgb_plan* plan, const void* const* inputs,
+                                   const void* const* tangents, void* out,
+                                   void* tangent_out, double* exponent_dev,
+                                   void* workspace, size_t workspace_bytes,
+                                   int64_t slice_begin, int64_t slice_step,
+                                   int64_t slice_count, void* stream);
 
 /* Same job for a forward plan with HOST buffers: copies the inputs
  * host->device, runs the slices, copies the accumulated output (out_elements of the

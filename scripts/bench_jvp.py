@@ -6,6 +6,13 @@ limit.
 
     python scripts/bench_jvp.py [--configs peps8x8 m10s] [--dtypes complex64 complex128]
                                 [--slices 2 --steps 10 --warmup 3 --rounds 5]
+    python scripts/bench_jvp.py --strip [--m20-widths 26 30] ...
+
+``--strip`` times the stripped JVP (``strip_exponent=True, stripped_grad=True``) against the
+unstripped one instead, for one input and for every input, alternated round by round, and reports
+the launches per slice and the stripped two-term nodes of both plans; ``--m20-widths`` adds slice 0
+of the Sycamore-m20 tree at those widths in complex64 (a plan that does not fit the card is reported
+with its bytes and not run).
 
 Times are CUDA-event times per call, averaged over ``--steps`` calls after ``--warmup``; the two-form
 comparison takes the median of ``--rounds`` alternated rounds.  The trees run as ``TreeExecutor``
@@ -100,6 +107,76 @@ def run(config, dtype, args, card):
     print(json.dumps(line), flush=True)
 
 
+def run_strip(config, dtype, args, card, spec=None, arrays=None, desc=None):
+    import torch
+
+    import cotengra_b200 as cb
+
+    if spec is None:
+        spec, arrays, desc = bench.load_workload(config, dtype)
+    plain = cb.TreeExecutor(spec, dtype=dtype)
+    strip = cb.TreeExecutor(spec, dtype=dtype, strip_exponent=True, stripped_grad=True)
+    count = min(plain.nslices, args.slices)
+    n = len(arrays)
+    big = max(range(n), key=lambda i: arrays[i].size)
+    line = {"metric": f"{config}_jvp_strip", "config": config, "dtype": dtype, "workload": desc, "card": card,
+            "slices": count, "inputs": n, "one_input": big}
+    plans = {}
+    free = torch.cuda.mem_get_info()[0]
+    for name, ex in (("unstripped", plain), ("stripped", strip)):
+        for wrt, key in ((None, "all"), ([big], "one")):
+            p = ex.jvp_plan(wrt)
+            plans[name, key] = p
+            line[f"{name}_{key}_launches_per_slice"] = p.launches_per_slice()
+            line[f"{name}_{key}_two_term_nodes"] = p.two_term_nodes
+            line[f"{name}_{key}_workspace_bytes"] = p.total_bytes
+    need = max(p.total_bytes for p in plans.values()) + strip.plan.total_bytes
+    if need > 0.9 * free:
+        line["note"] = f"the JVP workspace ({need} bytes) does not fit the card ({free} bytes free): not run"
+        print(json.dumps(line), flush=True)
+        return
+    dev = [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in arrays]
+    tans = [torch.from_numpy(t).cuda() for t in make_arrays([a.shape for a in arrays], dtype, seed=1, scale=0.35)]
+
+    def timed(fn, steps=args.steps, warmup=args.warmup):
+        for _ in range(warmup):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(steps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / 1e3 / steps
+
+    calls = {
+        ("unstripped", "one"): lambda: plain.jvp(dev, [tans[big]], 0, 1, count, wrt=[big]),
+        ("stripped", "one"): lambda: strip.jvp(dev, [tans[big]], 0, 1, count, wrt=[big]),
+        ("unstripped", "all"): lambda: plain.jvp(dev, tans, 0, 1, count),
+        ("stripped", "all"): lambda: strip.jvp(dev, tans, 0, 1, count),
+    }
+    for f in calls.values():
+        timed(f, steps=1, warmup=args.warmup)
+    rounds = {k: [] for k in calls}
+    for _ in range(args.rounds):  # alternated: a drift in clocks hits both forms alike
+        for k, f in calls.items():
+            rounds[k].append(timed(f, warmup=1))
+    for (name, key), r in rounds.items():
+        line[f"{name}_{key}_s"] = statistics.median(r)
+        line[f"{name}_{key}_rounds_s"] = r
+    for key in ("one", "all"):
+        line[f"stripped_over_unstripped_{key}"] = line[f"stripped_{key}_s"] / line[f"unstripped_{key}_s"]
+    # the stripped tangent times 10^e against the unstripped one (complex128: ~1e-13)
+    (_m, e), dm = strip.jvp(dev, tans, 0, 1, count)
+    _o, want = plain.jvp(dev, tans, 0, 1, count)
+    got = dm.to(torch.complex128) * 10.0 ** float(e.item())
+    line["exponent"] = float(e.item())
+    line["stripped_vs_unstripped_rel_diff"] = float(torch.linalg.vector_norm(got - want.to(torch.complex128))
+                                                    / max(float(torch.linalg.vector_norm(want)), 1e-300))
+    print(json.dumps(line), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", nargs="+", default=["peps8x8", "m10s"], choices=sorted(bench.METRICS))
@@ -108,8 +185,22 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--strip", action="store_true", help="stripped against unstripped JVP")
+    ap.add_argument("--m20-widths", nargs="*", type=int, default=[], help="with --strip: m20 slice 0 at 2^W")
     args = ap.parse_args()
     card = card_name()
+    if args.strip:
+        from tests.slicing_util import appxB_at_width
+
+        for config in args.configs:
+            for dtype in args.dtypes:
+                run_strip(config, dtype, args, card)
+        for w in args.m20_widths:
+            spec = appxB_at_width(w)
+            arrays = make_arrays(spec.shapes(), "complex64", seed=0, scale=0.65)
+            run_strip(f"m20_w{w}", "complex64", argparse.Namespace(**{**vars(args), "slices": 1}), card, spec, arrays,
+                      f"Sycamore m20 slice 0 at W = 2^{w}")
+        return
     for config in args.configs:
         for dtype in args.dtypes:
             run(config, dtype, args, card)
