@@ -5,9 +5,9 @@ reference but no GPU.
 
 Everything above the C-ABI call is the product: argument handling, classification, lowering
 to descriptors, plan building (arenas, slice offsets, hoisting, stem fusion).  Only the last
-step -- ``ctgb_contract_pair`` / ``ctgb_reduce_single`` / ``ctgb_plan_execute`` of forward and
-reverse-mode plans -- is replaced by ``tests/desc_emulator.py``, which walks the very descriptors
-the kernels would receive.
+step -- ``ctgb_contract_pair`` / ``ctgb_reduce_single`` / ``ctgb_plan_execute*`` of forward,
+reverse- and forward-mode plans -- is replaced by ``tests/desc_emulator.py``, which walks the very
+descriptors the kernels would receive.
 Host tensors (torch CPU) stand in for device memory.  NOT a fallback: it lives under
 ``tests/``, is never imported by ``cotengra_b200`` and is installed by monkeypatching only.
 """
@@ -32,6 +32,26 @@ def _view(ptr, dtype, count=None):
     n = (1 << 40) if count is None else int(count) * dtype.itemsize
     raw = np.ctypeslib.as_array(C.cast(int(ptr), C.POINTER(C.c_uint8)), shape=(max(n, 1),))
     return raw[: n - n % dtype.itemsize].view(dtype) if count is None else raw[:n].view(dtype)
+
+
+def _arrays(plan, ptrs):
+    """numpy views of the buffers at ``ptrs``, one per plan input (``None`` stays ``None``), each in its
+    input's full shape and the plan dtype."""
+    sizes = getattr(plan, "fwd", plan).size_dict
+    shapes = [tuple(sizes[ix] for ix in term) for term in plan.inputs]
+    return [None if p is None else _view(p, plan.dtype, math.prod(s)).reshape(s) for p, s in zip(ptrs, shapes)]
+
+
+def _emulate(plan, ws_bytes, begin, step, count, arrays, **buffers):
+    """``emu.emulate_plan`` over the slice range ``begin, step, count`` of an execute call, with every
+    node it runs counted as one launch."""
+    if ws_bytes < plan.total_bytes:
+        raise MemoryError("workspace too small")
+    before = emu.node_runs
+    ids = range(int(begin), int(begin) + int(step) * int(count), int(step))
+    res = emu.emulate_plan(plan, arrays, slice_ids=ids, **buffers)
+    FakeLib.launches += emu.node_runs - before
+    return res
 
 
 class FakeLib:
@@ -133,7 +153,7 @@ def install(monkeypatch):
     ``monkeypatch`` fixture)."""
     import torch
 
-    from cotengra_b200 import _lib, contract, executor, vjp
+    from cotengra_b200 import _lib, contract, executor, jvp, vjp
 
     fake_torch = _FakeTorch()
     fake_lib = FakeLib()
@@ -157,52 +177,46 @@ def install(monkeypatch):
         return self
 
     def execute(self, input_ptrs, out_ptr, exp_ptr, ws_ptr, ws_bytes, begin, step, count, stream=0):
-        dt = np.dtype(self.dtype)
-        arrays = []
-        for ptr, term in zip(input_ptrs, self.inputs):
-            shape = tuple(self.size_dict[ix] for ix in term)
-            arrays.append(_view(ptr, dt, math.prod(shape)).reshape(shape))
-        ids = range(int(begin), int(begin) + int(step) * int(count), int(step))
-        res = emu.emulate_plan(self, arrays, slice_ids=ids)
-        out = _view(out_ptr, dt, max(self.out_elements, 1))[: self.out_elements]
-        FakeLib.launches += len(self.nodes)
-        if self.strip_exponent:
-            m, e = res
-            # fresh accumulators only (what the drop-in tests use)
-            assert not np.any(out), "emulated execute: accumulating into a stripped partial sum"
-            out[:] = np.asarray(m).reshape(-1)
-            _view(exp_ptr, np.float64, 1)[0] = e
-        else:
-            out += np.asarray(res).reshape(-1)
+        out = _view(out_ptr, self.acc_dtype, max(self.out_elements, 1))
+        if not self.strip_exponent:
+            _emulate(self, ws_bytes, begin, step, count, _arrays(self, input_ptrs), out=out)
+            return
+        exp = _view(exp_ptr, np.float64, 1)
+        _m, exp[0] = _emulate(self, ws_bytes, begin, step, count, _arrays(self, input_ptrs), out=out,
+                              exponent=exp[0])
 
     def execute_host(self, host_arrays, host_out, ws_ptr, ws_bytes, begin, step, count, stream=0):
-        ids = range(int(begin), int(begin) + int(step) * int(count), int(step))
-        res = emu.emulate_plan(self, list(host_arrays), slice_ids=ids)
+        res = _emulate(self, ws_bytes, begin, step, count, list(host_arrays))
         if self.strip_exponent:
             host_out[...] = np.asarray(res[0]).reshape(host_out.shape)
             return float(res[1])
         host_out[...] = np.asarray(res).reshape(host_out.shape)
         return 0.0
 
-    def execute_vjp(self, input_ptrs, cot_ptr, grad_ptrs, ws_ptr, ws_bytes, begin, step, count, stream=0):
-        if ws_bytes < self.total_bytes:
-            raise MemoryError("workspace too small")
-        dt = np.dtype(self.dtype)
-        arrays, grads = [], []
-        for i, (ptr, term) in enumerate(zip(input_ptrs, self.inputs)):
-            shape = tuple(self.fwd.size_dict[ix] for ix in term)
-            arrays.append(_view(ptr, dt, math.prod(shape)).reshape(shape))
-            gp = grad_ptrs[i]
-            grads.append(None if gp is None else _view(gp, dt, math.prod(shape)))
-        cot = _view(cot_ptr, dt, max(self.out_elements, 1))[: self.out_elements]
-        ids = range(int(begin), int(begin) + int(step) * int(count), int(step))
-        emu.emulate_plan(self, arrays, cot.copy(), slice_ids=ids, grads=grads)
-        # phases 0 and 3 run once, phases 1 and 2 once per slice
-        FakeLib.launches += sum(1 if nd["phase"] in (0, 3) else len(ids) for nd in self.nodes)
+    def execute_vjp(self, input_ptrs, cot_ptr, grad_ptrs, ws_ptr, ws_bytes, begin, step, count, stream=0,
+                    exp_ptr=None):
+        cot = _view(cot_ptr, self.dtype, max(self.out_elements, 1))[: self.out_elements]
+        exponent = None if exp_ptr is None else _view(exp_ptr, np.float64, 1)[0]
+        _emulate(self, ws_bytes, begin, step, count, _arrays(self, input_ptrs), cotangent=cot,
+                 grads=_arrays(self, grad_ptrs), exponent=exponent)
+
+    def execute_jvp(self, input_ptrs, tangent_ptrs, out_ptr, tangent_out_ptr, ws_ptr, ws_bytes, begin, step,
+                    count, stream=0, exp_ptr=None):
+        n = max(self.out_elements, 1)
+        out = None if out_ptr is None else _view(out_ptr, self.acc_dtype, n)
+        kw = dict(tangents=[t for i, t in enumerate(_arrays(self, tangent_ptrs)) if i in self.wrt],
+                  primal=out_ptr is not None, out=out, tout=_view(tangent_out_ptr, self.acc_dtype, n))
+        if not self.strip_exponent:
+            _emulate(self, ws_bytes, begin, step, count, _arrays(self, input_ptrs), **kw)
+            return
+        exp = _view(exp_ptr, np.float64, 1)
+        _m, exp[0], _t = _emulate(self, ws_bytes, begin, step, count, _arrays(self, input_ptrs), exponent=exp[0],
+                                  **kw)
 
     monkeypatch.setattr(executor._DevicePlan, "create", create)
     monkeypatch.setattr(executor._DevicePlan, "destroy", lambda self: None)
     monkeypatch.setattr(executor.ExecPlan, "execute", execute)
     monkeypatch.setattr(executor.ExecPlan, "execute_host", execute_host)
     monkeypatch.setattr(vjp.VjpPlan, "execute", execute_vjp)
+    monkeypatch.setattr(jvp.JvpPlan, "execute", execute_jvp)
     return fake_lib

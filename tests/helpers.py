@@ -69,3 +69,18 @@ def rel_err(x, ref):
     if den == 0:
         return float(np.max(np.abs(x))) if x.size else 0.0
     return float(np.max(np.abs(x - ref)) / den)
+
+
+def jvp_oracle(spec, contractions, arrays, tangents, wrt, slice_ids=None):
+    """The exact JVP of a multilinear tree: ``sum_{i in wrt} f(x_1, ..., v_i, ..., x_n)`` through the
+    torch-CPU oracle (``oracle/grad_oracle.py``), in the arrays' dtype."""
+    import torch
+
+    from oracle import grad_oracle as go
+
+    total = 0
+    for i, t in zip(wrt, tangents):
+        xs = [torch.tensor(t if j == i else a) for j, a in enumerate(arrays)]
+        total = total + go.contract_tree(spec.inputs, spec.output, spec.sliced, contractions, xs,
+                                         slice_ids=slice_ids).detach().numpy()
+    return np.asarray(total)

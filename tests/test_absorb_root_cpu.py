@@ -12,7 +12,7 @@ import pytest
 import cotengra_b200 as cb
 from cotengra_b200 import lowering as L
 from cotengra_b200.fusion import fuse_stems
-from tests.emu_absorb import emulate_absorb, emulate_plan
+from tests.desc_emulator import emulate_absorb, emulate_plan
 from tests.helpers import decode_sliced, load_json
 
 

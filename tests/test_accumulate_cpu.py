@@ -12,8 +12,8 @@ import pytest
 import cotengra_b200 as cb
 from cotengra_b200 import _lib, executor as X, lowering as L
 from oracle import ctg_oracle as orc
-from tests import emu_accumulate
-from tests.emu_accumulate import emulate_plan
+from tests import emu_device
+from tests.desc_emulator import emulate_plan
 from tests.helpers import GOLDEN_DIR, decode_ir, decode_sliced, load_json, make_arrays, rel_err, tree_spec
 
 TREES = load_json("trees.json")
@@ -168,7 +168,7 @@ def test_emulated_wide_plans_match_the_oracle(name, dtype):
     plan = _plan(spec, dtype, accumulate="double")
     got = emulate_plan(plan, arrays)
     assert got.dtype == np.dtype(WIDE[dtype]) and got.shape == want.shape
-    # (the emulation holds every value of a wide plan in the accumulator dtype: tests/emu_accumulate.py)
+    # (the emulation holds every value of a wide plan in the accumulator dtype: tests/desc_emulator.py)
     assert rel_err(got, want) < 1e-10
     # zero slices: the zeroed wide output
     none = emulate_plan(plan, arrays, slice_ids=[])
@@ -209,7 +209,7 @@ def _tag(spec, dtype, strip, arrays, extra=b""):
 
 
 def test_checkpoint_tag_and_entry_points(monkeypatch, tmp_path):
-    emu_accumulate.install(monkeypatch)
+    emu_device.install(monkeypatch)
     rec = _rec("lattice6x6_d3_sliced")
     spec = tree_spec(rec)
     arrays = make_arrays(spec.shapes(), "complex64", seed=rec["seed"])

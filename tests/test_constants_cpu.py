@@ -16,7 +16,7 @@ import torch
 import cotengra_b200 as cb
 from cotengra_b200 import ExecPlan
 from cotengra_b200.constants import plan_folds
-from tests import emu_device, emu_strip
+from tests import emu_device
 from tests.helpers import load_json, load_npz, make_arrays, rel_err, tree_spec
 
 TREES = load_json("trees.json")
@@ -28,7 +28,7 @@ GRAD_TREES = [r for r in TREES if r["sliced"] or r["name"].startswith(("pre_", "
 
 @pytest.fixture
 def emu(monkeypatch):
-    emu_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     yield
     gc.collect()  # (autograd graphs hold executors: free them while the emulator is installed)
 

@@ -1,5 +1,5 @@
 """Forward mode on the device: the two-term stream kernels through ``ctgb_contract_pair2`` in
-guarded buffers, ``TreeExecutor.jvp`` against the exact multilinear oracle (``tests/emu_jvp.py``),
+guarded buffers, ``TreeExecutor.jvp`` against the exact multilinear oracle (``tests/helpers.py``),
 the dot-product identity with reverse mode, and ``torch.autograd.forward_ad`` through every entry
 point that records the autograd node."""
 
@@ -18,7 +18,7 @@ import torch.autograd.forward_ad as fwAD  # noqa: E402
 import cotengra_b200 as cb  # noqa: E402
 from cotengra_b200 import _lib  # noqa: E402
 from cotengra_b200 import lowering as L  # noqa: E402
-from tests.emu_jvp import jvp_oracle  # noqa: E402
+from tests.helpers import jvp_oracle  # noqa: E402
 from tests.helpers import GOLDEN_DIR, load_json, make_arrays, tree_spec  # noqa: E402
 
 TREES = load_json("trees.json")

@@ -1,5 +1,5 @@
 """Forward mode (``cotengra_b200/jvp.py``) on the CPU: the JVP plans' records walked by the emulator
-(``tests/emu_jvp.py``) against the exact multilinear oracle ``J v = sum_i f(x_1, ..., v_i, ..., x_n)``,
+(``tests/desc_emulator.py``) against the exact multilinear oracle ``J v = sum_i f(x_1, ..., v_i, ..., x_n)``,
 and the plans' structure."""
 
 import numpy as np
@@ -9,8 +9,8 @@ from cotengra_b200 import ExecPlan, VjpPlan
 from cotengra_b200.executor import K_TANGENT, K_TOUT, PHASE_INV_FWD
 from cotengra_b200.fusion import fuse_stems
 from cotengra_b200.jvp import JvpPlan, two_term_fits
-from tests.emu_jvp import emulate_jvp, jvp_oracle
-from tests.helpers import load_json, make_arrays, tree_spec
+from tests.desc_emulator import emulate_plan
+from tests.helpers import jvp_oracle, load_json, make_arrays, tree_spec
 
 TREES = load_json("trees.json")
 DT = "complex128"
@@ -49,21 +49,21 @@ def test_jvp_matches_multilinear_oracle(rec):
         want_out = jvp_oracle(spec, ir, arrays, [arrays[wrt[0]]], [wrt[0]])  # f(x) itself
         for contractions in (None, fused.contractions()):
             plan = _plan(spec, contractions, wrt=wrt)
-            out, tout = emulate_jvp(plan, arrays, tans)
+            out, tout = emulate_plan(plan, arrays, tangents=tans)
             assert _nrel(tout, want) <= 1e-12, (wrt, _nrel(tout, want))
             assert _nrel(out, want_out) <= 1e-12
             # without the primal the root is skipped and the tangent is the same
-            assert _nrel(emulate_jvp(plan, arrays, tans, primal=False), want) <= 1e-12
+            assert _nrel(emulate_plan(plan, arrays, tangents=tans, primal=False), want) <= 1e-12
     plan = _plan(spec, hoist=False)
     tans = make_arrays(spec.shapes(), DT, seed=rec["seed"] + 7)
-    assert _nrel(emulate_jvp(plan, arrays, tans, primal=False), jvp_oracle(spec, ir, arrays, tans, range(n))) <= 1e-12
+    assert _nrel(emulate_plan(plan, arrays, tangents=tans, primal=False), jvp_oracle(spec, ir, arrays, tans, range(n))) <= 1e-12
     if plan.nslices > 1:
         # slice ranges add up to the whole
         h = plan.nslices // 2
-        t1 = emulate_jvp(plan, arrays, tans, slice_ids=range(h), primal=False)
-        t2 = emulate_jvp(plan, arrays, tans, slice_ids=range(h, plan.nslices), primal=False)
+        t1 = emulate_plan(plan, arrays, tangents=tans, slice_ids=range(h), primal=False)
+        t2 = emulate_plan(plan, arrays, tangents=tans, slice_ids=range(h, plan.nslices), primal=False)
         assert _nrel(t1, jvp_oracle(spec, ir, arrays, tans, range(n), slice_ids=range(h))) <= 1e-12
-        assert _nrel(t1 + t2, emulate_jvp(plan, arrays, tans, primal=False)) <= 1e-12
+        assert _nrel(t1 + t2, emulate_plan(plan, arrays, tangents=tans, primal=False)) <= 1e-12
 
 
 def _below(plan):

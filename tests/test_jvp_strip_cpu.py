@@ -1,6 +1,6 @@
 """Forward-mode derivatives of strip_exponent results (``JvpPlan(strip_exponent=True,
 stripped_grad=True)``) on the CPU: the stripped JVP plans' records, factor slots and running exponent
-walked by the lazy-scheme model (``tests/emu_jvp_strip.py``) against the exact multilinear oracle with
+walked by the plan emulator (``tests/desc_emulator.py``) against the exact multilinear oracle with
 ``dm = 10^-e d(amp)``; zero slices and results; central differences of ``log|m| + e ln 10``; forward AD
 through the public interface with the device launch emulated; two gloo ranks; and the plans that must
 not change, against digests of the parent's descriptors (``tests/golden/plan_digests.json``)."""
@@ -23,11 +23,9 @@ from cotengra_b200 import ExecPlan, VjpPlan
 from cotengra_b200.fusion import fuse_stems
 from cotengra_b200.jvp import JvpPlan
 from oracle import ctg_oracle as orc
-from tests import emu_jvp_strip
+from tests import emu_device
 from tests.desc_emulator import emulate_plan
-from tests.emu_jvp import jvp_oracle
-from tests.emu_jvp_strip import emulate_stripped_jvp
-from tests.helpers import GOLDEN_DIR, load_json, make_arrays, tree_spec
+from tests.helpers import GOLDEN_DIR, jvp_oracle, load_json, make_arrays, tree_spec
 from tests.test_vjp_cpu import ctg  # noqa: F401  (the drop-in fixture)
 from tests.zero_util import zero_one_digit
 
@@ -161,7 +159,7 @@ def test_stripped_tangent_matches_oracle(rec):
         want = jvp_oracle(spec, ir, arrays, tans, wrt)
         for contractions, opts in ((None, {}), (None, {"hoist": False}), (fused.contractions(), {})):
             m0, e0 = _forward(spec, arrays, contractions, **opts)
-            m, e, dm = emulate_stripped_jvp(_plan(spec, contractions, wrt=wrt, **opts), arrays, tans)
+            m, e, dm = emulate_plan(_plan(spec, contractions, wrt=wrt, **opts), arrays, tangents=tans)
             assert abs(e - e0) <= 1e-12 and nrel(m, m0) <= 1e-12
             assert nrel(dm * 10.0 ** e, want) <= 1e-11, (wrt, opts, nrel(dm * 10.0 ** e, want))
     plan = _plan(spec)
@@ -169,14 +167,14 @@ def test_stripped_tangent_matches_oracle(rec):
     if plan.nslices > 1:
         h = plan.nslices // 2
         ids = range(h, plan.nslices)
-        m, e, dm = emulate_stripped_jvp(plan, arrays, tans, slice_ids=ids)
+        m, e, dm = emulate_plan(plan, arrays, tangents=tans, slice_ids=ids)
         assert abs(e - _forward(spec, arrays, slice_ids=ids)[1]) <= 1e-12
         assert nrel(dm * 10.0 ** e, jvp_oracle(spec, ir, arrays, tans, range(n), slice_ids=ids)) <= 1e-11
 
 
 def test_constants(monkeypatch):
     """folded constants: the exponent of the folds is added to e and leaves dm as it is"""
-    emu_jvp_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     rec = BY_NAME["lattice6x6_d3_sliced"]
     spec = tree_spec(rec)
     dt = rec["dtype"]
@@ -209,17 +207,17 @@ def test_zero_slices_and_results(name):
     # the tangent of the zeroed input too: the zero slices stay zero along it
     tans, _ = zero_one_digit(spec, make_arrays(spec.shapes(), DT, seed=3), which=0, digit=1)
     plan = _plan(spec)
-    m, e, dm = emulate_stripped_jvp(plan, arrays, tans)
+    m, e, dm = emulate_plan(plan, arrays, tangents=tans)
     assert math.isfinite(e) and not np.isnan(dm).any()
     want = jvp_oracle(spec, spec.contractions(), arrays, tans, range(len(arrays)), slice_ids=live)
     assert nrel(dm * 10.0 ** e, want) <= 1e-11
     zero = [np.zeros_like(a) for a in arrays]
-    mz, ez, dmz = emulate_stripped_jvp(plan, zero, tans)
+    mz, ez, dmz = emulate_plan(plan, zero, tangents=tans)
     assert ez == -math.inf and np.all(dmz == 0) and np.all(mz == 0)
     # a NaN in the inputs: NaN exponent, NaN tangent
     bad = [a.copy() for a in arrays]
     bad[1].reshape(-1)[0] = np.nan
-    _mn, en, dmn = emulate_stripped_jvp(plan, bad, tans)
+    _mn, en, dmn = emulate_plan(plan, bad, tangents=tans)
     assert math.isnan(en) and np.isnan(dmn).all()
 
 
@@ -231,7 +229,7 @@ def test_central_differences_of_log_amplitude(name):
     arrays = make_arrays(spec.shapes(), "float64", seed=rec["seed"], scale=5.0)
     tans = make_arrays(spec.shapes(), "float64", seed=rec["seed"] + 1)
     plan = _plan(spec, dtype="float64")
-    m, e, dm = emulate_stripped_jvp(plan, arrays, tans)
+    m, e, dm = emulate_plan(plan, arrays, tangents=tans)
     m0, dm0 = np.asarray(m).reshape(-1)[0], np.asarray(dm).reshape(-1)[0]
     got = float(np.real(np.conj(m0) * dm0) / abs(m0) ** 2)
 
@@ -257,7 +255,7 @@ def test_forward_ad_through_public_entry_points(monkeypatch):
 
     from oracle import grad_oracle as go
 
-    emu_jvp_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     rec = BY_NAME["rand_r3_o1_hi1_ho1_None_s42_sliced_out"]
     spec = tree_spec(rec)
     dt = rec["dtype"]
@@ -313,7 +311,7 @@ def test_installed_tree_contract_forward_ad(ctg, monkeypatch):  # noqa: F811
     combiner propagates the slices' tangents through torch ops"""
     from torch.autograd import forward_ad
 
-    emu_jvp_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     con = ctg.utils.lattice_equation([3, 3], d_min=2, d_max=3, seed=1)
     tree = ctg.array_contract_tree(con.inputs, con.output, con.size_dict, optimize="greedy")
     tree.slice_(target_slices=4)
@@ -347,7 +345,7 @@ def _rank_tangent(rec, ids):
     spec = tree_spec(rec)
     arrays = make_arrays(spec.shapes(), DT, seed=rec["seed"], scale=3.0)
     tans = make_arrays(spec.shapes(), DT, seed=rec["seed"] + 1)
-    _m, e, dm = emulate_stripped_jvp(_plan(spec), arrays, tans, slice_ids=ids)
+    _m, e, dm = emulate_plan(_plan(spec), arrays, tangents=tans, slice_ids=ids)
     return np.array(dm), e
 
 
@@ -420,11 +418,11 @@ def test_zero_amplitude_slice_keeps_its_tangent(zero_slice):
     zero_only = jvp_oracle(spec, spec.contractions(), arrays, tans, range(3), slice_ids=[zero_slice])
     assert np.linalg.norm(zero_only) > 0.1 * np.linalg.norm(want)  # (the slice's tangent matters)
     for ids in ([0, 1], [1, 0]):
-        m, e, dm = emulate_stripped_jvp(plan, arrays, tans, slice_ids=ids)
+        m, e, dm = emulate_plan(plan, arrays, tangents=tans, slice_ids=ids)
         assert math.isfinite(e)
         assert nrel(dm * 10.0 ** e, want) <= 1e-13, (ids, nrel(dm * 10.0 ** e, want))
     # one call per slice, combined as reduce_partials does: additive over slices
-    parts = [emulate_stripped_jvp(plan, arrays, tans, slice_ids=[s]) for s in (0, 1)]
+    parts = [emulate_plan(plan, arrays, tangents=tans, slice_ids=[s]) for s in (0, 1)]
     emax = max(p[1] for p in parts)
     tot = sum(p[2] * (0.0 if p[1] == -math.inf else 10.0 ** (p[1] - emax)) for p in parts)
     # (the zero slice's own call has e = -inf: alone it is a zero result, with a zero tangent)
@@ -433,6 +431,6 @@ def test_zero_amplitude_slice_keeps_its_tangent(zero_slice):
     # the zero slice alone, with the exponent of the other slice given as the running exponent it
     # continues from: its tangent is kept
     other = parts[1 - zero_slice]
-    m2, e2, dm2 = emulate_stripped_jvp(plan, arrays, tans, slice_ids=[zero_slice], out=np.array(other[0]).reshape(-1),
+    m2, e2, dm2 = emulate_plan(plan, arrays, tangents=tans, slice_ids=[zero_slice], out=np.array(other[0]).reshape(-1),
                                        tout=np.array(other[2]).reshape(-1), exponent=other[1])
     assert nrel(dm2 * 10.0 ** e2, want) <= 1e-13

@@ -71,7 +71,7 @@ def _same_plan(a, b):
 
 def _check_budgets(ir, spec, dt, arrays, cot, want, **kw):
     base = _plan(ir, spec, dt, **kw)
-    ref = emulate_plan(base, arrays, cot)
+    ref = emulate_plan(base, arrays, cotangent=cot)
     lo = min_bytes(ir, spec, dt, **kw)
     fwd_words = [np.asarray(nd["words"]) for nd in base.fwd.nodes]
     for budget in sorted({lo, (lo + base.total_bytes) // 2, base.total_bytes}):
@@ -84,7 +84,7 @@ def _check_budgets(ir, spec, dt, arrays, cot, want, **kw):
         for nd in recomputed(plan):
             assert nd["phase"] == PHASE_VAR_BWD
             assert any(np.array_equal(nd["words"], w) for w in fwd_words)
-        got = emulate_plan(plan, arrays, cot)
+        got = emulate_plan(plan, arrays, cotangent=cot)
         for g, r, w in zip(got, ref, want):
             assert np.array_equal(g, r)  # the same descriptors on the same operands
             d = np.linalg.norm(w)
@@ -150,8 +150,8 @@ def test_sycamore_stems_at_small_width(width):
     assert wide == {0, 1} == sides
     arrays = make_arrays(spec.shapes(), dt, seed=3, scale=0.65)
     cot = np.ones(base.out_shape, dt)
-    ref = emulate_plan(base, arrays, cot, slice_ids=[0])
-    got = emulate_plan(plan, arrays, cot, slice_ids=[0])
+    ref = emulate_plan(base, arrays, cotangent=cot, slice_ids=[0])
+    got = emulate_plan(plan, arrays, cotangent=cot, slice_ids=[0])
     for g, r in zip(got, ref):
         assert np.array_equal(g, r)
 

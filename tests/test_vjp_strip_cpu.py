@@ -1,6 +1,6 @@
 """Gradients of strip_exponent results (``VjpPlan(strip_exponent=True, stripped_grad=True)``) on the
-CPU: the stripped VJP plans' descriptors, factor slots and seeds walked by the lazy-scheme model
-(``tests/emu_strip.py``) against the torch-CPU gradient oracle (``oracle/grad_oracle.py``) with
+CPU: the stripped VJP plans' descriptors, factor slots and seeds walked by the plan emulator
+(``tests/desc_emulator.py``) against the torch-CPU gradient oracle (``oracle/grad_oracle.py``) with
 ``dm/dx = 10^-e damp/dx``; central differences of ``log|m| + e ln 10``; the autograd paths of the
 public interface with the device launch emulated; and the default path, which is unchanged."""
 
@@ -18,9 +18,8 @@ from cotengra_b200.executor import PHASE_INV_FWD, PHASE_VAR_FWD
 from cotengra_b200.fusion import fuse_stems
 from oracle import ctg_oracle as orc
 from oracle import grad_oracle as go
-from tests import emu_strip
+from tests import emu_device
 from tests.desc_emulator import emulate_plan
-from tests.emu_strip import emulate_stripped_vjp
 from tests.helpers import load_json, make_arrays, tree_spec
 from tests.test_vjp_cpu import ctg  # noqa: F401  (the drop-in fixture)
 from tests.zero_util import zero_one_digit
@@ -88,13 +87,13 @@ def test_stripped_gradients_match_oracle(name):
     cot = make_arrays([np.shape(m)], dt, seed=rec["seed"] + 1)[0]
     want = _want(spec, arrays, cot, e)
     plan = _plan(ir, spec, dt)
-    _check(emulate_stripped_vjp(plan, arrays, cot, e), want)
-    _check(emulate_stripped_vjp(_plan(ir, spec, dt, hoist=False), arrays, cot, e), want)
+    _check(emulate_plan(plan, arrays, cotangent=cot, exponent=e), want)
+    _check(emulate_plan(_plan(ir, spec, dt, hoist=False), arrays, cotangent=cot, exponent=e), want)
     fused, _info = fuse_stems(spec, dt, min_big=2, ratio=1.0, min_gain=-1.0, model=_bytes_only)
     fir = fused.contractions()
-    _check(emulate_stripped_vjp(_plan(fir, spec, dt), arrays, cot, e), want)
+    _check(emulate_plan(_plan(fir, spec, dt), arrays, cotangent=cot, exponent=e), want)
     # the exponent is a parameter: another e scales the gradient by 10^(e - e2)
-    got = emulate_stripped_vjp(plan, arrays, cot, e + 3.5)
+    got = emulate_plan(plan, arrays, cotangent=cot, exponent=e + 3.5)
     _check(got, [w * 10.0 ** -3.5 for w in want])
 
 
@@ -110,7 +109,7 @@ def test_single_operand_root_is_seeded():
     assert e == 0.0
     cot = make_arrays([np.shape(m)], rec["dtype"], seed=3)[0]
     for ex in (e, 12.25):
-        _check(emulate_stripped_vjp(plan, arrays, cot, ex), _want(spec, arrays, cot, ex))
+        _check(emulate_plan(plan, arrays, cotangent=cot, exponent=ex), _want(spec, arrays, cot, ex))
 
 
 def test_scale_slots():
@@ -163,8 +162,8 @@ def test_budgeted_plan_recomputes_with_phase1_factors(name):
     m, e = _forward(ir, spec, dt, arrays)
     cot = make_arrays([np.shape(m)], dt, seed=5)[0]
     want = _want(spec, arrays, cot, e)
-    _check(emulate_stripped_vjp(plan, arrays, cot, e), want)
-    _check(emulate_stripped_vjp(base, arrays, cot, e), want)
+    _check(emulate_plan(plan, arrays, cotangent=cot, exponent=e), want)
+    _check(emulate_plan(base, arrays, cotangent=cot, exponent=e), want)
 
 
 @pytest.mark.parametrize("name", ["lattice4x4_sliced", "rand_r3_o1_hi1_ho1_None_s42_sliced_out"])
@@ -180,17 +179,17 @@ def test_zero_slices_contribute_nothing(monkeypatch, name):
     m, e = _forward(ir, spec, dt, arrays)
     cot = make_arrays([np.shape(m)], dt, seed=8)[0]
     plan = _plan(ir, spec, dt)
-    _check(emulate_stripped_vjp(plan, arrays, cot, e), _want(spec, arrays, cot, e, slice_ids=live))
+    _check(emulate_plan(plan, arrays, cotangent=cot, exponent=e), _want(spec, arrays, cot, e, slice_ids=live))
     # all zero: e = -inf, every seed 0
     zero = [np.zeros_like(a) if k == 0 else a for k, a in enumerate(arrays)]
     mz, ez = _forward(ir, spec, dt, zero)
     assert ez == -math.inf
-    for g in emulate_stripped_vjp(plan, zero, cot, ez):
+    for g in emulate_plan(plan, zero, cotangent=cot, exponent=ez):
         assert np.all(g == 0)
     # a NaN exponent gives NaN gradients
-    assert all(np.isnan(g).all() for g in emulate_stripped_vjp(plan, arrays, cot, math.nan))
+    assert all(np.isnan(g).all() for g in emulate_plan(plan, arrays, cotangent=cot, exponent=math.nan))
     # the public paths: check_zero returns (0.0, -inf) without a graph; without it, zero gradients
-    emu_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     ex = cb.TreeExecutor(spec, dtype=dt, strip_exponent=True, stripped_grad=True)
     ts = [torch.tensor(a, requires_grad=True) for a in zero]
     assert cb.contract_tree(ex, ts, check_zero=True) == (0.0, -math.inf)
@@ -209,7 +208,7 @@ def test_zero_slices_contribute_nothing(monkeypatch, name):
 def test_central_differences_of_log_amplitude(monkeypatch, name):
     """d(log|m| + e ln 10)/dx through contract_tree's autograd node against central differences of
     log|amp| (the exponent is a float; its split from m does not change the loss)."""
-    emu_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     rec = TREES[name]
     spec = tree_spec(rec)
     arrays = make_arrays(spec.shapes(), "float64", seed=rec["seed"], scale=5.0)
@@ -241,7 +240,7 @@ def test_central_differences_of_log_amplitude(monkeypatch, name):
 def test_public_interface(monkeypatch):
     """TreeExecutor.vjp(exponent=), contract_tree and B200Contractor record the mantissa's gradient;
     e is the same float as without stripped_grad"""
-    emu_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     rec, spec, arrays = _case("rand_r3_o1_hi1_ho1_None_s42_sliced_out", scale=9.0)
     dt = rec["dtype"]
     ex = cb.TreeExecutor(spec, dtype=dt, strip_exponent=True, stripped_grad=True)
@@ -281,7 +280,7 @@ def test_public_interface(monkeypatch):
 
 def test_default_path_unchanged(monkeypatch):
     """without stripped_grad: the warning, no graph, and NotImplementedError from the plan"""
-    emu_strip.install(monkeypatch)
+    emu_device.install(monkeypatch)
     rec, spec, arrays = _case("lattice4x4_sliced")
     ex = cb.TreeExecutor(spec, dtype=rec["dtype"], strip_exponent=True)
     with pytest.warns(UserWarning, match="no gradient") as warned:
@@ -314,7 +313,7 @@ def test_installed_tree_contract_stripped_backward(ctg, monkeypatch):  # noqa: F
     """``cb.install(tree, strip_exponent=True, stripped_grad=True)``; cotengra's own
     ``tree.contract(..., strip_exponent=True)`` on torch tensors combines the slices' (m_s, e_s);
     ``backward()`` through that combiner gives 10^-e damp/dx."""
-    emu_strip.install(monkeypatch)  # (the fixture's emulated launch, with stripped VJP plans)
+    emu_device.install(monkeypatch)  # (the fixture's emulated launch, with stripped VJP plans)
     con = ctg.utils.lattice_equation([3, 3], d_min=2, d_max=3, seed=1)
     tree = ctg.array_contract_tree(con.inputs, con.output, con.size_dict, optimize="greedy")
     tree.slice_(target_slices=4)
